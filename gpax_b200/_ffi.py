@@ -4,6 +4,7 @@ C-ABI; everything numerical happens behind it on the GPU.  There is no CPU fallb
 library or a CUDA device is missing, importing works (so CPU-only hosts can run the host-logic
 tests) but the first call raises `B200GPError`.
 """
+import contextlib
 import ctypes as C
 import os
 import threading
@@ -48,6 +49,7 @@ SIGNATURES = {
     "b2gp_ctx_destroy": (C.c_int, [_vp]),
     "b2gp_last_error": (C.c_char_p, [_vp]),
     "b2gp_set_option": (C.c_int, [_vp, C.c_char_p, C.c_int64]),
+    "b2gp_get_option": (C.c_int, [_vp, C.c_char_p, C.POINTER(C.c_int64)]),
     "b2gp_device_info": (C.c_int, [_vp, _ip, _ip, _ip, C.POINTER(C.c_size_t)]),
     "b2gp_last_timing": (C.c_int, [_vp, C.POINTER(Timing)]),
     "b2gp_dev_alloc": (C.c_int, [_vp, C.c_size_t, C.POINTER(_vp)]),
@@ -211,6 +213,42 @@ class Context:
 
     def set_option(self, key, value):
         self._check(self.lib.b2gp_set_option(self.h, key.encode(), int(value)))
+
+    def get_option(self, key):
+        v = C.c_int64()
+        self._check(self.lib.b2gp_get_option(self.h, key.encode(), C.byref(v)))
+        return v.value
+
+    @contextlib.contextmanager
+    def options(self, **kw):
+        """set the given options for the duration of a `with` block, then restore the values they had before"""
+        old = {k: self.get_option(k) for k in kw}
+        try:
+            for k, v in kw.items():
+                self.set_option(k, v)
+            yield self
+        finally:
+            for k, v in old.items():
+                self.set_option(k, v)
+
+    # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
+    PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall")
+
+    def path_counts(self):
+        """development aid: how often each kernel was launched / each solver route entered on this context so far"""
+        fn = self.lib.b2gp_debug_path_counts
+        fn.restype, fn.argtypes = C.c_int, [_vp, C.POINTER(C.c_int64), C.c_int]
+        out = (C.c_int64 * len(self.PATHS))()
+        n = fn(self.h, out, len(self.PATHS))
+        if n != len(self.PATHS):
+            raise B200GPError(f"b2gp_debug_path_counts reports {n} counters, the binding knows {len(self.PATHS)}")
+        return dict(zip(self.PATHS, out))
+
+    def cache_hits(self):
+        """development aid: posterior calls on this context that reused the cached factor (b2gp_debug_cache_hits)"""
+        fn = self.lib.b2gp_debug_cache_hits
+        fn.restype, fn.argtypes = C.c_int64, [_vp]
+        return fn(self.h)
 
     def device_info(self):
         sm, ma, mi, mem = C.c_int(), C.c_int(), C.c_int(), C.c_size_t()

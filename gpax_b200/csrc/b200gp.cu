@@ -276,6 +276,24 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
     return set_err(ctx, B2GP_ERR_ARG, "b2gp_set_option", "unknown key", __FILE__, __LINE__);
 }
 
+// every key of b2gp_set_option that has state ("drop_factor_cache" is an action, not a value)
+extern "C" int b2gp_get_option(b2gp_ctx* ctx, const char* key, int64_t* value) {
+    if (!ctx || !key || !value) return B2GP_ERR_ARG;
+    const struct {
+        const char* key;
+        int v;
+    } tab[] = {{"streams", ctx->n_streams},       {"ozaki", ctx->ozaki},         {"trsm_strip", ctx->trsm_strip},
+               {"oz_cluster", ctx->oz_cluster},   {"enqueue_threads", ctx->enqueue_threads}, {"big_grid", ctx->big_grid},
+               {"oz_min_tiles", ctx->oz_min_tiles}, {"panel", ctx->panel},       {"tall_min", ctx->tall_min},
+               {"oz_debug", ctx->oz_debug},       {"tma", ctx->use_tma}};
+    for (const auto& e : tab)
+        if (strcmp(key, e.key) == 0) {
+            *value = e.v;
+            return B2GP_OK;
+        }
+    return set_err(ctx, B2GP_ERR_ARG, "b2gp_get_option", "unknown key", __FILE__, __LINE__);
+}
+
 extern "C" int b2gp_device_info(b2gp_ctx* ctx, int* sm_count, int* cc_major, int* cc_minor, size_t* mem_bytes) {
     if (!ctx) return B2GP_ERR_ARG;
     if (sm_count) *sm_count = ctx->sm_count;
@@ -286,6 +304,14 @@ extern "C" int b2gp_device_info(b2gp_ctx* ctx, int* sm_count, int* cc_major, int
 }
 
 extern "C" int64_t b2gp_debug_cache_hits(b2gp_ctx* ctx) { return ctx ? extra_of(ctx)->cache_hits : -1; }
+
+// Development aid (not part of include/b200gp.h): the first n cumulative path counters of this context, in the order of
+// PathCounter (common.cuh).  Returns how many there are.
+extern "C" int b2gp_debug_path_counts(b2gp_ctx* ctx, int64_t* out, int n) {
+    if (!ctx || (n > 0 && !out)) return B2GP_ERR_ARG;
+    for (int i = 0; i < n && i < PATH_COUNT; ++i) out[i] = ctx->path[i].load(std::memory_order_relaxed);
+    return PATH_COUNT;
+}
 
 extern "C" int b2gp_last_timing(b2gp_ctx* ctx, b2gp_timing* out) {
     if (!ctx || !out) return B2GP_ERR_ARG;
@@ -610,7 +636,7 @@ extern "C" int b2gp_gemm_nt(b2gp_ctx* ctx, int64_t m, int64_t n, int64_t k, doub
                             const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int lower_only, unsigned flags) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, A && B && C && m >= 0 && n >= 0 && k >= 0 && lda >= k && ldb >= k && ldc >= n);
-    ARG_CHECK(ctx, !lower_only || m == n);
+    ARG_CHECK(ctx, !lower_only || m >= n);   // m > n: lower triangle of the leading n x n block, all of the rows below it
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
@@ -827,6 +853,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
             // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
+            if (fused_solve) count_path(ctx, PATH_POTRF_TALL);
             if (fused_solve)
                 RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, P + 1, Linv, inf, 0, keepU ? (double*)ex->Ukeep.p : nullptr));
             else
@@ -2089,7 +2116,6 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
     ARG_CHECK(ctx, N >= 1 && P >= 1 && d >= 1 && d <= GRAM_MAX_D);
     ARG_CHECK(ctx, nb >= 128 && nb <= 1024 && nb % 128 == 0 && N % nb == 0);
     ARG_CHECK(ctx, !(flags & B2GP_FLAG_DEVICE_PTRS) && !(flags & (B2GP_OUT_COV | B2GP_OUT_SAMPLE)));
-    if (ctx->ozaki == 0) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_dist_posterior", "needs the int8 path (ozaki != 0)", __FILE__, __LINE__);
     const bool want_var = flags & B2GP_OUT_VAR;
     ARG_CHECK(ctx, !want_var || var);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
@@ -2151,6 +2177,8 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
     CUDA_TRY(ctx, cudaStreamSynchronize(cs));   // the host staging vectors are pageable
     const double* dth = (const double*)ctx->d_in[3].p;
     double* A = (double*)ds->Aloc.p;
+    // The block-cyclic factorisation has no fp64 trailing update to fall back to: every panel solve and update is an int8
+    // GEMM, so ozaki == 0 (the library default) means "planes from the conditioning bound" here, like -1.
     sl.oz_planes = ctx->ozaki > 0 ? ctx->ozaki : oz_auto_planes((double)N, theta[d], theta[d + 1], jitter);
 
     // ---- the local matrix, generated in place: k(rows, columns) for every local tile, then the diagonal term and y

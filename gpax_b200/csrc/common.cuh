@@ -52,6 +52,22 @@ struct Slot {
     cudaEvent_t ev[8];
 };
 
+// Cumulative per-context counters of the kernels launched and the solver routes entered, in the order
+// b2gp_debug_path_counts reports them.  They sit next to the `launches++` of each site and steer nothing: tests read them
+// to prove which path a call took.
+enum PathCounter {
+    PATH_GEMM_NT = 0,   // gemm_nt_kernel launches (cp.async + DMMA), the 64x64 tail launch of the TMA kernel included
+    PATH_GEMM_TMA,      // gemm_tma_kernel launches (persistent TMA + DMMA)
+    PATH_OZ_MMA,        // oz_mma_kernel launches (int8 wgmma)
+    PATH_OZ_SLICE,      // oz_slice_kernel launches (digit planes of one operand)
+    PATH_TRSM_STRIP,    // trsm_strip_kernel launches
+    PATH_POTRF_DIAG,    // potrf_diag_kernel launches (128-wide leaves)
+    PATH_PANEL_SOLVE,   // panel_solve_all_rows calls
+    PATH_TRSM_TALL,     // trsm_tall calls
+    PATH_POTRF_TALL,    // factorisations that took potrf_tall (top-level entries, not its recursion)
+    PATH_COUNT
+};
+
 struct b2gp_ctx {
     int device = 0;
     int sm_count = 0;
@@ -81,8 +97,11 @@ struct b2gp_ctx {
     DevBuf last_linv;
     int64_t last_n = 0;
     std::atomic<int64_t> launches{0};  // kernels queued (draws may be queued from several host threads)
+    std::atomic<int64_t> path[PATH_COUNT] = {};  // which kernels / routes the work took (b2gp_debug_path_counts)
     std::string err;
 };
+
+static inline void count_path(b2gp_ctx* ctx, int which) { ctx->path[which].fetch_add(1, std::memory_order_relaxed); }
 
 static inline int set_err(b2gp_ctx* ctx, int code, const char* what, const char* detail, const char* file, int line) {
     char buf[512];

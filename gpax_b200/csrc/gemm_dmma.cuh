@@ -216,6 +216,7 @@ static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     kern<<<(unsigned)grid, WARPS_M * WARPS_N * 32, smem_bytes, st>>>(a);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches++;
+    count_path(ctx, PATH_GEMM_NT);
     return B2GP_OK;
 }
 

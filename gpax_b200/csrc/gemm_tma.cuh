@@ -245,12 +245,16 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     // of the last, partial wave are handed to a follow-up launch as 64x64 quarters (2 CTAs/SM): a quarter of the
     // work per CTA on four times the CTAs, so the tail costs ~0.3-0.6 tile-times instead of 1.
     const int S = persist_sms(ctx);
+    // Not when C aliases an operand (the in-place leaf solve B <- B Linv^T): there each row block must be read and written
+    // by ONE CTA, and the quarters of a tile are four CTAs, two of which would read the columns the other two overwrite.
+    const bool inplace = (a.C == a.A || a.C == a.B);
     int64_t main_tiles = tiles;
-    if (tiles > S && tiles % S != 0) main_tiles = tiles - tiles % S;
+    if (!inplace && tiles > S && tiles % S != 0) main_tiles = tiles - tiles % S;
     const int grid = (int)(main_tiles < S ? main_tiles : S);
     gemm_tma_kernel<STAGES, KSUB><<<grid, TG_THREADS, smem_bytes, st>>>(mapA, mapB, a, (int)main_tiles);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches++;
+    count_path(ctx, PATH_GEMM_TMA);
     if (main_tiles < tiles) {
         GemmArgs t = a;
         t.tile_base = (int)main_tiles;
@@ -267,6 +271,7 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
         kern<<<(unsigned)(4 * (tiles - main_tiles)), 256, tail_smem, st>>>(t);
         CUDA_TRY(ctx, cudaGetLastError());
         ctx->launches++;
+        count_path(ctx, PATH_GEMM_NT);
     }
     return B2GP_OK;
 }

@@ -463,6 +463,7 @@ static int oz_slice_launch(b2gp_ctx* ctx, cudaStream_t st, const double* src, in
                                                      trans ? 1 : 0, rowmap128);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches++;
+    count_path(ctx, PATH_OZ_SLICE);
     out->planes = (const int8_t*)planes.p;
     out->scale = (const double*)scale.p;
     out->rows_pad = rp;
@@ -573,6 +574,7 @@ static int oz_mma_launch(b2gp_ctx* ctx, cudaStream_t st, OzWork& w, const OzOper
     }
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches++;
+    count_path(ctx, PATH_OZ_MMA);
     return B2GP_OK;
 }
 

@@ -93,6 +93,8 @@ const char* b2gp_last_error(const b2gp_ctx* ctx);
 /* options: "streams" (draws in flight, 1..16, default 2); "ozaki" (0: fp64 DMMA only, 6 / 7: int8 wgmma base-256 digit
  * planes, -1: 6 or 7 chosen per call from a bound on cond(K); default 0); the full table is in INTEGRATION.md */
 int  b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value);
+/* the current value of any option that holds one (every key of the table except the action "drop_factor_cache") */
+int  b2gp_get_option(b2gp_ctx* ctx, const char* key, int64_t* value);
 int  b2gp_device_info(b2gp_ctx* ctx, int* sm_count, int* cc_major, int* cc_minor, size_t* mem_bytes);
 /* device timing of the most recent entry-point call on this ctx (every call records total_ms) */
 int  b2gp_last_timing(b2gp_ctx* ctx, b2gp_timing* out);
@@ -146,7 +148,9 @@ int  b2gp_trsm_lower(b2gp_ctx* ctx, int64_t n, int64_t nrhs,
                      const double* L, int64_t ldl, double* B, int64_t ldb, unsigned flags);
 
 /* C[m,n] = beta C + alpha A[m,k] B[n,k]^T (fp64, DMMA tensor pipe); lower_only != 0 updates only
- * j <= i (SYRK when A == B).  The trailing-update kernel of the factorisation, exported for the
+ * j <= i (SYRK when A == B) and needs m >= n: with m > n that is the lower triangle of the leading
+ * n x n block plus all n columns of the rows below it (the trapezoid the factorisation updates when
+ * right-hand-side rows ride under the matrix).  The trailing-update kernel of the factorisation, exported for the
  * roofline measurement and the parity tests; replaces the jnp.matmul calls of gp.py:272-273.       */
 int  b2gp_gemm_nt(b2gp_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha,
                   const double* A, int64_t lda, const double* B, int64_t ldb,
@@ -266,6 +270,8 @@ int  b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, co
  *   nb x nb tiles (N a multiple of nb, nb a multiple of 128), generated in place; right-looking Cholesky with the panel
  *   solve spread over the process column, the panel broadcast along process rows and all-gathered down process columns,
  *   look-ahead of one panel, trailing updates on the int8 wgmma kernel; the right-hand sides ride below the matrix.
+ *   There is no fp64 trailing update on this path: option "ozaki" = 0 (the default) picks the digit-plane count from
+ *   the bound on cond(K) exactly like -1; 6 / 7 force it.
  *   Every rank receives mean[P], var[P] (B2GP_OUT_VAR) and info.
  * b2gp_dist_layout: the block-cyclic index algebra as a pure function (no GPU), see dist.cuh.                         */
 int  b2gp_dist_unique_id(void* id128);

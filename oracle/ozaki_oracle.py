@@ -52,10 +52,14 @@ def class_sums(PA, PB):
 
 
 def gemm_nt(A, B, C, alpha=-1.0, S=7, lower_only=False):
-    """C + alpha * A B^T exactly as the CUDA path rounds it.  alpha must be +-1 (power-of-two scale -> exact product)."""
+    """C + alpha * A B^T exactly as the CUDA path rounds it.  alpha must be +-1 (power-of-two scale -> exact product).
+    lower_only needs m >= n and follows the kernel's trapezoid rule (ozaki.cuh, OzMode): rows i < n update j <= i only, the
+    rows below the square part update all n columns; every other entry is C unchanged."""
     if abs(alpha) != 1.0:
         raise ValueError("bit-exact restatement needs alpha = +-1")
     A, B = np.asarray(A, dtype=np.float64), np.asarray(B, dtype=np.float64)
+    if lower_only and A.shape[0] < B.shape[0]:
+        raise ValueError("lower_only needs m >= n")
     if A.shape[1] > K_MAX:                                    # the library splits longer k into launches of <= K_MAX
         out = np.asarray(C, dtype=np.float64)
         for k0 in range(0, A.shape[1], K_MAX):
@@ -70,5 +74,5 @@ def gemm_nt(A, B, C, alpha=-1.0, S=7, lower_only=False):
         acc = D[t].astype(np.float64) * np.ldexp(1.0, -(12 + 8 * t)) + acc      # exact product, one rounding: the fma
     out = (sa[:, None] * alpha * sb[None, :]) * acc + np.asarray(C, dtype=np.float64)
     if lower_only:
-        out = np.where(np.tril(np.ones(out.shape, bool)), out, C)
+        out = np.where(np.tril(np.ones(out.shape, bool)), out, C)      # j <= i: for rows i >= n that is the whole row
     return out

@@ -24,12 +24,14 @@ def main():
     kernel, out = sys.argv[6], sys.argv[7]
     from gpax_b200 import dist
     dc = dist.DistContext(grid=(pr, pc))
-    dc.ctx.set_option("ozaki", int(os.environ.get("B200GP_TEST_OZAKI", "-1")))
+    if "B200GP_TEST_OZAKI" in os.environ:       # unset: the context keeps the library's defaults, as a user's would
+        dc.ctx.set_option("ozaki", int(os.environ["B200GP_TEST_OZAKI"]))
     X, y, Xn, theta = problem(N, P, kernel)
     res = dc.posterior(kernel, X, y, Xn, theta, nb=nb)
     res2 = dc.posterior(kernel, X, y, Xn, theta, nb=nb)          # a second call reuses the cached lists / buffers
     assert np.array_equal(res["mean"], res2["mean"]) and np.array_equal(res["var"], res2["var"])
-    np.savez(out + f".rank{dc.rank}.npz", mean=res["mean"], var=res["var"], info=res["info"], potrf_ms=res["timing"]["potrf_ms"])
+    np.savez(out + f".rank{dc.rank}.npz", mean=res["mean"], var=res["var"], info=res["info"], potrf_ms=res["timing"]["potrf_ms"],
+             ozaki=dc.ctx.get_option("ozaki"))
     dc.close()
 
 

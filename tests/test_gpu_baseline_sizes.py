@@ -24,9 +24,8 @@ RTOL = 1e-9
 def ctx():
     import gpax_b200
     c = gpax_b200.default_context()
-    yield c
-    c.set_option("ozaki", -1)
-    c.set_option("streams", 2)
+    with c.options(ozaki=c.get_option("ozaki"), streams=c.get_option("streams")):      # whatever a test sets is put back
+        yield c
 
 
 def cond_bound(K, floor):
@@ -58,11 +57,14 @@ def test_headline_N16384_vs_oracle(ctx):
     theta = np.concatenate([params["k_length"], [1.0, 0.1, 1.0]])[None, :]
     tol = RTOL * max(1.0, cond / 1e5)
     for planes in (-1, 7, 6, 0):
-        ctx.set_option("ozaki", planes)
-        ctx.set_option("drop_factor_cache", 1)
-        want = ("mean", "var", "cov") if planes == -1 else ("mean", "var")
-        out = ctx.posterior("RBF", X, y, Xn, theta, want=want)
+        want = ("mean", "var", "cov") if planes in (-1, 0) else ("mean", "var")      # full covariance on the default path too
+        with ctx.options(ozaki=planes):
+            ctx.set_option("drop_factor_cache", 1)
+            before = ctx.path_counts()
+            out = ctx.posterior("RBF", X, y, Xn, theta, want=want)
+            moved = {k: v - before[k] for k, v in ctx.path_counts().items()}
         assert out["info"][0] == 0
+        assert (moved["oz_mma"] > 0) == (moved["potrf_tall"] == 1) == (planes != 0), (planes, moved)
         what = f"N=16384 headline, ozaki={planes}, cond(K) <= {cond:.2e}"
         # 6 digit planes are what the auto rule picks below cond 1e6 (DESIGN 4.6); when forced above that they get the
         # model's bound instead of the parity bar
@@ -74,7 +76,6 @@ def test_headline_N16384_vs_oracle(ctx):
         print(f"{what}: scaled error mean {err_m:.2e} var {err_v:.2e}")
         if "cov" in want:
             assert_close(out["cov"][0], rcov, t, "cov " + what)
-    ctx.set_option("ozaki", -1)
 
 
 def c2_inputs():
@@ -98,6 +99,7 @@ def test_c2_N8192_200_draws_vs_oracle():
     S = len(samples["noise"])
     m = gpax_b200.ExactGP(2, "Matern")
     m.X_train, m.y_train = X, y
+    streams0 = m.ctx.get_option("streams")
     m.ctx.set_option("streams", 4)
     mean, y_sampled = m.predict(0, Xn, samples, n=1)
     assert mean.shape == (1024,) and y_sampled.shape == (S, 1, 1024) and np.isfinite(y_sampled).all()
@@ -118,7 +120,7 @@ def test_c2_N8192_200_draws_vs_oracle():
         one = m.get_mvn_posterior(Xn, ps)
         assert_close(one[0], rmean, tol, "get_mvn_posterior mean " + what)
         assert_close(one[1], rcov, tol, "get_mvn_posterior cov " + what)
-    m.ctx.set_option("streams", 2)
+    m.ctx.set_option("streams", streams0)
 
 
 def test_c3_N16384_vigp_tile_vs_oracle():

@@ -24,14 +24,17 @@ def n_gpus():
 
 
 def run_grid(pr, pc, N, P, nb, kernel, ozaki=-1):
+    """ozaki=None: the workers set no option at all (the library's defaults)"""
     world = pr * pc
     port = 29600 + (os.getpid() + 7 * pr + 13 * pc + N) % 300
     with tempfile.TemporaryDirectory() as td:
         out = os.path.join(td, "res")
         procs = []
         for r in range(world):
-            env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), LOCAL_RANK=str(r), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port),
-                       B200GP_TEST_OZAKI=str(ozaki))
+            env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), LOCAL_RANK=str(r), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+            env.pop("B200GP_TEST_OZAKI", None)
+            if ozaki is not None:
+                env["B200GP_TEST_OZAKI"] = str(ozaki)
             procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "dist_lib_worker.py"), str(pr), str(pc), str(N),
                                            str(P), str(nb), kernel, out], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
         logs = [p.communicate(timeout=600)[0] for p in procs]
@@ -44,11 +47,8 @@ def single_gpu(N, P, kernel, ozaki=-1):
     import gpax_b200
     X, y, Xn, theta = problem(N, P, kernel)
     ctx = gpax_b200.default_context()
-    ctx.set_option("ozaki", ozaki)
-    try:
+    with ctx.options(ozaki=ozaki):
         return ctx.posterior(kernel, X, y, Xn, theta[None], want=("mean", "var"))
-    finally:
-        ctx.set_option("ozaki", -1)
 
 
 # The block-cyclic path runs EVERY update through the int8 kernel at k = nb, the single-GPU path only the large ones, so

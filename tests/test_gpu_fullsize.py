@@ -85,16 +85,15 @@ def test_many_draws_stream_through_few_workspaces(ctx):
     y1, y2 = rng.standard_normal(N), rng.standard_normal(N)
     theta = np.column_stack([np.exp(rng.normal(np.log(0.3), 0.1, (S, d))), np.exp(rng.normal(0, 0.1, S)),
                              np.exp(rng.normal(np.log(0.1), 0.1, S)), np.ones(S)])
-    ctx.set_option("streams", 4)
-    a = ctx.posterior("RBF", X, y1, Xn, theta, want=("mean",))["mean"]
-    b = ctx.posterior("RBF", X, y2, Xn, theta, want=("mean",))["mean"]
-    c = ctx.posterior("RBF", X, y1 + 2 * y2, Xn, theta, want=("mean",))["mean"]
+    with ctx.options(streams=4):
+        a = ctx.posterior("RBF", X, y1, Xn, theta, want=("mean",))["mean"]
+        b = ctx.posterior("RBF", X, y2, Xn, theta, want=("mean",))["mean"]
+        c = ctx.posterior("RBF", X, y1 + 2 * y2, Xn, theta, want=("mean",))["mean"]
     scale = np.abs(c).max()
     np.testing.assert_allclose(c, a + 2 * b, rtol=0, atol=1e-9 * scale)
-    ctx.set_option("streams", 2)
 
 
-def test_int8_tcgen05_path_matches_fp64_dmma_path(ctx):
+def test_int8_wgmma_path_matches_fp64_dmma_path(ctx):
     """N = 8192 (large enough for the int8 digit-plane kernel to take the trailing updates): the posterior through the
     int8 path with 7 base-256 planes agrees with the all-fp64 DMMA path to the parity bar (1e-9, scale-relative) at
     cond(K) ~ 1e5, and so does 6 planes to 1e-7; the factor itself agrees to 1e-12 of its scale.  (The comparison
@@ -109,11 +108,13 @@ def test_int8_tcgen05_path_matches_fp64_dmma_path(ctx):
     theta = np.array([[0.25, 0.3, 1.0, 1e-3, 1.0]])       # noise 1e-3 -> cond(K) ~ N * scale / noise ~ 1e5 .. 1e6 effective
     res = {}
     for planes in (0, 7, 6):
-        ctx.set_option("ozaki", planes)
-        ctx.set_option("drop_factor_cache", 1)
-        res[planes] = ctx.posterior("Matern", X, y, Xn, theta, want=("mean", "var"))
+        with ctx.options(ozaki=planes):
+            ctx.set_option("drop_factor_cache", 1)
+            before = ctx.path_counts()
+            res[planes] = ctx.posterior("Matern", X, y, Xn, theta, want=("mean", "var"))
+            moved = {k: v - before[k] for k, v in ctx.path_counts().items()}
         assert res[planes]["info"][0] == 0
-    ctx.set_option("ozaki", -1)
+        assert (moved["oz_mma"] > 0) == (moved["potrf_tall"] == 1) == (planes != 0), (planes, moved)
     ref = res[0]
     for planes, tol in ((7, 1e-9), (6, 1e-7)):
         for k in ("mean", "var"):
@@ -125,16 +126,15 @@ def test_int8_tcgen05_path_matches_fp64_dmma_path(ctx):
     ell = np.array([0.25, 0.3])
     Ls = {}
     for planes in (0, 7):
-        ctx.set_option("ozaki", planes)
         K = ctx.alloc((N, N))
         ctx._check(ctx.lib.b2gp_gram(ctx.h, 1, dX.ptr, N, dX.ptr, N, d, _ffi._ptr(ell), 1.0, 1.0, 1e-3 + 1e-6, 1, K.ptr, N,
                                      _ffi.FLAG_DEVICE_PTRS))
         info = C.c_int(0)
-        ctx._check(ctx.lib.b2gp_potrf(ctx.h, N, K.ptr, N, C.byref(info), _ffi.FLAG_DEVICE_PTRS))
+        with ctx.options(ozaki=planes):
+            ctx._check(ctx.lib.b2gp_potrf(ctx.h, N, K.ptr, N, C.byref(info), _ffi.FLAG_DEVICE_PTRS))
         assert info.value == 0
         Ls[planes] = _download_rows(ctx, K, N, N - 64, 64)      # the last 64 rows depend on every update
         K.free()
-    ctx.set_option("ozaki", -1)
     mask = np.tril(np.ones((N, N), bool))[N - 64:]
     dev = np.abs(Ls[7] - Ls[0])[mask].max() / np.abs(Ls[0][mask]).max()
     print(f"factor rows {N-64}..{N}: max scaled deviation {dev:.2e}")

@@ -112,14 +112,13 @@ def test_gemm_large_tma_path(ctx, m, n, k, lower):
         np.testing.assert_array_equal(np.triu(C, 1), np.triu(C0, 1))
     else:
         np.testing.assert_allclose(C, ref, rtol=0, atol=tol)
-    ctx.set_option("tma", 0)
-    C2 = ctx.gemm_nt(A, B, C0, alpha=-1.0, beta=1.0, lower_only=lower)
-    ctx.set_option("tma", 1)
+    with ctx.options(tma=0):
+        C2 = ctx.gemm_nt(A, B, C0, alpha=-1.0, beta=1.0, lower_only=lower)
     np.testing.assert_array_equal(C, C2)
 
 
 @pytest.mark.parametrize("m,n,k,lower", [(2500, 1300, 700, False), (3000, 3000, 1536, True), (1025, 8192, 4096, False)])
-def test_int8_tcgen05_gemm(ctx, m, n, k, lower):
+def test_int8_wgmma_gemm(ctx, m, n, k, lower):
     """the rank-k update through the int8 digit-plane kernel (ozaki.cuh): rows of very different magnitude (each row
     carries its own power-of-two scale), ragged m / n / k; error measured against |a_i| |b_j| like a DGEMM's"""
     rng = np.random.default_rng(m + n + k)
@@ -131,16 +130,18 @@ def test_int8_tcgen05_gemm(ctx, m, n, k, lower):
     scale = np.linalg.norm(A, axis=1)[:, None] * np.linalg.norm(B, axis=1)[None, :] + np.abs(C0) + np.abs(ref)
     errs = {}
     for planes in (0, 7, 6):
-        ctx.set_option("ozaki", planes)
-        C = ctx.gemm_nt(A, B, C0, alpha=-1.0, beta=1.0, lower_only=lower)
+        with ctx.options(ozaki=planes):
+            before = ctx.path_counts()["oz_mma"]
+            C = ctx.gemm_nt(A, B, C0, alpha=-1.0, beta=1.0, lower_only=lower)
+            assert ctx.path_counts()["oz_mma"] - before == (1 if planes else 0)   # the kernel the error bar is for
         mask = np.tril(np.ones((m, n), bool)) if lower else np.ones((m, n), bool)
         errs[planes] = (np.abs(C - ref) / scale)[mask].max()
         if lower:
             np.testing.assert_array_equal(C[~mask], C0[~mask])
-    ctx.set_option("ozaki", 7)
     assert errs[0] <= 3e-15 and errs[7] <= 2e-14 and errs[6] <= 5e-13, errs
     # alpha, and a B different from A with lower_only off
-    C = ctx.gemm_nt(A, B, C0, alpha=0.5, beta=1.0, lower_only=lower)
+    with ctx.options(ozaki=7):
+        C = ctx.gemm_nt(A, B, C0, alpha=0.5, beta=1.0, lower_only=lower)
     ref2 = C0 + 0.5 * A @ B.T
     scale2 = scale + np.abs(ref2)
     assert (np.abs(C - ref2) / scale2)[np.tril(np.ones((m, n), bool)) if lower else np.ones((m, n), bool)].max() <= 2e-14
@@ -168,14 +169,15 @@ def test_trsm_strip_kernel_matches_recursion(ctx, n, nrhs):
     A = spd(rng, n)
     B = rng.standard_normal((nrhs, n))
     out = {}
-    try:
-        for strip in (0, 256, 512):
-            ctx.set_option("trsm_strip", strip)
+    assert ctx.get_option("ozaki") == 0          # with the int8 path on, >= 1024 rows would take the panel route, not the strip kernel
+    for strip in (0, 256, 512):
+        with ctx.options(trsm_strip=strip):
             L, info = ctx.potrf(A)
             assert info == 0
+            before = ctx.path_counts()
             out[strip] = (np.tril(L), ctx.trsm_lower(L, B))
-    finally:
-        ctx.set_option("trsm_strip", 256)
+            after = ctx.path_counts()
+            assert (after["trsm_strip"] > before["trsm_strip"]) == (strip > 0) and after["panel_solve"] == before["panel_solve"]
     ref = sla.solve_triangular(out[0][0], B.T, lower=True).T
     for strip in (256, 512):
         np.testing.assert_allclose(out[strip][0], out[0][0], rtol=0, atol=1e-12 * np.abs(out[0][0]).max())

@@ -122,13 +122,12 @@ def test_batched_draws_and_sampling(gp):
     theta = np.concatenate([samples["k_length"], samples["k_scale"][:, None], samples["noise"][:, None], np.ones((S, 1))], 1)
     ctx = gp.default_context()
     for streams in (1, 2, 4):
-        ctx.set_option("streams", streams)
-        out = ctx.posterior("Matern", Xtr, ytr, Xte, theta, want=("mean", "cov"), eps=eps)
+        with ctx.options(streams=streams):
+            out = ctx.posterior("Matern", Xtr, ytr, Xte, theta, want=("mean", "cov"), eps=eps)
         assert_close(out["mean"], means, RTOL)
         assert_close(out["mean"].mean(0), ymean, RTOL)
         # chol(cov) amplifies rounding of cov by its condition number: looser bar on the samples
         assert_close(out["y_sampled"], ysamp, 1e-6)
-    ctx.set_option("streams", 2)
     one = ctx.posterior("Matern", Xtr, ytr, Xte, theta[2:3], want=("mean", "cov"))
     np.testing.assert_array_equal(one["mean"][0], out["mean"][2])      # batched == single, bit for bit
     np.testing.assert_array_equal(one["cov"][0], out["cov"][2])
@@ -302,12 +301,18 @@ def test_kernel_functions_shapes(gp):
                 assert isinstance(K, np.ndarray) and K.shape == (5, 5)
 
 
+def moved(ctx, before):
+    return {k: v - before[k] for k, v in ctx.path_counts().items()}
+
+
 # ------------------------------------------------------------------ tall-panel factorisation (N >= 2048, int8 path on)
+@pytest.mark.parametrize("ozaki", [7, -1])
 @pytest.mark.parametrize("kname,N,P", [("RBF", 2500, 300), ("Matern", 3100, 129), ("Periodic", 2048, 64)])
-def test_tall_panel_path_vs_oracle(gp, kname, N, P):
-    """N >= 2048 takes potrf_tall (potrf.cuh): the right-hand-side rows [k_pX; y] ride under k_XX through int8 panel GEMMs
-    with explicit inverses of the 512-wide diagonal blocks.  Ragged N (not a multiple of 512 / 128), all three kernels,
-    mean + full covariance against the oracle, and against the recursive scheme (panel = 0)."""
+def test_tall_panel_path_vs_oracle(gp, kname, N, P, ozaki):
+    """With the int8 path on (`ozaki` 7, or -1 = planes from the conditioning bound) N >= 2048 takes potrf_tall (potrf.cuh):
+    the right-hand-side rows [k_pX; y] ride under k_XX through int8 panel GEMMs with explicit inverses of the `panel`-wide
+    diagonal blocks.  Ragged N (not a multiple of 512 / 128), all three kernels, mean + full covariance against the
+    oracle, for every panel width and for the recursive scheme (panel = 0); the path counters prove which one ran."""
     rng = np.random.default_rng(N + P)
     d = 2
     X = rng.uniform(0, 1, (N, d))
@@ -320,17 +325,23 @@ def test_tall_panel_path_vs_oracle(gp, kname, N, P):
     tol = RTOL * max(1.0, cond / 1e5)
     m = gp.ExactGP(d, kname)
     m.X_train, m.y_train = X, y
-    outs = {}
     for panel in (1024, 512, 256, 0):
-        m.ctx.set_option("panel", panel)
-        mean, cov = m.get_mvn_posterior(Xn, params)
-        assert_close(mean, rmean, tol, f"mean panel={panel} cond={cond:.1e}")
-        assert_close(cov, rcov, tol, f"cov panel={panel} cond={cond:.1e}")
-        outs[panel] = mean
-    m.ctx.set_option("panel", 1024)
+        with m.ctx.options(ozaki=ozaki, panel=panel):
+            before = m.ctx.path_counts()
+            mean, cov = m.get_mvn_posterior(Xn, params)
+            c = moved(m.ctx, before)
+        assert_close(mean, rmean, tol, f"mean panel={panel} ozaki={ozaki} cond={cond:.1e}")
+        assert_close(cov, rcov, tol, f"cov panel={panel} ozaki={ozaki} cond={cond:.1e}")
+        if panel:
+            assert c["potrf_tall"] == 1 and c["panel_solve"] == -(-N // panel) and c["oz_mma"] >= c["panel_solve"], (panel, c)
+        else:
+            assert c["potrf_tall"] == c["panel_solve"] == 0, c
     # a failed factorisation still gives NaNs, not an exception, on this path
     bad = dict(params, k_scale=-1.0)
-    mean, cov = m.get_mvn_posterior(Xn, bad)
+    with m.ctx.options(ozaki=ozaki):
+        before = m.ctx.path_counts()
+        mean, cov = m.get_mvn_posterior(Xn, bad)
+        assert moved(m.ctx, before)["potrf_tall"] == 1
     assert np.isnan(mean).all() and np.isnan(cov).all()
 
 
@@ -338,9 +349,8 @@ def test_tall_panel_path_vs_oracle(gp, kname, N, P):
 def test_factor_cache_reuse_with_more_and_fewer_test_points(gp, N):
     """Single-theta calls keep the factor of k_XX (the reference re-inverts it per call, gp.py:269-271).  The right-hand
     sides live under the factor in the same buffer, so a later call with MORE test points has to grow the buffer around
-    the factor; at N >= 2048 the reuse solves through the kept inverses of the diagonal blocks (trsm_tall).  Each reuse
-    is checked against the oracle, for a handful and for many test points."""
-    import ctypes
+    the factor; at N >= 2048 with the int8 path on (set here: ozaki = 7) the reuse solves through the kept inverses of the
+    diagonal blocks (trsm_tall).  Each reuse is checked against the oracle, for a handful and for many test points."""
     rng = np.random.default_rng(N)
     d = 2
     X = rng.uniform(0, 1, (N, d))
@@ -348,16 +358,18 @@ def test_factor_cache_reuse_with_more_and_fewer_test_points(gp, N):
     params = {"k_length": np.array([0.3, 0.4]), "k_scale": 1.2, "noise": 0.05}
     m = gp.ExactGP(d, "Matern")
     m.X_train, m.y_train = X, y
-    hits = m.ctx.lib.b2gp_debug_cache_hits
-    hits.restype, hits.argtypes = ctypes.c_int64, [ctypes.c_void_p]
     m.ctx.set_option("drop_factor_cache", 1)
     cond = np.linalg.cond(oracle.get_kernel("Matern")(X, X, params, params["noise"]))
     tol = RTOL * max(1.0, cond / 1e5)
-    h0 = hits(m.ctx.h)
+    h0 = m.ctx.cache_hits()
     for k, P in enumerate((40, 10, 700, 1500, 3)):            # the first call factors, the others reuse; 700 and 1500 grow the buffer
         Xn = rng.uniform(0, 1, (P, d))
-        mean, cov = m.get_mvn_posterior(Xn, params)
+        with m.ctx.options(ozaki=7):
+            before = m.ctx.path_counts()
+            mean, cov = m.get_mvn_posterior(Xn, params)
+            c = moved(m.ctx, before)
         rmean, rcov = oracle.exact_posterior_chol(X, y, Xn, params, "Matern")
         assert_close(mean, rmean, tol, f"mean call {k} P={P} cond={cond:.1e}")
         assert_close(cov, rcov, tol, f"cov call {k} P={P} cond={cond:.1e}")
-        assert hits(m.ctx.h) - h0 == k
+        assert m.ctx.cache_hits() - h0 == k
+        assert c["trsm_tall"] == (1 if N >= 2048 and k > 0 else 0) and c["potrf_tall"] == (1 if N >= 2048 and k == 0 else 0), (k, c)

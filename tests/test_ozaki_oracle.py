@@ -70,6 +70,26 @@ def test_gemm_error_against_exact_rational(S, bound):
     np.testing.assert_array_equal(np.triu(low, 1), np.triu(C[:5, :5], 1))
 
 
+@pytest.mark.parametrize("S", [7, 6])
+def test_lower_only_trapezoid_rule(S):
+    """lower_only with more rows than columns (right-hand-side rows riding below the matrix): rows < n take j <= i, the rows
+    below take all n columns; everything written equals the full product, everything else is C untouched"""
+    rng = np.random.default_rng(7)
+    m, n, k = 9, 5, 40
+    A, C = _rows(rng, m, k), rng.standard_normal((m, n))
+    full = oz.gemm_nt(A, A[:n], C, alpha=-1.0, S=S)
+    trap = oz.gemm_nt(A, A[:n], C, alpha=-1.0, S=S, lower_only=True)
+    for i in range(m):
+        for j in range(n):
+            assert trap[i, j] == (full[i, j] if (i >= n or j <= i) else C[i, j]), (i, j)
+    ref = C - A @ A[:n].T                                           # and the written part is the product, by plain NumPy
+    written = np.tril(np.ones((m, n), bool))
+    scale = np.linalg.norm(A, axis=1)[:, None] * np.linalg.norm(A[:n], axis=1)[None, :] + np.abs(C)
+    assert (np.abs(trap - ref) / scale)[written].max() < (2.0 ** -49 if S == 7 else 2.0 ** -42)
+    with pytest.raises(ValueError):
+        oz.gemm_nt(A[:n - 1], A[:n], C[:n - 1], alpha=-1.0, S=S, lower_only=True)     # fewer rows than columns
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("S", [7, 6])
 def test_int8_kernel_equals_the_restatement_bit_for_bit(S):
@@ -79,9 +99,8 @@ def test_int8_kernel_equals_the_restatement_bit_for_bit(S):
     rng = np.random.default_rng(3)
     m, n, k = 1536, 1280, 544                                       # >= 132 tiles of 128 x 64 (one per SM of an H100 SXM), k >= 512, ragged k-block
     A, B, C = _rows(rng, m, k), _rows(rng, n, k), rng.standard_normal((m, n))
-    try:
-        ctx.set_option("ozaki", S)
+    before = ctx.path_counts()["oz_mma"]
+    with ctx.options(ozaki=S):
         got = ctx.gemm_nt(A, B, C, alpha=-1.0, beta=1.0)
-    finally:
-        ctx.set_option("ozaki", -1)
+    assert ctx.path_counts()["oz_mma"] == before + 1                # the int8 kernel is what ran
     np.testing.assert_array_equal(got, oz.gemm_nt(A, B, C, alpha=-1.0, S=S))
