@@ -18,101 +18,33 @@
 #include "dist.cuh"
 
 // ------------------------------------------------------------------------------------------ helpers
-namespace {
-
-struct EventPool {
-    std::vector<cudaEvent_t> ev;
-    size_t next = 0;
-    cudaEvent_t get() {
-        if (next == ev.size()) {
-            cudaEvent_t e;
-            if (cudaEventCreate(&e) != cudaSuccess) return nullptr;
-            ev.push_back(e);
-        }
-        return ev[next++];
-    }
-    void reset() { next = 0; }
-    void destroy() {
-        for (auto e : ev) cudaEventDestroy(e);
-        ev.clear();
-        next = 0;
-    }
-};
-
-struct Extra {  // ctx-private state that is not part of the struct the kernels' headers see
-    EventPool pool;
-    b2gp_timing last{};
-    cudaEvent_t slot_done[B2GP_MAX_STREAMS] = {};
-    cudaEvent_t inputs_ready = nullptr;
-    DevBuf theta1;     // one-draw theta for b2gp_gram
-    DevBuf potrf_buf;  // staging for host-pointer b2gp_potrf / trsm / gemm
-    DevBuf gemm_buf[3];
-    std::vector<void*> user_allocs;
-    DevBuf eb[12];     // scratch of b2gp_sparse_elbo
-    DevBuf f32_in[8];  // fp32 staging of the inputs / outputs of calls made with B2GP_FLAG_F32
-    DevBuf f32_out[4];
-    // factor cache of slot 0 (host-pointer, single-draw calls): predict_in_batches / viGP chunk loops call the
-    // posterior repeatedly with the same training set and theta; the reference re-inverts k_XX every time
-    // (gp.py:319-322 -> gp.py:269-271), here the factor L and its inverted diagonal blocks are kept.
-    struct {
-        bool valid = false;
-        int kind = -1, d = 0;
-        int64_t N = 0;
-        double jitter = 0.0;
-        std::vector<double> theta;
-        std::vector<char> X;   // raw bytes of the caller's training inputs (fp64 or fp32)
-        int info = 0;
-        int64_t U_nb = 0;      // > 0: `Ukeep` holds the explicit inverses of the factor's U_nb-wide diagonal blocks (potrf_tall)
-    } fcache;
-    DevBuf Ukeep;
-    int64_t cache_hits = 0;
-    DistState* dist = nullptr;   // multi-GPU state (dist.cuh), created by b2gp_dist_init
-};
-
-}  // namespace
-
-static std::vector<std::pair<b2gp_ctx*, Extra*>> g_extras;
-static Extra* extra_of(b2gp_ctx* ctx) {
-    for (auto& p : g_extras)
-        if (p.first == ctx) return p.second;
-    return nullptr;
-}
-
 static inline bool dev_ptrs(unsigned flags) { return (flags & B2GP_FLAG_DEVICE_PTRS) != 0; }
-
-static int free_buf(DevBuf& b) {
-    if (b.p) cudaFree(b.p);
-    b.p = nullptr;
-    b.cap = 0;
-    return 0;
-}
 
 struct CallTimer {
     b2gp_ctx* ctx;
-    Extra* ex;
     int64_t launches0;
-    CallTimer(b2gp_ctx* c) : ctx(c), ex(extra_of(c)), launches0(c->launches) {}
+    CallTimer(b2gp_ctx* c) : ctx(c), launches0(c->launches) {}
     std::chrono::steady_clock::time_point t_begin;
     int begin(cudaStream_t st) {
         t_begin = std::chrono::steady_clock::now();
-        ex->last = b2gp_timing{};
-        ex->pool.reset();
+        ctx->last = b2gp_timing{};
+        ctx->pool.reset();
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_begin, st));
         return B2GP_OK;
     }
     // host time spent queueing work so far (call before any copy into pageable memory, which blocks the host)
     void mark_enqueued() {
-        ex->last.host_enqueue_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
+        ctx->last.host_enqueue_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count();
     }
     int end(cudaStream_t st, b2gp_timing* out) {
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_end, st));
-        if (ex->last.host_enqueue_ms == 0.0) mark_enqueued();
+        if (ctx->last.host_enqueue_ms == 0.0) mark_enqueued();
         CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_end));
         float ms = 0.f;
         CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_begin, ctx->ev_end));
-        ex->last.total_ms = ms;
-        ex->last.launches = ctx->launches - launches0;
-        if (out) *out = ex->last;
+        ctx->last.total_ms = ms;
+        ctx->last.launches = ctx->launches - launches0;
+        if (out) *out = ctx->last;
         return B2GP_OK;
     }
 };
@@ -150,64 +82,25 @@ extern "C" int b2gp_ctx_create(int device, b2gp_ctx** out) {
     cudaEventCreate(&ctx->ev_end);
     cudaEventCreate(&ctx->ev_a);
     cudaEventCreate(&ctx->ev_b);
-    Extra* ex = new Extra();
-    for (int i = 0; i < B2GP_MAX_STREAMS; ++i) cudaEventCreateWithFlags(&ex->slot_done[i], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&ex->inputs_ready, cudaEventDisableTiming);
-    g_extras.emplace_back(ctx, ex);
+    for (int i = 0; i < B2GP_MAX_STREAMS; ++i) cudaEventCreateWithFlags(&ctx->slot_done[i], cudaEventDisableTiming);
+    cudaEventCreateWithFlags(&ctx->inputs_ready, cudaEventDisableTiming);
     *out = ctx;
     return B2GP_OK;
 }
 
+// The device buffers (and the multi-GPU state, if b2gp_dist_finalize was not called) are released by `delete ctx`.
 extern "C" int b2gp_ctx_destroy(b2gp_ctx* ctx) {
     if (!ctx) return B2GP_OK;
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    Extra* ex = extra_of(ctx);
-    for (int i = 0; i < B2GP_MAX_STREAMS; ++i) {
-        Slot& s = ctx->slots[i];
-        free_buf(s.A);
-        free_buf(s.Vt);
-        free_buf(s.Linv);
-        free_buf(s.cov);
-        free_buf(s.LinvC);
-        free_buf(s.misc);
-        free_buf(s.panelU);
-        free_buf(s.oz.planesA);
-        free_buf(s.oz.planesB);
-        free_buf(s.oz.scaleA);
-        free_buf(s.oz.scaleB);
-        free_buf(s.oz.prof);
-        for (auto& l : s.oz.lists) free_buf(l.dev);
+    for (Slot& s : ctx->slots) {
         for (int e = 0; e < 8; ++e) cudaEventDestroy(s.ev[e]);
         cudaStreamDestroy(s.stream);
     }
-    for (auto& b : ctx->d_in) free_buf(b);
-    for (auto& b : ctx->d_out) free_buf(b);
-    free_buf(ctx->d_info);
-    free_buf(ctx->last_linv);
-    cudaEventDestroy(ctx->ev_begin);
-    cudaEventDestroy(ctx->ev_end);
-    cudaEventDestroy(ctx->ev_a);
-    cudaEventDestroy(ctx->ev_b);
-    if (ex) {
-        ex->pool.destroy();
-        for (int i = 0; i < B2GP_MAX_STREAMS; ++i) cudaEventDestroy(ex->slot_done[i]);
-        cudaEventDestroy(ex->inputs_ready);
-        free_buf(ex->theta1);
-        free_buf(ex->Ukeep);
-        for (auto& b : ex->eb) free_buf(b);
-        for (auto& b : ex->f32_in) free_buf(b);
-        for (auto& b : ex->f32_out) free_buf(b);
-        free_buf(ex->potrf_buf);
-        for (auto& b : ex->gemm_buf) free_buf(b);
-        for (void* p : ex->user_allocs) cudaFree(p);
-        for (size_t i = 0; i < g_extras.size(); ++i)
-            if (g_extras[i].first == ctx) {
-                g_extras.erase(g_extras.begin() + i);
-                break;
-            }
-        delete ex;
-    }
+    for (cudaEvent_t e : {ctx->ev_begin, ctx->ev_end, ctx->ev_a, ctx->ev_b, ctx->inputs_ready}) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->slot_done) cudaEventDestroy(e);
+    ctx->pool.destroy();
+    for (void* p : ctx->user_allocs) cudaFree(p);
     delete ctx;
     return B2GP_OK;
 }
@@ -252,7 +145,7 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
     if (strcmp(key, "panel") == 0) {   // diagonal-block width of the tall-panel factorisation; 0 = recursive scheme only
         ARG_CHECK(ctx, value == 0 || value == 128 || value == 256 || value == 512 || value == 1024);
         ctx->panel = (int)value;
-        extra_of(ctx)->fcache.valid = false;
+        ctx->fcache.valid = false;
         return B2GP_OK;
     }
     if (strcmp(key, "tall_min") == 0) {
@@ -270,7 +163,7 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
         return B2GP_OK;
     }
     if (strcmp(key, "drop_factor_cache") == 0) {
-        extra_of(ctx)->fcache.valid = false;
+        ctx->fcache.valid = false;
         return B2GP_OK;
     }
     return set_err(ctx, B2GP_ERR_ARG, "b2gp_set_option", "unknown key", __FILE__, __LINE__);
@@ -303,7 +196,7 @@ extern "C" int b2gp_device_info(b2gp_ctx* ctx, int* sm_count, int* cc_major, int
     return B2GP_OK;
 }
 
-extern "C" int64_t b2gp_debug_cache_hits(b2gp_ctx* ctx) { return ctx ? extra_of(ctx)->cache_hits : -1; }
+extern "C" int64_t b2gp_debug_cache_hits(b2gp_ctx* ctx) { return ctx ? ctx->cache_hits : -1; }
 
 // Development aid (not part of include/b200gp.h): the first n cumulative path counters of this context, in the order of
 // PathCounter (common.cuh).  Returns how many there are.
@@ -315,7 +208,7 @@ extern "C" int b2gp_debug_path_counts(b2gp_ctx* ctx, int64_t* out, int n) {
 
 extern "C" int b2gp_last_timing(b2gp_ctx* ctx, b2gp_timing* out) {
     if (!ctx || !out) return B2GP_ERR_ARG;
-    *out = extra_of(ctx)->last;
+    *out = ctx->last;
     return B2GP_OK;
 }
 
@@ -326,7 +219,7 @@ extern "C" int b2gp_dev_alloc(b2gp_ctx* ctx, size_t bytes, void** dptr) {
     void* p = nullptr;
     cudaError_t e = cudaMalloc(&p, bytes ? bytes : 16);
     if (e != cudaSuccess) return set_err(ctx, B2GP_ERR_NOMEM, "cudaMalloc", cudaGetErrorString(e), __FILE__, __LINE__);
-    extra_of(ctx)->user_allocs.push_back(p);
+    ctx->user_allocs.push_back(p);
     *dptr = p;
     return B2GP_OK;
 }
@@ -334,7 +227,7 @@ extern "C" int b2gp_dev_alloc(b2gp_ctx* ctx, size_t bytes, void** dptr) {
 extern "C" int b2gp_dev_free(b2gp_ctx* ctx, void* dptr) {
     if (!ctx) return B2GP_ERR_ARG;
     if (!dptr) return B2GP_OK;
-    auto& v = extra_of(ctx)->user_allocs;
+    auto& v = ctx->user_allocs;
     for (size_t i = 0; i < v.size(); ++i)
         if (v[i] == dptr) {
             v.erase(v.begin() + i);
@@ -421,17 +314,24 @@ static int stage_in_t(b2gp_ctx* ctx, cudaStream_t st, DevBuf& buf, DevBuf& tmp, 
         fsrc = (const float*)tmp.p;
     }
     RET_IF(ensure(ctx, buf, count * 8));
-    cvt_f32_f64_kernel<<<grid_for((int64_t)count), 256, 0, st>>>((double*)buf.p, fsrc, (int64_t)count);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch(ctx, st, grid_for((int64_t)count), 256, 0, cvt_f32_f64_kernel, (double*)buf.p, fsrc, (int64_t)count));
     *out = (const double*)buf.p;
     return B2GP_OK;
 }
 
-// device doubles [rows, cols] (leading dimension lds) -> the caller's float array (host or device, leading dimension ldd)
-static int store_out_f32(b2gp_ctx* ctx, cudaStream_t st, DevBuf& tmp, void* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows,
-                         int64_t cols, bool is_dev) {
-    if (rows <= 0 || cols <= 0) return B2GP_OK;
+// A result of doubles [rows, cols] at `src` (device, leading dimension lds) -> the caller's array `dst` (leading dimension
+// ldd): with f32 narrowed into the caller's float array (host or device); else copied back to the host array, or, for a
+// device array, already in place (the result was written there).
+static int store_out(b2gp_ctx* ctx, cudaStream_t st, DevBuf& tmp, void* dst, int64_t ldd, const double* src, int64_t lds, int64_t rows,
+                     int64_t cols, bool is_dev, bool f32) {
+    if (rows <= 0 || cols <= 0 || (is_dev && !f32)) return B2GP_OK;
+    if (!f32) {
+        if (ldd == cols && lds == cols)
+            CUDA_TRY(ctx, cudaMemcpyAsync(dst, src, (size_t)rows * cols * 8, cudaMemcpyDeviceToHost, st));
+        else
+            CUDA_TRY(ctx, cudaMemcpy2DAsync(dst, (size_t)ldd * 8, src, (size_t)lds * 8, (size_t)cols * 8, (size_t)rows, cudaMemcpyDeviceToHost, st));
+        return B2GP_OK;
+    }
     float* fdst = (float*)dst;
     int64_t ldt = ldd;
     if (!is_dev) {
@@ -439,9 +339,7 @@ static int store_out_f32(b2gp_ctx* ctx, cudaStream_t st, DevBuf& tmp, void* dst,
         fdst = (float*)tmp.p;
         ldt = cols;
     }
-    cvt_f64_f32_kernel<<<grid_for(rows * cols), 256, 0, st>>>(fdst, ldt, src, lds, rows, cols);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch(ctx, st, grid_for(rows * cols), 256, 0, cvt_f64_f32_kernel, fdst, ldt, src, lds, rows, cols));
     if (!is_dev)
         CUDA_TRY(ctx, cudaMemcpy2DAsync(dst, (size_t)ldd * 4, fdst, (size_t)ldt * 4, (size_t)cols * 4, (size_t)rows, cudaMemcpyDeviceToHost, st));
     return B2GP_OK;
@@ -456,7 +354,6 @@ extern "C" int b2gp_gram(b2gp_ctx* ctx, int kind, const double* X, int64_t n, co
     ARG_CHECK(ctx, X && Z && K && lengthscale);
     ARG_CHECK(ctx, n >= 0 && m >= 0 && d >= 1 && d <= GRAM_MAX_D && ldk >= m);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
@@ -466,16 +363,16 @@ extern "C" int b2gp_gram(b2gp_ctx* ctx, int kind, const double* X, int64_t n, co
     th[d] = scale;
     th[d + 1] = diag_add;
     th[d + 2] = period;
-    RET_IF(ensure(ctx, ex->theta1, sizeof th));
-    CUDA_TRY(ctx, cudaMemcpyAsync(ex->theta1.p, th, (d + 3) * sizeof(double), cudaMemcpyHostToDevice, st));
+    RET_IF(ensure(ctx, ctx->theta1, sizeof th));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->theta1.p, th, (d + 3) * sizeof(double), cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));  // th is a stack buffer
     const bool dev = dev_ptrs(flags), f32 = f32_io(flags);
     const double *dX, *dZ;
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ex->f32_in[0], X, (size_t)n * d, dev, f32, &dX));
+    RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ctx->f32_in[0], X, (size_t)n * d, dev, f32, &dX));
     if (Z == X && (!dev || f32))
         dZ = dX;
     else
-        RET_IF(stage_in_t(ctx, st, ctx->d_in[1], ex->f32_in[1], Z, (size_t)m * d, dev, f32, &dZ));
+        RET_IF(stage_in_t(ctx, st, ctx->d_in[1], ctx->f32_in[1], Z, (size_t)m * d, dev, f32, &dZ));
     double* dK = K;
     int64_t ld = ldk;
     if (!dev || f32) {
@@ -485,13 +382,10 @@ extern "C" int b2gp_gram(b2gp_ctx* ctx, int kind, const double* X, int64_t n, co
     }
     const int lower = (flags & B2GP_FLAG_LOWER_ONLY) && same_xz && n == m;
     if (lower && (!dev || f32)) CUDA_TRY(ctx, cudaMemsetAsync(dK, 0, (size_t)n * ld * 8, st));
-    RET_IF(launch_gram(ctx, st, kind, dX, n, dZ, m, d, (const double*)ex->theta1.p, 1.0, 0.0, same_xz ? 1 : 0, lower, dK, ld));
-    if (f32)
-        RET_IF(store_out_f32(ctx, st, ex->f32_out[0], K, ldk, dK, ld, n, m, dev));
-    else if (!dev)
-        CUDA_TRY(ctx, cudaMemcpy2DAsync(K, (size_t)ldk * 8, dK, (size_t)ld * 8, (size_t)m * 8, (size_t)n, cudaMemcpyDeviceToHost, st));
+    RET_IF(launch_gram(ctx, st, kind, dX, n, dZ, m, d, (const double*)ctx->theta1.p, 1.0, 0.0, same_xz ? 1 : 0, lower, dK, ld));
+    RET_IF(store_out(ctx, st, ctx->f32_out[0], K, ldk, dK, ld, n, m, dev, f32));
     RET_IF(tm.end(st, nullptr));
-    ex->last.gram_bytes = 8.0 * (double)n * (double)m + 8.0 * (double)(n + m) * d;
+    ctx->last.gram_bytes = 8.0 * (double)n * (double)m + 8.0 * (double)(n + m) * d;
     return B2GP_OK;
 }
 
@@ -527,7 +421,6 @@ extern "C" int b2gp_gram_multitask(b2gp_ctx* ctx, int kind, const double* X, con
     ARG_CHECK(ctx, n >= 1 && m >= 1 && T >= 1 && group >= 1 && d >= 1 && d <= GRAM_MAX_D && ldk >= m);
     ARG_CHECK(ctx, !(flags & (B2GP_FLAG_DEVICE_PTRS | B2GP_FLAG_F32)));      // host fp64 arrays (a callable-kernel building block)
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
@@ -536,8 +429,8 @@ extern "C" int b2gp_gram_multitask(b2gp_ctx* ctx, int kind, const double* X, con
     th[d] = scale;
     th[d + 1] = 0.0;
     th[d + 2] = period;
-    RET_IF(ensure(ctx, ex->theta1, sizeof th));
-    CUDA_TRY(ctx, cudaMemcpyAsync(ex->theta1.p, th, (d + 3) * sizeof(double), cudaMemcpyHostToDevice, st));
+    RET_IF(ensure(ctx, ctx->theta1, sizeof th));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->theta1.p, th, (d + 3) * sizeof(double), cudaMemcpyHostToDevice, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     const double *dX, *dZ, *dB, *dn = nullptr, *dtx, *dtz;
     RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)n * d * 8, false, &dX));
@@ -549,10 +442,9 @@ extern "C" int b2gp_gram_multitask(b2gp_ctx* ctx, int kind, const double* X, con
     const int64_t ld = round_up(m, 2);
     RET_IF(ensure(ctx, ctx->d_out[0], (size_t)n * ld * 8));
     double* dK = (double*)ctx->d_out[0].p;
-    RET_IF(launch_gram(ctx, st, kind, dX, n, dZ, m, d, (const double*)ex->theta1.p, 0.0, 0.0, 0, 0, dK, ld));
-    mt_task_kernel<<<grid_for(n * m), 256, 0, st>>>(dK, ld, n, m, (const int*)dtx, (const int*)dtz, dB, T, dn, jitter, same_xz ? 1 : 0, group);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch_gram(ctx, st, kind, dX, n, dZ, m, d, (const double*)ctx->theta1.p, 0.0, 0.0, 0, 0, dK, ld));
+    RET_IF(launch(ctx, st, grid_for(n * m), 256, 0, mt_task_kernel, dK, ld, n, m, (const int*)dtx, (const int*)dtz, dB, T, dn, jitter,
+                  same_xz ? 1 : 0, group));
     CUDA_TRY(ctx, cudaMemcpy2DAsync(K, (size_t)ldk * 8, dK, (size_t)ld * 8, (size_t)m * 8, (size_t)n, cudaMemcpyDeviceToHost, st));
     return tm.end(st, nullptr);
 }
@@ -562,7 +454,6 @@ extern "C" int b2gp_potrf(b2gp_ctx* ctx, int64_t n, double* A, int64_t lda, int*
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, A && info && n >= 0 && lda >= n);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
@@ -573,8 +464,8 @@ extern "C" int b2gp_potrf(b2gp_ctx* ctx, int64_t n, double* A, int64_t lda, int*
     int64_t ld = lda;
     if (!dev) {
         ld = round_up(n, 2);
-        RET_IF(ensure(ctx, ex->potrf_buf, (size_t)n * ld * 8));
-        dA = (double*)ex->potrf_buf.p;
+        RET_IF(ensure(ctx, ctx->potrf_buf, (size_t)n * ld * 8));
+        dA = (double*)ctx->potrf_buf.p;
         CUDA_TRY(ctx, cudaMemcpy2DAsync(dA, (size_t)ld * 8, A, (size_t)lda * 8, (size_t)n * 8, (size_t)n, cudaMemcpyHostToDevice, st));
     }
     RET_IF(ensure(ctx, ctx->last_linv, (size_t)linv_bytes(n)));
@@ -592,8 +483,8 @@ extern "C" int b2gp_potrf(b2gp_ctx* ctx, int64_t n, double* A, int64_t lda, int*
     }
     CUDA_TRY(ctx, cudaMemcpyAsync(info, ctx->d_info.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
-    ex->last.flops = (double)n * (double)n * (double)n / 3.0;
-    ex->last.potrf_ms = ex->last.total_ms;
+    ctx->last.flops = (double)n * (double)n * (double)n / 3.0;
+    ctx->last.potrf_ms = ctx->last.total_ms;
     return B2GP_OK;
 }
 
@@ -604,7 +495,6 @@ extern "C" int b2gp_trsm_lower(b2gp_ctx* ctx, int64_t n, int64_t nrhs, const dou
     if (ctx->last_n != n || !ctx->last_linv.p)
         return set_err(ctx, B2GP_ERR_ARG, "b2gp_trsm_lower", "call b2gp_potrf on this factor first (same ctx, same n)", __FILE__, __LINE__);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
@@ -616,19 +506,19 @@ extern "C" int b2gp_trsm_lower(b2gp_ctx* ctx, int64_t n, int64_t nrhs, const dou
     if (!dev) {
         ll = round_up(n, 2);
         lb = ll;
-        RET_IF(ensure(ctx, ex->gemm_buf[0], (size_t)n * ll * 8));
-        RET_IF(ensure(ctx, ex->gemm_buf[1], (size_t)nrhs * lb * 8));
-        CUDA_TRY(ctx, cudaMemcpy2DAsync(ex->gemm_buf[0].p, (size_t)ll * 8, L, (size_t)ldl * 8, (size_t)n * 8, (size_t)n, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(ctx, cudaMemcpy2DAsync(ex->gemm_buf[1].p, (size_t)lb * 8, B, (size_t)ldb * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyHostToDevice, st));
-        dL = (const double*)ex->gemm_buf[0].p;
-        dB = (double*)ex->gemm_buf[1].p;
+        RET_IF(ensure(ctx, ctx->gemm_buf[0], (size_t)n * ll * 8));
+        RET_IF(ensure(ctx, ctx->gemm_buf[1], (size_t)nrhs * lb * 8));
+        CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->gemm_buf[0].p, (size_t)ll * 8, L, (size_t)ldl * 8, (size_t)n * 8, (size_t)n, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->gemm_buf[1].p, (size_t)lb * 8, B, (size_t)ldb * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyHostToDevice, st));
+        dL = (const double*)ctx->gemm_buf[0].p;
+        dB = (double*)ctx->gemm_buf[1].p;
     }
     RET_IF(trsm_rec(ctx, st, dB, lb, nrhs, dL, ll, n, (const double*)ctx->last_linv.p));
     if (!dev)
         CUDA_TRY(ctx, cudaMemcpy2DAsync(B, (size_t)ldb * 8, dB, (size_t)lb * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
-    ex->last.flops = (double)n * (double)n * (double)nrhs;
-    ex->last.trsm_ms = ex->last.total_ms;
+    ctx->last.flops = (double)n * (double)n * (double)nrhs;
+    ctx->last.trsm_ms = ctx->last.total_ms;
     return B2GP_OK;
 }
 
@@ -638,7 +528,6 @@ extern "C" int b2gp_gemm_nt(b2gp_ctx* ctx, int64_t m, int64_t n, int64_t k, doub
     ARG_CHECK(ctx, A && B && C && m >= 0 && n >= 0 && k >= 0 && lda >= k && ldb >= k && ldc >= n);
     ARG_CHECK(ctx, !lower_only || m >= n);   // m > n: lower triangle of the leading n x n block, all of the rows below it
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
@@ -649,15 +538,15 @@ extern "C" int b2gp_gemm_nt(b2gp_ctx* ctx, int64_t m, int64_t n, int64_t k, doub
     if (!dev) {
         la = lb = round_up(k > 0 ? k : 1, 2);
         lc = round_up(n > 0 ? n : 1, 2);
-        RET_IF(ensure(ctx, ex->gemm_buf[0], (size_t)(m + 1) * la * 8));
-        RET_IF(ensure(ctx, ex->gemm_buf[1], (size_t)(n + 1) * lb * 8));
-        RET_IF(ensure(ctx, ex->gemm_buf[2], (size_t)(m + 1) * lc * 8));
-        if (m && k) CUDA_TRY(ctx, cudaMemcpy2DAsync(ex->gemm_buf[0].p, (size_t)la * 8, A, (size_t)lda * 8, (size_t)k * 8, (size_t)m, cudaMemcpyHostToDevice, st));
-        if (n && k) CUDA_TRY(ctx, cudaMemcpy2DAsync(ex->gemm_buf[1].p, (size_t)lb * 8, B, (size_t)ldb * 8, (size_t)k * 8, (size_t)n, cudaMemcpyHostToDevice, st));
-        if (m && n) CUDA_TRY(ctx, cudaMemcpy2DAsync(ex->gemm_buf[2].p, (size_t)lc * 8, C, (size_t)ldc * 8, (size_t)n * 8, (size_t)m, cudaMemcpyHostToDevice, st));
-        dA = (const double*)ex->gemm_buf[0].p;
-        dB = (A == B && lda == ldb && m == n) ? dA : (const double*)ex->gemm_buf[1].p;
-        dC = (double*)ex->gemm_buf[2].p;
+        RET_IF(ensure(ctx, ctx->gemm_buf[0], (size_t)(m + 1) * la * 8));
+        RET_IF(ensure(ctx, ctx->gemm_buf[1], (size_t)(n + 1) * lb * 8));
+        RET_IF(ensure(ctx, ctx->gemm_buf[2], (size_t)(m + 1) * lc * 8));
+        if (m && k) CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->gemm_buf[0].p, (size_t)la * 8, A, (size_t)lda * 8, (size_t)k * 8, (size_t)m, cudaMemcpyHostToDevice, st));
+        if (n && k) CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->gemm_buf[1].p, (size_t)lb * 8, B, (size_t)ldb * 8, (size_t)k * 8, (size_t)n, cudaMemcpyHostToDevice, st));
+        if (m && n) CUDA_TRY(ctx, cudaMemcpy2DAsync(ctx->gemm_buf[2].p, (size_t)lc * 8, C, (size_t)ldc * 8, (size_t)n * 8, (size_t)m, cudaMemcpyHostToDevice, st));
+        dA = (const double*)ctx->gemm_buf[0].p;
+        dB = (A == B && lda == ldb && m == n) ? dA : (const double*)ctx->gemm_buf[1].p;
+        dC = (double*)ctx->gemm_buf[2].p;
     }
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
     RET_IF(gemm_nt(ctx, st, m, n, k, alpha, dA, la, dB, lb, beta, dC, lc, lower_only != 0));
@@ -667,8 +556,8 @@ extern "C" int b2gp_gemm_nt(b2gp_ctx* ctx, int64_t m, int64_t n, int64_t k, doub
     RET_IF(tm.end(st, nullptr));
     float ms = 0.f;
     CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
-    ex->last.epilogue_ms = ms;  // kernel-only time of the GEMM launch
-    ex->last.flops = (lower_only ? 1.0 : 2.0) * (double)m * (double)n * (double)k;
+    ctx->last.epilogue_ms = ms;  // kernel-only time of the GEMM launch
+    ctx->last.flops = (lower_only ? 1.0 : 2.0) * (double)m * (double)n * (double)k;
     return B2GP_OK;
 }
 
@@ -708,7 +597,6 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     ARG_CHECK(ctx, !want_cov || cov);
     ARG_CHECK(ctx, !want_samp || (eps && y_sampled && n_samp >= 1));
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     const bool dev = dev_ptrs(flags), f32 = f32_io(flags);
     const int nslots = (int)(S < ctx->n_streams ? S : ctx->n_streams);
     cudaStream_t st0 = ctx->slots[0].stream;
@@ -721,14 +609,14 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     const double *dXtr, *dy, *dXnew, *dtheta, *deps = nullptr, *dnv = nullptr;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st0));
     // with B2GP_FLAG_F32 the data arrays (X, y, X_new, noise_vec, eps) are floats; theta stays double
-    RET_IF(stage_in_t(ctx, st0, ctx->d_in[0], ex->f32_in[0], Xtr, (size_t)(xtr_stride ? S * xtr_stride : N * d), dev, f32, &dXtr));
-    RET_IF(stage_in_t(ctx, st0, ctx->d_in[1], ex->f32_in[1], yres, (size_t)(yres_stride ? S * yres_stride : N), dev, f32, &dy));
-    RET_IF(stage_in_t(ctx, st0, ctx->d_in[2], ex->f32_in[2], Xnew, (size_t)(xnew_stride ? S * xnew_stride : P * d), dev, f32, &dXnew));
-    if (noise_vec) RET_IF(stage_in_t(ctx, st0, ctx->d_in[6], ex->f32_in[6], noise_vec, (size_t)(nv_stride ? S * nv_stride : N), dev, f32, &dnv));
+    RET_IF(stage_in_t(ctx, st0, ctx->d_in[0], ctx->f32_in[0], Xtr, (size_t)(xtr_stride ? S * xtr_stride : N * d), dev, f32, &dXtr));
+    RET_IF(stage_in_t(ctx, st0, ctx->d_in[1], ctx->f32_in[1], yres, (size_t)(yres_stride ? S * yres_stride : N), dev, f32, &dy));
+    RET_IF(stage_in_t(ctx, st0, ctx->d_in[2], ctx->f32_in[2], Xnew, (size_t)(xnew_stride ? S * xnew_stride : P * d), dev, f32, &dXnew));
+    if (noise_vec) RET_IF(stage_in_t(ctx, st0, ctx->d_in[6], ctx->f32_in[6], noise_vec, (size_t)(nv_stride ? S * nv_stride : N), dev, f32, &dnv));
     RET_IF(stage_in(ctx, st0, ctx->d_in[3], theta, (size_t)S * nth * 8, dev, &dtheta));
-    if (want_samp) RET_IF(stage_in_t(ctx, st0, ctx->d_in[4], ex->f32_in[4], eps, (size_t)S * n_samp * P, dev, f32, &deps));
+    if (want_samp) RET_IF(stage_in_t(ctx, st0, ctx->d_in[4], ctx->f32_in[4], eps, (size_t)S * n_samp * P, dev, f32, &deps));
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st0));
-    CUDA_TRY(ctx, cudaEventRecord(ex->inputs_ready, st0));
+    CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
 
     // ---- outputs
     double *dmean = mean, *dvar = var, *dcov = cov, *dsamp = y_sampled;
@@ -762,15 +650,14 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     for (int q = 0; q < nslots; ++q) {
         Slot& sl = ctx->slots[q];
         const size_t needA = (size_t)(N + P + 1) * ldA * 8;
-        if (q == 0 && ex->fcache.valid && ex->fcache.N == N && sl.A.p && sl.A.cap < needA) {
+        if (q == 0 && ctx->fcache.valid && ctx->fcache.N == N && sl.A.p && sl.A.cap < needA) {
             // slot 0's matrix holds the cached factor and this call brings more test points than the one that made it:
             // grow the buffer AROUND the factor (a plain ensure() would free it and the reuse below would read garbage)
             DevBuf grown;
             RET_IF(ensure(ctx, grown, needA));
             CUDA_TRY(ctx, cudaMemcpyAsync(grown.p, sl.A.p, (size_t)N * ldA * 8, cudaMemcpyDeviceToDevice, st0));
             CUDA_TRY(ctx, cudaStreamSynchronize(st0));
-            free_buf(sl.A);
-            sl.A = grown;
+            sl.A = std::move(grown);
         }
         RET_IF(ensure(ctx, sl.A, needA));
         RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
@@ -779,9 +666,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         if (!want_mean) RET_IF(ensure(ctx, sl.misc, (size_t)P * 8));
     }
     // inputs and the memset of dinfo were queued on st0: order the other streams behind them
-    CUDA_TRY(ctx, cudaEventRecord(ex->inputs_ready, st0));
+    CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
     for (int q = 0; q < nslots; ++q)
-        if (slot_stream(q) != st0) CUDA_TRY(ctx, cudaStreamWaitEvent(slot_stream(q), ex->inputs_ready, 0));
+        if (slot_stream(q) != st0) CUDA_TRY(ctx, cudaStreamWaitEvent(slot_stream(q), ctx->inputs_ready, 0));
 
     // host copy of theta: the accuracy-aware digit-plane count of the int8 path is chosen per draw (oz_auto_planes)
     std::vector<double> htheta;
@@ -798,7 +685,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     std::vector<StageEvents> sev;
     if (timing) sev.resize((size_t)S);
 
-    // factor reuse (see Extra::fcache): same kind / N / d / jitter / theta / training inputs as the previous
+    // factor reuse (see b2gp_ctx::fcache): same kind / N / d / jitter / theta / training inputs as the previous
     // single-draw host-pointer call -> skip the Gram build and the factorisation
     // The cache is invalid for the whole duration of the call: any early return (allocation failure, launch error)
     // leaves it so, and it is re-validated -- together with the factor's `info` -- only after the call's work has
@@ -806,16 +693,16 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     bool reuse = false;
     const bool cacheable = (S == 1 && !dev && !noise_vec);
     if (cacheable) {
-        auto& fc = ex->fcache;
+        auto& fc = ctx->fcache;
         const size_t xbytes = (size_t)N * d * (f32 ? 4 : 8);
         reuse = fc.valid && fc.kind == kind && fc.N == N && fc.d == d && fc.jitter == jitter && fc.X.size() == xbytes &&
                 memcmp(fc.theta.data(), theta, (size_t)nth * 8) == 0 && memcmp(fc.X.data(), Xtr, xbytes) == 0;
-        if (reuse) ex->cache_hits++;
+        if (reuse) ctx->cache_hits++;
     }
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     // a cacheable call that factors by the tall-panel scheme also keeps the diagonal blocks' explicit inverses
     const bool keepU = cacheable && !reuse && use_tall(ctx, N);
-    if (keepU) RET_IF(ensure(ctx, ex->Ukeep, (size_t)ceil_div(N, (int64_t)ctx->panel) * ctx->panel * ctx->panel * 8));
+    if (keepU) RET_IF(ensure(ctx, ctx->Ukeep, (size_t)ceil_div(N, (int64_t)ctx->panel) * ctx->panel * ctx->panel * 8));
 
     // One draw's whole pipeline, queued on its slot's stream.  Returns a B2GP_* code.
     auto enqueue_draw = [&](int64_t s) -> int {
@@ -831,7 +718,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         int* inf = dinfo + s;
         int* inf2 = dinfo + S + s;
         if (timing) {
-            for (int e = 0; e < 6; ++e) sev[s].e[e] = ex->pool.get();
+            for (int e = 0; e < 6; ++e) sev[s].e[e] = ctx->pool.get();
             CUDA_TRY(ctx, cudaEventRecord(sev[s].e[0], st));
         }
         // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7
@@ -845,42 +732,35 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         if (!reuse) {
             // k_XX = kernel(X_train, X_train, params, noise, jitter)  (gp.py:269) -- lower triangle only
             RET_IF(launch_gram(ctx, st, kind, dXtr_s, N, dXtr_s, N, d, th, 1.0, jitter, 1, 1, A, ldA));
-            if (dnv) {
-                add_diag_vec_kernel<<<grid_for(N), 256, 0, st>>>(A, ldA, N, dnv + s * nv_stride);
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches++;
-            }
+            if (dnv) RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ldA, N, dnv + s * nv_stride));
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
             // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
             if (fused_solve) count_path(ctx, PATH_POTRF_TALL);
             if (fused_solve)
-                RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, P + 1, Linv, inf, 0, keepU ? (double*)ex->Ukeep.p : nullptr));
+                RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, P + 1, Linv, inf, 0, keepU ? (double*)ctx->Ukeep.p : nullptr));
             else
                 RET_IF(potrf_rec(ctx, st, A, ldA, N, Linv, inf, 0));
         } else {
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
-            CUDA_TRY(ctx, cudaMemcpyAsync(inf, &ex->fcache.info, sizeof(int), cudaMemcpyHostToDevice, st));
+            CUDA_TRY(ctx, cudaMemcpyAsync(inf, &ctx->fcache.info, sizeof(int), cudaMemcpyHostToDevice, st));
         }
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[2], st));
         if (!fused_solve) RET_IF(rhs_rows());
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[3], st));
         // [V^T; w^T] = [k_pX; y^T] L^{-T}
         if (!fused_solve) {
-            if (reuse && ex->fcache.U_nb > 0 && ex->fcache.U_nb == ctx->panel && ctx->ozaki != 0)
-                RET_IF(trsm_tall(ctx, st, Vt, ldV, P + 1, A, ldA, N, (const double*)ex->Ukeep.p, ex->fcache.U_nb));
+            if (reuse && ctx->fcache.U_nb > 0 && ctx->fcache.U_nb == ctx->panel && ctx->ozaki != 0)
+                RET_IF(trsm_tall(ctx, st, Vt, ldV, P + 1, A, ldA, N, (const double*)ctx->Ukeep.p, ctx->fcache.U_nb));
             else
                 RET_IF(trsm_rec(ctx, st, Vt, ldV, P + 1, A, ldA, N, Linv));
         }
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[4], st));
         // mean / var
         double* mean_s = want_mean ? dmean + s * P : (double*)sl.misc.p;
-        if (want_mean || want_var || want_samp) {
-            rowdot_kernel<<<(unsigned)P, RD_THREADS, 0, st>>>(Vt, ldV, N, P, kind, d, th, noise_mult_new, jitter, inf, mean_s,
-                                                           want_var ? dvar + s * P : nullptr);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches++;
-        }
+        if (want_mean || want_var || want_samp)
+            RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, kind, d, th, noise_mult_new, jitter, inf, mean_s,
+                          want_var ? dvar + s * P : nullptr));
         if (need_cov) {
             sl.oz_planes = 7;
             // cov = k_pp - V^T V  (gp.py:267, 272), lower tiles then mirrored -> exactly symmetric
@@ -889,33 +769,19 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXnew_s, P, d, th, noise_mult_new, jitter, 1, 1, C, ldc));
             RET_IF(gemm_nt(ctx, st, P, P, N, -1.0, Vt, ldV, Vt, ldV, 1.0, C, ldc, true));
             dim3 g2((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), b2(32, 32);
-            mirror_lower_kernel<<<g2, b2, 0, st>>>(C, ldc, P);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches++;
+            RET_IF(launch(ctx, st, g2, b2, 0, mirror_lower_kernel, C, ldc, P));
             if (want_samp) {
                 // y = mean + chol(cov) eps  (gp.py:292)
                 double* CL = (double*)sl.cov.p;
-                if (want_cov) {
-                    copy2d_kernel<<<grid_for(P * P), 256, 0, st>>>(CL, ldC, C, ldc, P, P);
-                    CUDA_TRY(ctx, cudaGetLastError());
-                    ctx->launches++;
-                }
+                if (want_cov) RET_IF(launch(ctx, st, grid_for(P * P), 256, 0, copy2d_kernel, CL, ldC, C, ldc, P, P));
                 RET_IF(potrf_rec(ctx, st, CL, ldC, P, (double*)sl.LinvC.p, inf2, 0));
-                zero_upper_kernel<<<g2, b2, 0, st>>>(CL, ldC, P);
+                RET_IF(launch(ctx, st, g2, b2, 0, zero_upper_kernel, CL, ldC, P));
                 double* Y = dsamp + s * n_samp * P;
-                bcast_rows_kernel<<<grid_for(n_samp * P), 256, 0, st>>>(Y, P, n_samp, P, mean_s);
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches += 2;
+                RET_IF(launch(ctx, st, grid_for(n_samp * P), 256, 0, bcast_rows_kernel, Y, P, n_samp, P, mean_s));
                 RET_IF(gemm_nt(ctx, st, n_samp, P, P, 1.0, deps + s * n_samp * P, P, CL, ldC, 1.0, Y, P, false));
-                nan_if_bad_kernel<<<grid_for(n_samp * P), 256, 0, st>>>(Y, P, n_samp, P, inf, inf2);
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches++;
+                RET_IF(launch(ctx, st, grid_for(n_samp * P), 256, 0, nan_if_bad_kernel, Y, P, n_samp, P, inf, inf2));
             }
-            if (want_cov) {
-                nan_if_bad_kernel<<<grid_for(P * P), 256, 0, st>>>(C, ldc, P, P, inf, nullptr);
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches++;
-            }
+            if (want_cov) RET_IF(launch(ctx, st, grid_for(P * P), 256, 0, nan_if_bad_kernel, C, ldc, P, P, inf, nullptr));
         }
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[5], st));
         return B2GP_OK;
@@ -943,30 +809,23 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     // ---- join the slots on stream 0
     for (int q = 0; q < nslots; ++q) {
         if (slot_stream(q) == st0) continue;
-        CUDA_TRY(ctx, cudaEventRecord(ex->slot_done[q], slot_stream(q)));
-        CUDA_TRY(ctx, cudaStreamWaitEvent(st0, ex->slot_done[q], 0));
+        CUDA_TRY(ctx, cudaEventRecord(ctx->slot_done[q], slot_stream(q)));
+        CUDA_TRY(ctx, cudaStreamWaitEvent(st0, ctx->slot_done[q], 0));
     }
     cudaEvent_t ev_c = ctx->slots[0].ev[0], ev_d = ctx->slots[0].ev[1];
     CUDA_TRY(ctx, cudaEventRecord(ev_c, st0));
     std::vector<int> hinfo((size_t)2 * S);
     CUDA_TRY(ctx, cudaMemcpyAsync(hinfo.data(), dinfo, (size_t)2 * S * sizeof(int), cudaMemcpyDeviceToHost, st0));
-    if (f32) {
-        if (want_mean) RET_IF(store_out_f32(ctx, st0, ex->f32_out[0], mean, P, dmean, P, S, P, dev));
-        if (want_var) RET_IF(store_out_f32(ctx, st0, ex->f32_out[1], var, P, dvar, P, S, P, dev));
-        if (want_cov) RET_IF(store_out_f32(ctx, st0, ex->f32_out[2], cov, P, dcov, P, S * P, P, dev));
-        if (want_samp) RET_IF(store_out_f32(ctx, st0, ex->f32_out[3], y_sampled, P, dsamp, P, S * n_samp, P, dev));
-    } else if (!dev) {
-        if (want_mean) CUDA_TRY(ctx, cudaMemcpyAsync(mean, dmean, (size_t)S * P * 8, cudaMemcpyDeviceToHost, st0));
-        if (want_var) CUDA_TRY(ctx, cudaMemcpyAsync(var, dvar, (size_t)S * P * 8, cudaMemcpyDeviceToHost, st0));
-        if (want_cov) CUDA_TRY(ctx, cudaMemcpyAsync(cov, dcov, (size_t)S * P * P * 8, cudaMemcpyDeviceToHost, st0));
-        if (want_samp) CUDA_TRY(ctx, cudaMemcpyAsync(y_sampled, dsamp, (size_t)S * n_samp * P * 8, cudaMemcpyDeviceToHost, st0));
-    }
+    if (want_mean) RET_IF(store_out(ctx, st0, ctx->f32_out[0], mean, P, dmean, P, S, P, dev, f32));
+    if (want_var) RET_IF(store_out(ctx, st0, ctx->f32_out[1], var, P, dvar, P, S, P, dev, f32));
+    if (want_cov) RET_IF(store_out(ctx, st0, ctx->f32_out[2], cov, P, dcov, P, S * P, P, dev, f32));
+    if (want_samp) RET_IF(store_out(ctx, st0, ctx->f32_out[3], y_sampled, P, dsamp, P, S * n_samp, P, dev, f32));
     CUDA_TRY(ctx, cudaEventRecord(ev_d, st0));
     RET_IF(tm.end(st0, nullptr));
     for (int q = 0; q < B2GP_MAX_STREAMS; ++q) ctx->slots[q].oz_planes = 7;   // other entry points: the conservative count
     for (int64_t s = 0; s < S; ++s) info[s] = hinfo[s] != 0 ? hinfo[s] : -hinfo[S + s];
     if (cacheable) {
-        auto& fc = ex->fcache;
+        auto& fc = ctx->fcache;
         if (!reuse) {
             fc.kind = kind;
             fc.N = N;
@@ -980,7 +839,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         fc.valid = true;
     }
 
-    b2gp_timing& t = ex->last;
+    b2gp_timing& t = ctx->last;
     float ms = 0.f;
     CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
     t.h2d_ms = ms;
@@ -1111,22 +970,14 @@ static int sparse_partial_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* d
     // W^T = K_fu Luu^{-T}  (W = Luu^{-1} Kuf, sparse_gp.py:195-197), one training point per row
     RET_IF(launch_gram(ctx, st, kind, dXtr, N, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wt, ldM));
     RET_IF(trsm_rec(ctx, st, Wt, ldM, N, Luu, ldM, M, LinvU));   // tall right-hand sides: int8 panel GEMMs (potrf.cuh)
-    {
-        dim3 g((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), b(32, 8);
-        transpose_kernel<<<g, b, 0, st>>>(W, ldN, Wt, ldM, N, M);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches++;
-    }
+    RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), dim3(32, 8), 0, transpose_kernel, W, ldN, Wt, ldM, N, M));
     // W D^{-1} W^T with D = noise * 1  (sparse_gp.py:198-199).  Accumulated onto a zeroed matrix (beta = 1) so that the
     // product -- M^2 N flops, the bulk of the sparse posterior -- qualifies for the int8 wgmma path (k = N is split into
     // launches of <= 16384 by the dispatcher)
     CUDA_TRY(ctx, cudaMemsetAsync(Kpart, 0, (size_t)M * ldk * 8, st));
     RET_IF(gemm_nt(ctx, st, M, M, N, 1.0 / noise_h, W, ldN, W, ldN, 1.0, Kpart, ldk, true));
     // W D^{-1} y  (sparse_gp.py:203-204)
-    rowdot2_kernel<<<(unsigned)M, RD_THREADS, 0, st>>>(W, ldN, N, dy, 1.0 / noise_h, cpart, nullptr);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    return B2GP_OK;
+    return launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, dy, 1.0 / noise_h, cpart, nullptr);
 }
 
 // Posterior from the summed statistics: K = Ksum + I, L = chol(K), then sparse_gp.py:206-217.
@@ -1141,35 +992,27 @@ static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dX
     double* R = Wst + (P + 1) * ldM;            // (P+1) x ldM      rows 0..P-1: (L^{-1} Ws)^T; row P: L^{-1} c
     double* qv = (double*)sl.misc.p;            // |Ws^T[p]|^2
     double* rv = qv + P;                        // |R[p]|^2
-    add_diag_kernel<<<grid_for(M), 256, 0, st>>>(Kmat, ldk, M, 1.0);                            // sparse_gp.py:200
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch(ctx, st, grid_for(M), 256, 0, add_diag_kernel, Kmat, ldk, M, 1.0));           // sparse_gp.py:200
     RET_IF(potrf_auto(ctx, st, Kmat, ldk, M, 0, LinvK, dinfo + 1));                             // sparse_gp.py:201
     // Ws^T = K_su Luu^{-T}  (sparse_gp.py:206-207)
     RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wst, ldM));
     RET_IF(trsm_rec(ctx, st, Wst, ldM, P, Luu, ldM, M, LinvU));
     // pack = [c | Ws]; L^{-1} pack  (sparse_gp.py:208-212)
-    copy2d_kernel<<<grid_for(P * M), 256, 0, st>>>(R, ldM, Wst, ldM, P, M);
+    RET_IF(launch(ctx, st, grid_for(P * M), 256, 0, copy2d_kernel, R, ldM, Wst, ldM, P, M));
     CUDA_TRY(ctx, cudaMemcpyAsync(R + P * ldM, cvec, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
-    ctx->launches++;
     RET_IF(trsm_rec(ctx, st, R, ldM, P + 1, Kmat, ldk, M, LinvK));
     // mean = (L^{-1} c)^T (L^{-1} Ws)  (sparse_gp.py:213)
-    rowdot2_kernel<<<(unsigned)P, RD_THREADS, 0, st>>>(R, ldM, M, R + P * ldM, 1.0, dmean, rv);
-    rowdot2_kernel<<<(unsigned)P, RD_THREADS, 0, st>>>(Wst, ldM, M, nullptr, 1.0, nullptr, qv);
-    sparse_var_kernel<<<grid_for(P), 256, 0, st>>>(want_var ? dvar : nullptr, dmean, qv, rv, P, kind, d, dth,
-                                                   noiseless ? 0.0 : 1.0, jitter, dinfo, dinfo + 1);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 3;
+    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, R, ldM, M, R + P * ldM, 1.0, dmean, rv));
+    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, Wst, ldM, M, nullptr, 1.0, nullptr, qv));
+    RET_IF(launch(ctx, st, grid_for(P), 256, 0, sparse_var_kernel, want_var ? dvar : nullptr, dmean, qv, rv, P, kind, d, dth,
+                  noiseless ? 0.0 : 1.0, jitter, dinfo, dinfo + 1));
     if (want_cov) {
         // cov = Kss - Ws^T Ws + (L^{-1}Ws)^T (L^{-1}Ws)  (sparse_gp.py:215-217)
         RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXnew, P, d, dth, noiseless ? 0.0 : 1.0, jitter, 1, 1, C, ldc));
         RET_IF(gemm_nt(ctx, st, P, P, M, -1.0, Wst, ldM, Wst, ldM, 1.0, C, ldc, true));
         RET_IF(gemm_nt(ctx, st, P, P, M, 1.0, R, ldM, R, ldM, 1.0, C, ldc, true));
-        dim3 g2((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), b2(32, 32);
-        mirror_lower_kernel<<<g2, b2, 0, st>>>(C, ldc, P);
-        nan_if_bad_kernel<<<grid_for(P * P), 256, 0, st>>>(C, ldc, P, P, dinfo, dinfo + 1);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 2;
+        RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), dim3(32, 32), 0, mirror_lower_kernel, C, ldc, P));
+        RET_IF(launch(ctx, st, grid_for(P * P), 256, 0, nan_if_bad_kernel, C, ldc, P, P, dinfo, dinfo + 1));
     }
     return B2GP_OK;
 }
@@ -1187,20 +1030,19 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
     ARG_CHECK(ctx, !want_var || var);
     ARG_CHECK(ctx, !want_cov || cov);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
     const bool dev = dev_ptrs(flags), f32 = f32_io(flags);
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream;
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
     const int nth = d + 3;
     const double *dXu, *dXtr, *dy, *dXnew, *dth;
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ex->f32_in[0], Xtr, (size_t)N * d, dev, f32, &dXtr));
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[1], ex->f32_in[1], yres, (size_t)N, dev, f32, &dy));
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[2], ex->f32_in[2], Xnew, (size_t)P * d, dev, f32, &dXnew));
+    RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ctx->f32_in[0], Xtr, (size_t)N * d, dev, f32, &dXtr));
+    RET_IF(stage_in_t(ctx, st, ctx->d_in[1], ctx->f32_in[1], yres, (size_t)N, dev, f32, &dy));
+    RET_IF(stage_in_t(ctx, st, ctx->d_in[2], ctx->f32_in[2], Xnew, (size_t)P * d, dev, f32, &dXnew));
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, dev, &dth));
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[5], ex->f32_in[5], Xu, (size_t)M * d, dev, f32, &dXu));
+    RET_IF(stage_in_t(ctx, st, ctx->d_in[5], ctx->f32_in[5], Xu, (size_t)M * d, dev, f32, &dXu));
     double noise_h = 0.0;
     if (dev) {
         CUDA_TRY(ctx, cudaMemcpyAsync(&noise_h, dth + d + 1, 8, cudaMemcpyDeviceToHost, st));
@@ -1231,25 +1073,17 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
     const int64_t ldc = direct ? P : ldC;
     RET_IF(sparse_finish_dev(ctx, sl, kind, dXu, M, Luu, ldM, LinvU, Kmat, ldM, LinvK, cvec, dXnew, P, d, dth, noiseless, jitter,
                              want_var, want_cov, dmean, dvar, C, ldc, dinfo));
-    if (want_cov && f32)
-        RET_IF(store_out_f32(ctx, st, ex->f32_out[2], cov, P, C, ldc, P, P, dev));
-    else if (want_cov && !dev)
-        CUDA_TRY(ctx, cudaMemcpy2DAsync(cov, (size_t)P * 8, C, (size_t)ldc * 8, (size_t)P * 8, (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (want_cov) RET_IF(store_out(ctx, st, ctx->f32_out[2], cov, P, C, ldc, P, P, dev, f32));
     int hinfo[2] = {0, 0};
     CUDA_TRY(ctx, cudaMemcpyAsync(hinfo, dinfo, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    if (f32) {
-        if (want_mean) RET_IF(store_out_f32(ctx, st, ex->f32_out[0], mean, P, dmean, P, 1, P, dev));
-        if (want_var) RET_IF(store_out_f32(ctx, st, ex->f32_out[1], var, P, dvar, P, 1, P, dev));
-    } else if (!dev) {
-        if (want_mean) CUDA_TRY(ctx, cudaMemcpyAsync(mean, dmean, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
-        if (want_var) CUDA_TRY(ctx, cudaMemcpyAsync(var, dvar, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
-    }
+    if (want_mean) RET_IF(store_out(ctx, st, ctx->f32_out[0], mean, P, dmean, P, 1, P, dev, f32));
+    if (want_var) RET_IF(store_out(ctx, st, ctx->f32_out[1], var, P, dvar, P, 1, P, dev, f32));
     RET_IF(tm.end(st, nullptr));
     info[0] = hinfo[0] != 0 ? hinfo[0] : -hinfo[1];
     const double m = (double)M, n = (double)N, p = (double)P;
-    ex->last.flops = 2.0 * m * m * m / 3.0 + 2.0 * m * m * n + 2.0 * m * m * (p + 1.0) + (want_cov ? 2.0 * m * p * p : 0.0);
-    ex->last.gram_bytes = 8.0 * (m * n + m * m / 2.0 + m * p);
-    if (timing) *timing = ex->last;
+    ctx->last.flops = 2.0 * m * m * m / 3.0 + 2.0 * m * m * n + 2.0 * m * m * (p + 1.0) + (want_cov ? 2.0 * m * p * p : 0.0);
+    ctx->last.gram_bytes = 8.0 * (m * n + m * m / 2.0 + m * p);
+    if (timing) *timing = ctx->last;
     return B2GP_OK;
 }
 
@@ -1264,7 +1098,7 @@ extern "C" int b2gp_sparse_partial(b2gp_ctx* ctx, int kind, const double* Xu, in
     ARG_CHECK(ctx, Xu && Xtr && yres && theta && Kpart && cpart && info);
     ARG_CHECK(ctx, M >= 1 && N >= 1 && d >= 1 && d <= GRAM_MAX_D && ldk >= M);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    extra_of(ctx)->fcache.valid = false;
+    ctx->fcache.valid = false;
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream;
     CallTimer tm(ctx);
@@ -1294,7 +1128,7 @@ extern "C" int b2gp_sparse_finish(b2gp_ctx* ctx, int kind, const double* Xu, int
     ARG_CHECK(ctx, !want_var || var);
     ARG_CHECK(ctx, !want_cov || cov);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    extra_of(ctx)->fcache.valid = false;
+    ctx->fcache.valid = false;
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream;
     CallTimer tm(ctx);
@@ -1368,11 +1202,9 @@ extern "C" int b2gp_rowdot(b2gp_ctx* ctx, int64_t rows, int64_t len, const doubl
         RET_IF(ensure(ctx, ctx->slots[0].misc, (size_t)(2 * rows + 16) * 8));
         double* t1 = (double*)ctx->slots[0].misc.p;
         double* t2 = t1 + rows;
-        rowdot2_kernel<<<(unsigned)rows, RD_THREADS, 0, st>>>(R, ldr, len, w, scale, dot ? t1 : nullptr, nrm ? t2 : nullptr);
-        if (dot) accumulate_kernel<<<grid_for(rows), 256, 0, st>>>(dot, t1, rows, accumulate);
-        if (nrm) accumulate_kernel<<<grid_for(rows), 256, 0, st>>>(nrm, t2, rows, accumulate);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 3;
+        RET_IF(launch(ctx, st, (unsigned)rows, RD_THREADS, 0, rowdot2_kernel, R, ldr, len, w, scale, dot ? t1 : nullptr, nrm ? t2 : nullptr));
+        if (dot) RET_IF(launch(ctx, st, grid_for(rows), 256, 0, accumulate_kernel, dot, t1, rows, accumulate));
+        if (nrm) RET_IF(launch(ctx, st, grid_for(rows), 256, 0, accumulate_kernel, nrm, t2, rows, accumulate));
     }
     return tm.end(st, nullptr);
 }
@@ -1409,8 +1241,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     ARG_CHECK(ctx, X && yres && theta && value && info);
     ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= MLL_MAX_D);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     const bool dev = dev_ptrs(flags);
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream;
@@ -1437,44 +1268,32 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     double* sc = alpha + ld;             // [0] sum log L_ii, [1] |w|^2, [8..8+nth) grad
     double* partial = sc + 64;
     RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, dth, 1.0, jitter, 1, 1, A, ld));
-    if (dnv) {   // k + diag(measured_noise) / k + diag(exp(log_var)): mngp.py:96, hskgp.py:147
-        add_diag_vec_kernel<<<grid_for(N), 256, 0, st>>>(A, ld, N, dnv);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches++;
-    }
+    if (dnv)   // k + diag(measured_noise) / k + diag(exp(log_var)): mngp.py:96, hskgp.py:147
+        RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ld, N, dnv));
     CUDA_TRY(ctx, cudaMemcpyAsync(w, dy, (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
     // the scheme of the posterior (tall-panel int8 at N >= 2048); w = L^{-1} y falls out of the panel solves instead of
     // a separate chain of 2 N / 128 strip launches for one row
     RET_IF(potrf_auto(ctx, st, A, ld, N, 1, Linv, dinfo));
-    logdiag_kernel<<<1, 256, 0, st>>>(A, ld, N, sc);
-    rowdot2_kernel<<<1, RD_THREADS, 0, st>>>(w, ld, N, nullptr, 1.0, nullptr, sc + 1);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 2;
+    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, A, ld, N, sc));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, w, ld, N, nullptr, 1.0, nullptr, sc + 1));
     if (grad || alpha_out) {
         RET_IF(ensure(ctx, sl.cov, (size_t)N * ld * 8));
         double* Bt = (double*)sl.cov.p;  // (L^{-1})^T
-        set_identity_kernel<<<grid_for(N * N), 256, 0, st>>>(Bt, ld, N);
-        CUDA_TRY(ctx, cudaGetLastError());
+        RET_IF(launch(ctx, st, grid_for(N * N), 256, 0, set_identity_kernel, Bt, ld, N));
         RET_IF(trsm_rec(ctx, st, Bt, ld, N, A, ld, N, Linv));
         // alpha = L^{-T} w : alpha_i = <Bt[i,:], w>
-        rowdot2_kernel<<<(unsigned)N, RD_THREADS, 0, st>>>(Bt, ld, N, w, 1.0, alpha, nullptr);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 2;
+        RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Bt, ld, N, w, 1.0, alpha, nullptr));
         if (grad) {
             RET_IF(ensure(ctx, sl.Vt, (size_t)N * ld * 8));
             double* Kinv = (double*)sl.Vt.p;
             // K^{-1} = L^{-T} L^{-1} accumulated onto zeros: beta = 1 is what the int8 tensor-core path takes (7 planes here)
             CUDA_TRY(ctx, cudaMemsetAsync(Kinv, 0, (size_t)N * ld * 8, st));
             RET_IF(gemm_nt(ctx, st, N, N, N, 1.0, Bt, ld, Bt, ld, 1.0, Kinv, ld, true));
-            dim3 g((unsigned)tiles, (unsigned)tiles);
-            mll_grad_kernel<<<g, MLL_THREADS, 0, st>>>(dX, N, d, kind, dth, alpha, Kinv, ld, partial);
-            mll_finish_kernel<<<1, 32, 0, st>>>(partial, tiles * tiles, nth, sc + 8);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches += 2;
+            RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv, ld,
+                          partial));
+            RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8));
             if (grad_noise_vec) {
-                mll_diag_grad_kernel<<<grid_for(N), 256, 0, st>>>(alpha, Kinv, ld, N, w);   // w is free again
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches++;
+                RET_IF(launch(ctx, st, grid_for(N), 256, 0, mll_diag_grad_kernel, alpha, Kinv, ld, N, w));   // w is free again
                 CUDA_TRY(ctx, cudaMemcpyAsync(grad_noise_vec, w, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
             }
         }
@@ -1494,7 +1313,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
         if (grad_noise_vec)
             for (int64_t i = 0; i < N; ++i) grad_noise_vec[i] = NAN;
     }
-    ex->last.flops = (double)N * N * N * (grad ? 1.0 / 3 + 1.0 + 1.0 : 1.0 / 3);
+    ctx->last.flops = (double)N * N * N * (grad ? 1.0 / 3 + 1.0 + 1.0 : 1.0 / 3);
     return B2GP_OK;
 }
 
@@ -1519,8 +1338,7 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     ARG_CHECK(ctx, Xu && X && yres && theta && value && grad_theta && grad_Xu && info);
     ARG_CHECK(ctx, M >= 1 && N >= 1 && d >= 1 && d <= MLL_MAX_D);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     const bool dev = dev_ptrs(flags);
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream;
@@ -1537,21 +1355,21 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(ensure(ctx, sl.A, (size_t)2 * M * ldM * 8));
     RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
     RET_IF(ensure(ctx, ctx->d_info, 64));
-    for (int i = 0; i < 6; ++i) RET_IF(ensure(ctx, ex->eb[i], (size_t)M * ldM * 8));
-    RET_IF(ensure(ctx, ex->eb[6], (size_t)N * ldM * 8));
-    RET_IF(ensure(ctx, ex->eb[7], (size_t)N * ldM * 8));
-    RET_IF(ensure(ctx, ex->eb[8], (size_t)M * ldN * 8));
-    RET_IF(ensure(ctx, ex->eb[9], (size_t)(4 * ldM + 3 * ldN + 64 + M * (nth + d)) * 8));
+    for (int i = 0; i < 6; ++i) RET_IF(ensure(ctx, ctx->eb[i], (size_t)M * ldM * 8));
+    RET_IF(ensure(ctx, ctx->eb[6], (size_t)N * ldM * 8));
+    RET_IF(ensure(ctx, ctx->eb[7], (size_t)N * ldM * 8));
+    RET_IF(ensure(ctx, ctx->eb[8], (size_t)M * ldN * 8));
+    RET_IF(ensure(ctx, ctx->eb[9], (size_t)(4 * ldM + 3 * ldN + 64 + M * (nth + d)) * 8));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
     double* Luu = (double*)sl.A.p;
     double* Cm = Luu + M * ldM;
     double* LinvU = (double*)sl.Linv.p;
     double* LinvC = LinvU + linv_bytes(M) / 8;
-    double *BtU = (double*)ex->eb[0].p, *BtC = (double*)ex->eb[1].p, *Cinv = (double*)ex->eb[2].p;
-    double *T1 = (double*)ex->eb[3].p, *T2 = (double*)ex->eb[4].p, *T3 = (double*)ex->eb[5].p;
-    double *E = (double*)ex->eb[6].p, *GKuft = (double*)ex->eb[7].p, *GKuf = (double*)ex->eb[8].p;
-    double* vec = (double*)ex->eb[9].p;
+    double *BtU = (double*)ctx->eb[0].p, *BtC = (double*)ctx->eb[1].p, *Cinv = (double*)ctx->eb[2].p;
+    double *T1 = (double*)ctx->eb[3].p, *T2 = (double*)ctx->eb[4].p, *T3 = (double*)ctx->eb[5].p;
+    double *E = (double*)ctx->eb[6].p, *GKuft = (double*)ctx->eb[7].p, *GKuf = (double*)ctx->eb[8].p;
+    double* vec = (double*)ctx->eb[9].p;
     double *bvec = vec, *u = vec + ldM, *beta = vec + 2 * ldM, *tmpM = vec + 3 * ldM;
     double *tmpN = vec + 4 * ldM, *alpha = tmpN + ldN, *tmpN2 = alpha + ldN;
     double* scal = tmpN2 + ldN;          // [0] sum log LC_ii, [1] u'u, [2] y'y, [3] |W|_F^2, [4] tr(C^-1), [5] alpha'alpha, [8..] chain
@@ -1563,28 +1381,26 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(sparse_partial_dev(ctx, sl, kind, dXu, M, dX, N, dy, d, dth, jitter, noise, Luu, ldM, LinvU, Cm, ldM, bvec, dinfo));
     double* Wt = (double*)sl.Vt.p;
     double* W = (double*)sl.cov.p;
-    add_diag_kernel<<<grid_for(M), 256, 0, st>>>(Cm, ldM, M, 1.0);
+    RET_IF(launch(ctx, st, grid_for(M), 256, 0, add_diag_kernel, Cm, ldM, M, 1.0));
     RET_IF(potrf_rec(ctx, st, Cm, ldM, M, LinvC, dinfo + 1, 0));
     CUDA_TRY(ctx, cudaMemcpyAsync(u, bvec, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
     RET_IF(trsm_rec(ctx, st, u, ldM, 1, Cm, ldM, M, LinvC));
-    logdiag_kernel<<<1, 256, 0, st>>>(Cm, ldM, M, scal + 0);
-    rowdot2_kernel<<<1, RD_THREADS, 0, st>>>(u, ldM, M, nullptr, 1.0, nullptr, scal + 1);
-    rowdot2_kernel<<<1, RD_THREADS, 0, st>>>(dy, ldN, N, nullptr, 1.0, nullptr, scal + 2);
-    rowdot2_kernel<<<(unsigned)M, RD_THREADS, 0, st>>>(W, ldN, N, nullptr, 1.0, nullptr, tmpM);
-    vecsum_kernel<<<1, 256, 0, st>>>(tmpM, M, scal + 3);
+    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, Cm, ldM, M, scal + 0));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, u, ldM, M, nullptr, 1.0, nullptr, scal + 1));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, dy, ldN, N, nullptr, 1.0, nullptr, scal + 2));
+    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, nullptr, 1.0, nullptr, tmpM));
+    RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 3));
     // C^{-1} = BtC BtC^T with BtC = (LC^{-1})^T, beta = C^{-1} b
-    set_identity_kernel<<<grid_for(M * M), 256, 0, st>>>(BtC, ldM, M);
+    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtC, ldM, M));
     RET_IF(trsm_rec(ctx, st, BtC, ldM, M, Cm, ldM, M, LinvC));
-    rowdot2_kernel<<<(unsigned)M, RD_THREADS, 0, st>>>(BtC, ldM, M, u, 1.0, beta, tmpM);
-    vecsum_kernel<<<1, 256, 0, st>>>(tmpM, M, scal + 4);
+    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, BtC, ldM, M, u, 1.0, beta, tmpM));
+    RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 4));
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtC, ldM, BtC, ldM, 0.0, Cinv, ldM, true));
-    mirror_lower_kernel<<<gMM, b32, 0, st>>>(Cinv, ldM, M);
+    RET_IF(launch(ctx, st, gMM, b32, 0, mirror_lower_kernel, Cinv, ldM, M));
     // alpha = (y - W^T beta) / noise
-    rowdot2_kernel<<<(unsigned)N, RD_THREADS, 0, st>>>(Wt, ldM, M, beta, 1.0, tmpN, nullptr);
-    elbo_alpha_kernel<<<grid_for(N), 256, 0, st>>>(alpha, dy, tmpN, N, noise);
-    rowdot2_kernel<<<1, RD_THREADS, 0, st>>>(alpha, ldN, N, nullptr, 1.0, nullptr, scal + 5);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 14;
+    RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Wt, ldM, M, beta, 1.0, tmpN, nullptr));
+    RET_IF(launch(ctx, st, grid_for(N), 256, 0, elbo_alpha_kernel, alpha, dy, tmpN, N, noise));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, alpha, ldN, N, nullptr, 1.0, nullptr, scal + 5));
     // the clip of the trace term decides a coefficient of the reverse pass: fetch the scalars now
     double hs[8];
     CUDA_TRY(ctx, cudaMemcpyAsync(hs, scal, sizeof hs, cudaMemcpyDeviceToHost, st));
@@ -1598,34 +1414,27 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     const double coef = (T > 0.0) ? 1.0 : 0.0;
     // dELBO/dW^T = alpha beta^T + (coef W^T - W^T C^{-1}) / noise
     RET_IF(gemm_nt(ctx, st, N, M, M, 1.0, Wt, ldM, Cinv, ldM, 0.0, E, ldM, false));
-    elbo_gw_kernel<<<grid_for(N * M), 256, 0, st>>>(E, ldM, Wt, ldM, alpha, beta, N, M, coef, noise);
+    RET_IF(launch(ctx, st, grid_for(N * M), 256, 0, elbo_gw_kernel, E, ldM, Wt, ldM, alpha, beta, N, M, coef, noise));
     // dELBO/dKuf^T = (dELBO/dW^T) Luu^{-1}
-    set_identity_kernel<<<grid_for(M * M), 256, 0, st>>>(BtU, ldM, M);
+    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtU, ldM, M));
     RET_IF(trsm_rec(ctx, st, BtU, ldM, M, Luu, ldM, M, LinvU));
     RET_IF(gemm_nt(ctx, st, N, M, M, 1.0, E, ldM, BtU, ldM, 0.0, GKuft, ldM, false));
-    {
-        dim3 g((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), b(32, 8);
-        transpose_kernel<<<g, b, 0, st>>>(GKuf, ldN, GKuft, ldM, N, M);
-    }
+    RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), dim3(32, 8), 0, transpose_kernel, GKuf, ldN, GKuft, ldM,
+                  N, M));
     // H^T = W G_Kuf^T; G_L = -tril(H); dELBO/dKuu = Luu^{-T} Phi(Luu^T G_L) Luu^{-1}
     RET_IF(gemm_nt(ctx, st, M, M, N, 1.0, W, ldN, GKuf, ldN, 0.0, T1, ldM, false));
-    tri_kernel<<<gMM, b32, 0, st>>>(T2, ldM, T1, ldM, M, 1);              // T2 = G_L^T = -triu(H^T)
-    tri_kernel<<<gMM, b32, 0, st>>>(T3, ldM, Luu, ldM, M, 0);             // T3 = tril(Luu)
-    {
-        dim3 b(32, 8);
-        transpose_kernel<<<gMM, b, 0, st>>>(T1, ldM, T3, ldM, M, M);      // T1 = Luu^T
-    }
+    RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T2, ldM, T1, ldM, M, 1));                  // T2 = G_L^T = -triu(H^T)
+    RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T3, ldM, Luu, ldM, M, 0));                 // T3 = tril(Luu)
+    RET_IF(launch(ctx, st, gMM, dim3(32, 8), 0, transpose_kernel, T1, ldM, T3, ldM, M, M));    // T1 = Luu^T
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, T1, ldM, T2, ldM, 0.0, T3, ldM, false));   // T3 = Luu^T G_L
-    tri_kernel<<<gMM, b32, 0, st>>>(T2, ldM, T3, ldM, M, 2);              // T2 = Phi(.)
+    RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T2, ldM, T3, ldM, M, 2));                  // T2 = Phi(.)
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtU, ldM, T2, ldM, 0.0, T1, ldM, false));  // T1 = BtU P^T
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtU, ldM, T1, ldM, 0.0, T3, ldM, false));  // T3 = dELBO/dKuu
-    tri_kernel<<<gMM, b32, 0, st>>>(T2, ldM, T3, ldM, M, 3);              // T2 = T3 + T3^T
+    RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T2, ldM, T3, ldM, M, 3));                  // T2 = T3 + T3^T
     // contract with the kernel derivatives
-    elbo_chain_kernel<<<(unsigned)M, 256, 0, st>>>(kind, d, dth, dXu, (int)M, dX, N, GKuf, ldN, GKuf, ldN, 0, 0, partial, gXu);
-    elbo_chain_kernel<<<(unsigned)M, 256, 0, st>>>(kind, d, dth, dXu, (int)M, dXu, M, T3, ldM, T2, ldM, 1, 1, partial, gXu);
-    colsum_kernel<<<1, 32, 0, st>>>(partial, M, nth, scal + 8);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 12;
+    RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dX, N, GKuf, ldN, GKuf, ldN, 0, 0, partial, gXu));
+    RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dXu, M, T3, ldM, T2, ldM, 1, 1, partial, gXu));
+    RET_IF(launch(ctx, st, 1, 32, 0, colsum_kernel, partial, M, nth, scal + 8));
     double hs2[8 + MLL_MAX_D + 3];
     int hinfo[2] = {0, 0};
     CUDA_TRY(ctx, cudaMemcpyAsync(hs2, scal, sizeof hs2, cudaMemcpyDeviceToHost, st));
@@ -1679,17 +1488,13 @@ extern "C" int b2gp_mvn_sample(b2gp_ctx* ctx, const double* mean, const double* 
     double* CL = (double*)sl.cov.p;
     dim3 g2((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), b2(32, 32);
     for (int64_t s = 0; s < S; ++s) {
-        copy2d_kernel<<<grid_for(P * P), 256, 0, st>>>(CL, ldC, dcov + s * P * P, P, P, P);
+        RET_IF(launch(ctx, st, grid_for(P * P), 256, 0, copy2d_kernel, CL, ldC, dcov + s * P * P, P, P, P));
         RET_IF(potrf_rec(ctx, st, CL, ldC, P, (double*)sl.LinvC.p, dinfo + s, 0));
-        zero_upper_kernel<<<g2, b2, 0, st>>>(CL, ldC, P);
+        RET_IF(launch(ctx, st, g2, b2, 0, zero_upper_kernel, CL, ldC, P));
         double* Y = dy + s * n * P;
-        bcast_rows_kernel<<<grid_for(n * P), 256, 0, st>>>(Y, P, n, P, dmean + s * P);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches += 3;
+        RET_IF(launch(ctx, st, grid_for(n * P), 256, 0, bcast_rows_kernel, Y, P, n, P, dmean + s * P));
         RET_IF(gemm_nt(ctx, st, n, P, P, 1.0, deps + s * n * P, P, CL, ldC, 1.0, Y, P, false));
-        nan_if_bad_kernel<<<grid_for(n * P), 256, 0, st>>>(Y, P, n, P, dinfo + s, nullptr);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches++;
+        RET_IF(launch(ctx, st, grid_for(n * P), 256, 0, nan_if_bad_kernel, Y, P, n, P, dinfo + s, nullptr));
     }
     CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, (size_t)S * sizeof(int), cudaMemcpyDeviceToHost, st));
     if (!dev) CUDA_TRY(ctx, cudaMemcpyAsync(y, dy, (size_t)S * n * P * 8, cudaMemcpyDeviceToHost, st));
@@ -1725,13 +1530,10 @@ extern "C" int b2gp_acq_moments(b2gp_ctx* ctx, int kind, const double* mean, con
             CUDA_TRY(ctx, cudaMemcpyAsync(dbest, hb.data(), (size_t)R * 8, cudaMemcpyHostToDevice, st));
             CUDA_TRY(ctx, cudaStreamSynchronize(st));
         } else {
-            acq_best_kernel<<<(unsigned)R, 256, 0, st>>>(dmean, P, P, maximize, dbest);
-            ctx->launches++;
+            RET_IF(launch(ctx, st, (unsigned)R, 256, 0, acq_best_kernel, dmean, P, P, maximize, dbest));
         }
     }
-    acq_moments_kernel<<<grid_for(R * P), 256, 0, st>>>(kind, dmean, dvar, P, R, P, dbest, param, maximize, dout, P);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch(ctx, st, grid_for(R * P), 256, 0, acq_moments_kernel, kind, dmean, dvar, P, R, P, dbest, param, maximize, dout, P));
     if (!dev) CUDA_TRY(ctx, cudaMemcpyAsync(out, dout, (size_t)R * P * 8, cudaMemcpyDeviceToHost, st));
     return tm.end(st, nullptr);
 }
@@ -1754,20 +1556,16 @@ extern "C" int b2gp_acq_samples(b2gp_ctx* ctx, int kind, const double* y, int64_
     double* dout = dev ? out : dv + P;
     RET_IF(ensure(ctx, ctx->slots[0].misc, 16 * 8));
     double* dbest = (double*)ctx->slots[0].misc.p;
-    sample_moments_kernel<<<(unsigned)ceil_div(P, 128), 128, 0, st>>>(dy, R, P, dm, dv);
-    ctx->launches++;
+    RET_IF(launch(ctx, st, (unsigned)ceil_div(P, 128), 128, 0, sample_moments_kernel, dy, R, P, dm, dv));
     if (kind == ACQ_EI || kind == ACQ_POI) {
         if (have_best) {
             CUDA_TRY(ctx, cudaMemcpyAsync(dbest, &best_f, 8, cudaMemcpyHostToDevice, st));
             CUDA_TRY(ctx, cudaStreamSynchronize(st));
         } else {
-            acq_best_kernel<<<1, 256, 0, st>>>(dm, P, P, maximize, dbest);
-            ctx->launches++;
+            RET_IF(launch(ctx, st, 1, 256, 0, acq_best_kernel, dm, P, P, maximize, dbest));
         }
     }
-    acq_moments_kernel<<<grid_for(P), 256, 0, st>>>(kind, dm, dv, P, 1, P, dbest, param, maximize, dout, P);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
+    RET_IF(launch(ctx, st, grid_for(P), 256, 0, acq_moments_kernel, kind, dm, dv, P, 1, P, dbest, param, maximize, dout, P));
     const cudaMemcpyKind kd = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (!dev) CUDA_TRY(ctx, cudaMemcpyAsync(out, dout, (size_t)P * 8, kd, st));
     if (mean_out) CUDA_TRY(ctx, cudaMemcpyAsync(mean_out, dm, (size_t)P * 8, kd, st));
@@ -1795,10 +1593,8 @@ extern "C" int b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int
     }
     RET_IF(ensure(ctx, ctx->slots[0].misc, 16 * 8));
     double* dbest = (double*)ctx->slots[0].misc.p;
-    acq_best_kernel<<<1, 256, 0, st>>>(dmean, P, P, maximize, dbest);
-    kg_kernel<<<(unsigned)P, 256, 0, st>>>(dmean, dcov, P, dys, (int)n, P, diag_sub, noise_plus_jitter, maximize, dbest, dout);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches += 2;
+    RET_IF(launch(ctx, st, 1, 256, 0, acq_best_kernel, dmean, P, P, maximize, dbest));
+    RET_IF(launch(ctx, st, (unsigned)P, 256, 0, kg_kernel, dmean, dcov, P, dys, (int)n, P, diag_sub, noise_plus_jitter, maximize, dbest, dout));
     if (!dev) CUDA_TRY(ctx, cudaMemcpyAsync(out, dout, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
     return tm.end(st, nullptr);
 }
@@ -1819,8 +1615,7 @@ extern "C" int b2gp_debug_leaf(b2gp_ctx* ctx, int n, double* A_dev, int64_t lda,
         CUDA_TRY(ctx, cudaFuncSetAttribute(potrf_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PD_SMEM));
         attr.done(ctx->device);
     }
-    potrf_diag_kernel<<<1, PD_THREADS, PD_SMEM, st>>>(A_dev, lda, n, linv_dev, dinfo, 0, dprof);
-    CUDA_TRY(ctx, cudaGetLastError());
+    RET_IF(launch(ctx, st, 1, PD_THREADS, PD_SMEM, potrf_diag_kernel, A_dev, lda, n, linv_dev, dinfo, 0, dprof));
     CUDA_TRY(ctx, cudaMemcpyAsync(prof_host, dprof, 64 * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return B2GP_OK;
@@ -1861,7 +1656,6 @@ extern "C" int b2gp_debug_ozaki(b2gp_ctx* ctx, int S, int64_t m, int64_t n, int6
     if (!ctx) return B2GP_ERR_ARG;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->slots[0].stream;
-    Extra* ex = extra_of(ctx);
     const size_t prof_bytes = (size_t)ctx->sm_count * 8 * sizeof(long long);   // [CTA][8], one CTA per SM at most
     RET_IF(ensure(ctx, ctx->slots[0].oz.prof, prof_bytes));
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->slots[0].oz.prof.p, 0, prof_bytes, st));
@@ -1907,8 +1701,7 @@ extern "C" int b2gp_debug_i8_peak(b2gp_ctx* ctx, int iters, int reps, double* to
     double best = 1e30;
     for (int r = 0; r < reps + 1; ++r) {
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
-        oz_i8_peak_kernel<<<ctx->sm_count, OZ_PEAK_THREADS, smem, st>>>(iters, nullptr);
-        CUDA_TRY(ctx, cudaGetLastError());
+        RET_IF(launch(ctx, st, ctx->sm_count, OZ_PEAK_THREADS, smem, oz_i8_peak_kernel, iters, nullptr));
         CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
         CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_b));
         float ms = 0.f;
@@ -1932,38 +1725,12 @@ extern "C" int b2gp_dist_unique_id(void* id128) {
     return B2GP_OK;
 }
 
-static int dist_free(b2gp_ctx* ctx, DistState* ds) {
-    NcclApi* n = nccl_api();
-    cudaSetDevice(ctx->device);
-    cudaDeviceSynchronize();
-    for (DevBuf* b : {&ds->Aloc, &ds->PB[0], &ds->PB[1], &ds->UB, &ds->EB, &ds->Xrows, &ds->Zcols, &ds->yloc, &ds->red, &ds->linv, &ds->updA, &ds->updB,
-                      &ds->updSA, &ds->updSB, &ds->wseg})
-        free_buf(*b);
-    for (auto& st : ds->steps) {
-        free_buf(st.g1);
-        free_buf(st.g2);
-        free_buf(st.bmap);
-    }
-    for (cudaEvent_t e : {ds->ev_u, ds->ev_ubc[0], ds->ev_ubc[1], ds->ev_chunk, ds->ev_comm[0], ds->ev_comm[1], ds->ev_done, ds->ev_e,
-                          ds->ev_early[0], ds->ev_early[1], ds->ev_g2})
-        if (e) cudaEventDestroy(e);
-    if (ds->ms) cudaStreamDestroy(ds->ms);
-    if (ds->dq) cudaStreamDestroy(ds->dq);
-    if (n->handle) {
-        if (ds->rowc) n->CommDestroy(ds->rowc);
-        if (ds->colc) n->CommDestroy(ds->colc);
-        if (ds->world) n->CommDestroy(ds->world);
-    }
-    delete ds;
-    return B2GP_OK;
-}
-
 extern "C" int b2gp_dist_finalize(b2gp_ctx* ctx) {
     if (!ctx) return B2GP_ERR_ARG;
-    Extra* ex = extra_of(ctx);
-    if (ex->dist) {
-        dist_free(ctx, ex->dist);
-        ex->dist = nullptr;
+    if (ctx->dist) {
+        cudaSetDevice(ctx->device);
+        cudaDeviceSynchronize();
+        ctx->dist.reset();
     }
     return B2GP_OK;
 }
@@ -1976,10 +1743,9 @@ extern "C" int b2gp_dist_init(b2gp_ctx* ctx, const void* id128, int rank, int nr
     if (!n->handle || !n->error.empty())
         return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_dist_init", n->error.c_str(), __FILE__, __LINE__);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-    Extra* ex = extra_of(ctx);
-    if (ex->dist) RET_IF(b2gp_dist_finalize(ctx));
-    DistState* ds = new DistState();
-    ex->dist = ds;
+    if (ctx->dist) RET_IF(b2gp_dist_finalize(ctx));
+    ctx->dist = std::make_unique<DistState>();
+    DistState* ds = ctx->dist.get();
     ds->rank = rank;
     ds->nranks = nranks;
     ds->g.pr = grid_rows;
@@ -2004,7 +1770,7 @@ extern "C" int b2gp_dist_init(b2gp_ctx* ctx, const void* id128, int rank, int nr
 
 extern "C" int b2gp_dist_info(b2gp_ctx* ctx, int* rank, int* nranks, int* grid_rows, int* grid_cols) {
     if (!ctx) return B2GP_ERR_ARG;
-    DistState* ds = extra_of(ctx)->dist;
+    DistState* ds = ctx->dist.get();
     if (!ds || !ds->ready) return set_err(ctx, B2GP_ERR_ARG, "b2gp_dist_info", "call b2gp_dist_init first", __FILE__, __LINE__);
     if (rank) *rank = ds->rank;
     if (nranks) *nranks = ds->nranks;
@@ -2040,12 +1806,8 @@ static int dist_build_steps(b2gp_ctx* ctx, DistState* ds, cudaStream_t st, int C
     const BcGrid& g = ds->g;
     if (ds->cache_T == g.T && ds->cache_R == g.R && ds->cache_nb == g.nb && ds->cache_cl == CL) return B2GP_OK;
     CUDA_TRY(ctx, cudaStreamSynchronize(st));   // lists of a previous shape may still be in use
-    for (auto& s : ds->steps) {
-        free_buf(s.g1);
-        free_buf(s.g2);
-        free_buf(s.bmap);
-    }
-    ds->steps.assign((size_t)g.T, DistStep());
+    ds->steps.clear();
+    ds->steps.resize((size_t)g.T);
     const int64_t nb = g.nb, t128 = nb / 128;          // 128-row groups per tile
     const int64_t colw = CL == 2 ? 128 : 64;           // columns covered by one list entry
     const int64_t ent_per_tile = nb / colw;
@@ -2108,8 +1870,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
                                    int64_t P, int d, const double* theta, int noiseless, double jitter, int64_t nb, unsigned flags,
                                    double* mean, double* var, int* info, b2gp_timing* timing) {
     if (!ctx) return B2GP_ERR_ARG;
-    Extra* ex = extra_of(ctx);
-    DistState* ds = ex->dist;
+    DistState* ds = ctx->dist.get();
     if (!ds || !ds->ready) return set_err(ctx, B2GP_ERR_ARG, "b2gp_dist_posterior", "call b2gp_dist_init first", __FILE__, __LINE__);
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, Xtr && yres && Xnew && theta && mean && info);
@@ -2120,7 +1881,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
     ARG_CHECK(ctx, !want_var || var);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     NcclApi* nc = nccl_api();
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     Slot& sl = ctx->slots[0];
     cudaStream_t cs = sl.stream, ms = ds->ms;
     BcGrid& g = ds->g;
@@ -2193,11 +1954,8 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
                     step = gi - gi0;
                 ++count;
             }
-        if (count > 0) {
-            dist_diag_kernel<<<grid_for(count * nb), 256, 0, cs>>>(A, ld, nb, pr, pc, gi0, step ? step : 1, count, dth, d, jitter);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches++;
-        }
+        if (count > 0)
+            RET_IF(launch(ctx, cs, grid_for(count * nb), 256, 0, dist_diag_kernel, A, ld, nb, pr, pc, gi0, step ? step : 1, count, dth, d, jitter));
         const int64_t gy = T + P / nb;                      // tile row holding the y^T right-hand side (global rhs row P)
         if (gy % pr == myrow)
             CUDA_TRY(ctx, cudaMemcpyAsync(A + ((gy / pr) * nb + P % nb) * ld, ds->yloc.p, (size_t)ld * 8, cudaMemcpyDeviceToDevice, cs));
@@ -2211,7 +1969,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pev[PH_N];
     auto mark = [&](cudaStream_t s) -> cudaEvent_t {
         if (!prof) return nullptr;
-        cudaEvent_t e = ex->pool.get();
+        cudaEvent_t e = ctx->pool.get();
         cudaEventRecord(e, s);
         return e;
     };
@@ -2239,9 +1997,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
                 RET_IF(gemm_nt(ctx, s, nb, nb, nb, -1.0, E, local ? ld : nb, E, local ? ld : nb, 1.0, D, ld, true));
             }
             RET_IF(potrf_rec(ctx, s, D, ld, nb, (double*)ds->linv.p, dinfo, k * nb));
-            set_identity_kernel<<<grid_for(nb * nb), 256, 0, s>>>(U, nb, nb);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches++;
+            RET_IF(launch(ctx, s, grid_for(nb * nb), 256, 0, set_identity_kernel, U, nb, nb));
             RET_IF(trsm_rec(ctx, s, U, nb, nb, D, ld, nb, (const double*)ds->linv.p));      // U = L_kk^{-T}
             span(PH_POTRF, p0, mark(s));
         }
@@ -2273,11 +2029,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
         }
         if (k + 1 < T && myrow == (int)((k + 1) % pr)) {      // my process row holds tile (k+1, k) -- the first tile of its panel rows
             if (pc > 1) {
-                if (mycol == kc) {
-                    copy2d_kernel<<<grid_for(nb * nb), 256, 0, cs>>>(EBs[k & 1], nb, rp, ld, nb, nb);
-                    CUDA_TRY(ctx, cudaGetLastError());
-                    ctx->launches++;
-                }
+                if (mycol == kc) RET_IF(launch(ctx, cs, grid_for(nb * nb), 256, 0, copy2d_kernel, EBs[k & 1], nb, rp, ld, nb, nb));
                 CUDA_TRY(ctx, cudaEventRecord(ds->ev_e, cs));
                 CUDA_TRY(ctx, cudaStreamWaitEvent(ms, ds->ev_e, 0));
                 cudaEvent_t m0 = mark(ms);
@@ -2290,11 +2042,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
         }
         if (mycol == kc) {
             cudaEvent_t p0 = mark(cs);
-            if (rows > 0) {
-                copy2d_kernel<<<grid_for(rows * nb), 256, 0, cs>>>(PBk + (int64_t)myrow * slot * nb, nb, rp, ld, rows, nb);
-                CUDA_TRY(ctx, cudaGetLastError());
-                ctx->launches++;
-            }
+            if (rows > 0) RET_IF(launch(ctx, cs, grid_for(rows * nb), 256, 0, copy2d_kernel, PBk + (int64_t)myrow * slot * nb, nb, rp, ld, rows, nb));
             span(PH_PANEL, p0, mark(cs));
         }
         if (slot > 0) {
@@ -2404,9 +2152,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
             if (gi < T) continue;
             const int64_t p0 = (gi - T) * nb, np = std::min<int64_t>(nb, P - p0);
             if (np <= 0) continue;
-            rowdot2_kernel<<<(unsigned)np, RD_THREADS, 0, cs>>>(A + (li * nb) * ld, ld, ld, wseg, 1.0, red + p0, red + P + p0);
-            CUDA_TRY(ctx, cudaGetLastError());
-            ctx->launches++;
+            RET_IF(launch(ctx, cs, (unsigned)np, RD_THREADS, 0, rowdot2_kernel, A + (li * nb) * ld, ld, ld, wseg, 1.0, red + p0, red + P + p0));
         }
         CUDA_TRY(ctx, cudaEventRecord(ds->ev_chunk, cs));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ms, ds->ev_chunk, 0));
@@ -2414,10 +2160,8 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
         NCCL_TRY(ctx, nc->AllReduce(dinfo, dinfo, 1, ncclInt, ncclMax, ds->world, ms));
         CUDA_TRY(ctx, cudaEventRecord(ds->ev_done, ms));
         CUDA_TRY(ctx, cudaStreamWaitEvent(cs, ds->ev_done, 0));
-        dist_finish_kernel<<<grid_for(P), 256, 0, cs>>>(red, want_var ? red + 2 * P : nullptr, red + P, P, kind, d, dth, noiseless ? 0.0 : 1.0,
-                                                         jitter, dinfo);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches++;
+        RET_IF(launch(ctx, cs, grid_for(P), 256, 0, dist_finish_kernel, red, want_var ? red + 2 * P : nullptr, red + P, P, kind, d, dth,
+                      noiseless ? 0.0 : 1.0, jitter, dinfo));
     }
     CUDA_TRY(ctx, cudaMemcpyAsync(mean, red, (size_t)P * 8, cudaMemcpyDeviceToHost, cs));
     if (want_var) CUDA_TRY(ctx, cudaMemcpyAsync(var, red + 2 * P, (size_t)P * 8, cudaMemcpyDeviceToHost, cs));
@@ -2426,7 +2170,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
     sl.oz_planes = 7;
     float ms_f = 0.f;
     CUDA_TRY(ctx, cudaEventElapsedTime(&ms_f, ev_f0, ev_f1));
-    ex->last.potrf_ms = ms_f;
+    ctx->last.potrf_ms = ms_f;
     if (prof) {
         static const char* names[PH_N] = {"update slices", "g1 (next tile column)", "[diag stream] early update + potrf + U", "wait for U", "panel solve + pack",
                                           "g2 (rest of the update)", "wait for the panel exchange", "[comm stream] U broadcast",
@@ -2447,8 +2191,8 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
         fprintf(stderr, "%s\n", line);     // one write per rank: the ranks share a terminal
     }
     const double n = (double)N, p = (double)P;
-    ex->last.flops = n * n * n / 3.0 + n * n * (p + 1.0) + 4.0 * n * p;
-    if (timing) *timing = ex->last;
+    ctx->last.flops = n * n * n / 3.0 + n * n * (p + 1.0) + 4.0 * n * p;
+    if (timing) *timing = ctx->last;
     return B2GP_OK;
 }
 
@@ -2462,8 +2206,7 @@ extern "C" int b2gp_dist_sparse_posterior(b2gp_ctx* ctx, int kind, const double*
                                           const double* theta, int noiseless, double jitter, unsigned flags, double* mean,
                                           double* var, int* info, b2gp_timing* timing) {
     if (!ctx) return B2GP_ERR_ARG;
-    Extra* ex = extra_of(ctx);
-    DistState* ds = ex->dist;
+    DistState* ds = ctx->dist.get();
     if (!ds || !ds->ready) return set_err(ctx, B2GP_ERR_ARG, "b2gp_dist_sparse_posterior", "call b2gp_dist_init first", __FILE__, __LINE__);
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, Xu && Xtr_shard && y_shard && Xnew && theta && mean && info);
@@ -2473,7 +2216,7 @@ extern "C" int b2gp_dist_sparse_posterior(b2gp_ctx* ctx, int kind, const double*
     ARG_CHECK(ctx, !want_var || var);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     NcclApi* nc = nccl_api();
-    ex->fcache.valid = false;
+    ctx->fcache.valid = false;
     Slot& sl = ctx->slots[0];
     cudaStream_t st = sl.stream, ms = ds->ms;
     CallTimer tm(ctx);
@@ -2522,11 +2265,11 @@ extern "C" int b2gp_dist_sparse_posterior(b2gp_ctx* ctx, int kind, const double*
     info[0] = hinfo[0] != 0 ? hinfo[0] : -hinfo[1];
     float f = 0.f;
     CUDA_TRY(ctx, cudaEventElapsedTime(&f, e0, e1));
-    ex->last.potrf_ms = f;          // per-rank statistics (Gram, Luu, W, W W^T)
+    ctx->last.potrf_ms = f;          // per-rank statistics (Gram, Luu, W, W W^T)
     CUDA_TRY(ctx, cudaEventElapsedTime(&f, e1, e2));
-    ex->last.trsm_ms = f;           // the all-reduce
+    ctx->last.trsm_ms = f;           // the all-reduce
     const double m = (double)M, n = (double)N_shard * ds->nranks, p = (double)P;
-    ex->last.flops = 2.0 * m * m * m / 3.0 + 2.0 * m * m * n + 2.0 * m * m * (p + 1.0);
-    if (timing) *timing = ex->last;
+    ctx->last.flops = 2.0 * m * m * m / 3.0 + 2.0 * m * m * n + 2.0 * m * m * (p + 1.0);
+    if (timing) *timing = ctx->last;
     return B2GP_OK;
 }

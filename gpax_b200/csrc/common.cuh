@@ -1,4 +1,4 @@
-// common.cuh -- context, error handling, device buffers for libb200gp.so (sm_90a only).
+// common.cuh -- context, error handling, device buffers, kernel launches for libb200gp.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <atomic>
@@ -6,8 +6,10 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200gp.h"
@@ -18,10 +20,51 @@
 // SM count of the largest device a context has been created on (grid_for's cap)
 inline std::atomic<int> g_grid_sms{1};
 
+// A device allocation that frees itself; ensure() grows it.  Move-only: one owner per pointer.
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) {
+        o.p = nullptr;
+        o.cap = 0;
+    }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) {
+            if (p) cudaFree(p);
+            p = o.p;
+            cap = o.cap;
+            o.p = nullptr;
+            o.cap = 0;
+        }
+        return *this;
+    }
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
 };
+
+// Timing events handed out per call (per-stage timings, profiles), reused from call to call.
+struct EventPool {
+    std::vector<cudaEvent_t> ev;
+    size_t next = 0;
+    cudaEvent_t get() {
+        if (next == ev.size()) {
+            cudaEvent_t e;
+            if (cudaEventCreate(&e) != cudaSuccess) return nullptr;
+            ev.push_back(e);
+        }
+        return ev[next++];
+    }
+    void reset() { next = 0; }
+    void destroy() {
+        for (auto e : ev) cudaEventDestroy(e);
+        ev.clear();
+        next = 0;
+    }
+};
+
+struct DistState;  // multi-GPU state (dist.cuh)
 
 #define OZ_LISTS 192
 // scratch of the int8-split (Ozaki) GEMM path, one per stream: digit planes, row scales, tile list
@@ -53,8 +96,8 @@ struct Slot {
 };
 
 // Cumulative per-context counters of the kernels launched and the solver routes entered, in the order
-// b2gp_debug_path_counts reports them.  They sit next to the `launches++` of each site and steer nothing: tests read them
-// to prove which path a call took.
+// b2gp_debug_path_counts reports them.  The kernel counters are kept by launch() / count_launch(), the route counters by
+// count_path() at the entry of the route.  They steer nothing: tests read them to prove which path a call took.
 enum PathCounter {
     PATH_GEMM_NT = 0,   // gemm_nt_kernel launches (cp.async + DMMA), the 64x64 tail launch of the TMA kernel included
     PATH_GEMM_TMA,      // gemm_tma_kernel launches (persistent TMA + DMMA)
@@ -93,9 +136,36 @@ struct b2gp_ctx {
     DevBuf d_in[8];
     DevBuf d_out[4];
     DevBuf d_info;
+    DevBuf theta1;     // one-draw theta for b2gp_gram
+    DevBuf potrf_buf;  // staging for host-pointer b2gp_potrf / trsm / gemm
+    DevBuf gemm_buf[3];
+    DevBuf eb[12];     // scratch of b2gp_sparse_elbo
+    DevBuf f32_in[8];  // fp32 staging of the inputs / outputs of calls made with B2GP_FLAG_F32
+    DevBuf f32_out[4];
+    std::vector<void*> user_allocs;  // b2gp_dev_alloc
     // factor bookkeeping for b2gp_trsm_lower (host-pointer mode keeps the factor resident)
     DevBuf last_linv;
     int64_t last_n = 0;
+    // factor cache of slot 0 (host-pointer, single-draw calls): predict_in_batches / viGP chunk loops call the
+    // posterior repeatedly with the same training set and theta; the reference re-inverts k_XX every time
+    // (gp.py:319-322 -> gp.py:269-271), here the factor L and its inverted diagonal blocks are kept.
+    struct {
+        bool valid = false;
+        int kind = -1, d = 0;
+        int64_t N = 0;
+        double jitter = 0.0;
+        std::vector<double> theta;
+        std::vector<char> X;   // raw bytes of the caller's training inputs (fp64 or fp32)
+        int info = 0;
+        int64_t U_nb = 0;      // > 0: `Ukeep` holds the explicit inverses of the factor's U_nb-wide diagonal blocks (potrf_tall)
+    } fcache;
+    DevBuf Ukeep;
+    int64_t cache_hits = 0;
+    std::unique_ptr<DistState> dist;   // created by b2gp_dist_init, released by b2gp_dist_finalize or with the context
+    b2gp_timing last{};                // what b2gp_last_timing reports
+    EventPool pool;
+    cudaEvent_t slot_done[B2GP_MAX_STREAMS] = {};
+    cudaEvent_t inputs_ready = nullptr;
     std::atomic<int64_t> launches{0};  // kernels queued (draws may be queued from several host threads)
     std::atomic<int64_t> path[PATH_COUNT] = {};  // which kernels / routes the work took (b2gp_debug_path_counts)
     std::string err;
@@ -131,6 +201,28 @@ static inline int set_err(b2gp_ctx* ctx, int code, const char* what, const char*
         int r_ = (expr);            \
         if (r_ != B2GP_OK) return r_; \
     } while (0)
+
+// Every kernel of the library is launched through launch() (or, for a cluster launch, by cudaLaunchKernelEx followed
+// by count_launch()): the launch is checked where it is made, counted in ctx->launches (b2gp_timing::launches is the
+// difference over a call) and, when `path` names a kernel counter, in ctx->path.
+static inline int count_launch(b2gp_ctx* ctx, int path = -1) {
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_err(ctx, B2GP_ERR_CUDA, "kernel launch", cudaGetErrorString(e), __FILE__, __LINE__);
+    ctx->launches++;
+    if (path >= 0) count_path(ctx, path);
+    return B2GP_OK;
+}
+
+template <typename... P, typename... A>
+static int launch(b2gp_ctx* ctx, int path, cudaStream_t st, dim3 grid, dim3 block, size_t smem, void (*k)(P...), A&&... args) {
+    k<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+    return count_launch(ctx, path);
+}
+
+template <typename... P, typename... A>
+static int launch(b2gp_ctx* ctx, cudaStream_t st, dim3 grid, dim3 block, size_t smem, void (*k)(P...), A&&... args) {
+    return launch(ctx, -1, st, grid, block, smem, k, std::forward<A>(args)...);
+}
 
 static inline int ensure(b2gp_ctx* ctx, DevBuf& b, size_t bytes) {
     if (b.cap >= bytes && b.p) return B2GP_OK;

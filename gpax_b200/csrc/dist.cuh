@@ -135,6 +135,19 @@ struct DistState {
     int64_t cache_T = -1, cache_R = -1, cache_nb = -1;
     int cache_cl = -1;
     double last_potrf_ms = 0.0, last_total_ms = 0.0;
+    // the owner synchronises the device first; the buffers free themselves
+    ~DistState() {
+        for (cudaEvent_t e : {ev_u, ev_ubc[0], ev_ubc[1], ev_chunk, ev_comm[0], ev_comm[1], ev_done, ev_e, ev_early[0], ev_early[1], ev_g2})
+            if (e) cudaEventDestroy(e);
+        if (ms) cudaStreamDestroy(ms);
+        if (dq) cudaStreamDestroy(dq);
+        NcclApi* n = nccl_api();
+        if (n->handle) {
+            if (rowc) n->CommDestroy(rowc);
+            if (colc) n->CommDestroy(colc);
+            if (world) n->CommDestroy(world);
+        }
+    }
 };
 
 // diagonal term of k_XX on the diagonal tiles this process owns (gi = gi0 + t * step, t < count): K[i, i] += noise + jitter

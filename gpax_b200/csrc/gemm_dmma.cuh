@@ -213,11 +213,7 @@ static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
         attr_set[aligned ? 1 : 0].done(ctx->device);
     }
-    kern<<<(unsigned)grid, WARPS_M * WARPS_N * 32, smem_bytes, st>>>(a);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    count_path(ctx, PATH_GEMM_NT);
-    return B2GP_OK;
+    return launch(ctx, PATH_GEMM_NT, st, (unsigned)grid, WARPS_M * WARPS_N * 32, smem_bytes, kern, a);
 }
 
 static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);  // gemm_tma.cuh

@@ -251,10 +251,7 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     int64_t main_tiles = tiles;
     if (!inplace && tiles > S && tiles % S != 0) main_tiles = tiles - tiles % S;
     const int grid = (int)(main_tiles < S ? main_tiles : S);
-    gemm_tma_kernel<STAGES, KSUB><<<grid, TG_THREADS, smem_bytes, st>>>(mapA, mapB, a, (int)main_tiles);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    count_path(ctx, PATH_GEMM_TMA);
+    RET_IF(launch(ctx, PATH_GEMM_TMA, st, grid, TG_THREADS, smem_bytes, gemm_tma_kernel<STAGES, KSUB>, mapA, mapB, a, (int)main_tiles));
     if (main_tiles < tiles) {
         GemmArgs t = a;
         t.tile_base = (int)main_tiles;
@@ -268,10 +265,7 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
             CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tail_smem));
             tattr.done(ctx->device);
         }
-        kern<<<(unsigned)(4 * (tiles - main_tiles)), 256, tail_smem, st>>>(t);
-        CUDA_TRY(ctx, cudaGetLastError());
-        ctx->launches++;
-        count_path(ctx, PATH_GEMM_NT);
+        RET_IF(launch(ctx, PATH_GEMM_NT, st, (unsigned)(4 * (tiles - main_tiles)), 256, tail_smem, kern, t));
     }
     return B2GP_OK;
 }

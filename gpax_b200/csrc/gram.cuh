@@ -356,14 +356,17 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_fast_kernel(const GramArgs 
     }
 }
 
+using GramKernel = void (*)(const GramArgs);
+
+// the fixed-d kernel of KIND for d <= 4, else nullptr
 template <int KIND>
-static bool launch_gram_fast(cudaStream_t st, const GramArgs& a, dim3 grid) {
-    switch (a.d) {
-        case 1: gram_fast_kernel<KIND, 1><<<grid, GRAM_THREADS, 0, st>>>(a); return true;
-        case 2: gram_fast_kernel<KIND, 2><<<grid, GRAM_THREADS, 0, st>>>(a); return true;
-        case 3: gram_fast_kernel<KIND, 3><<<grid, GRAM_THREADS, 0, st>>>(a); return true;
-        case 4: gram_fast_kernel<KIND, 4><<<grid, GRAM_THREADS, 0, st>>>(a); return true;
-        default: return false;
+static GramKernel gram_fast_for(int d) {
+    switch (d) {
+        case 1: return gram_fast_kernel<KIND, 1>;
+        case 2: return gram_fast_kernel<KIND, 2>;
+        case 3: return gram_fast_kernel<KIND, 3>;
+        case 4: return gram_fast_kernel<KIND, 4>;
+        default: return nullptr;
     }
 }
 
@@ -399,11 +402,9 @@ static int launch_gram(b2gp_ctx* ctx, cudaStream_t st, int kind, const double* X
         attr.done(ctx->device);
     }
     dim3 grid((unsigned)ceil_div(m, GRAM_BN), (unsigned)ceil_div(n, GRAM_BM));
-    bool done = false;
-    if (kind == B2GP_KERNEL_RBF) done = launch_gram_fast<B2GP_KERNEL_RBF>(st, a, grid);
-    if (kind == B2GP_KERNEL_MATERN52) done = launch_gram_fast<B2GP_KERNEL_MATERN52>(st, a, grid);
-    if (!done) gram_kernel<<<grid, GRAM_THREADS, smem, st>>>(a);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    return B2GP_OK;
+    GramKernel fast = nullptr;
+    if (kind == B2GP_KERNEL_RBF) fast = gram_fast_for<B2GP_KERNEL_RBF>(d);
+    if (kind == B2GP_KERNEL_MATERN52) fast = gram_fast_for<B2GP_KERNEL_MATERN52>(d);
+    if (fast) return launch(ctx, st, grid, GRAM_THREADS, 0, fast, a);
+    return launch(ctx, st, grid, GRAM_THREADS, smem, gram_kernel, a);
 }

@@ -459,11 +459,8 @@ static int oz_slice_launch(b2gp_ctx* ctx, cudaStream_t st, const double* src, in
     const int64_t kpad = round_up(k, OZ_KB), rp = round_up(rows, 128);
     RET_IF(ensure(ctx, planes, (size_t)S * rp * kpad));
     RET_IF(ensure(ctx, scale, (size_t)rp * 8));
-    oz_slice_kernel<S><<<(unsigned)rp, 256, 0, st>>>(src, ld, (int)rows, (int)k, (int8_t*)planes.p, (int)rp, (int)kpad, (double*)scale.p,
-                                                     trans ? 1 : 0, rowmap128);
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    count_path(ctx, PATH_OZ_SLICE);
+    RET_IF(launch(ctx, PATH_OZ_SLICE, st, (unsigned)rp, 256, 0, oz_slice_kernel<S>, src, ld, (int)rows, (int)k, (int8_t*)planes.p, (int)rp,
+                  (int)kpad, (double*)scale.p, trans ? 1 : 0, rowmap128));
     out->planes = (const int8_t*)planes.p;
     out->scale = (const double*)scale.p;
     out->rows_pad = rp;
@@ -568,14 +565,10 @@ static int oz_mma_launch(b2gp_ctx* ctx, cudaStream_t st, OzWork& w, const OzOper
         cfg.attrs = at;
         cfg.numAttrs = 1;
         CUDA_TRY(ctx, cudaLaunchKernelEx(&cfg, oz_mma_kernel<S, 2>, mapA, mapB, a));
-    } else {
-        const int grid = (int)(tiles < nsm ? tiles : nsm);
-        oz_mma_kernel<S, 1><<<grid, OZ_THREADS, smem_bytes, st>>>(mapA, mapB, a);
+        return count_launch(ctx, PATH_OZ_MMA);
     }
-    CUDA_TRY(ctx, cudaGetLastError());
-    ctx->launches++;
-    count_path(ctx, PATH_OZ_MMA);
-    return B2GP_OK;
+    const int grid = (int)(tiles < nsm ? tiles : nsm);
+    return launch(ctx, PATH_OZ_MMA, st, grid, OZ_THREADS, smem_bytes, oz_mma_kernel<S, 1>, mapA, mapB, a);
 }
 
 template <int S>
