@@ -1639,6 +1639,10 @@ extern "C" int b2gp_debug_gemm_cfg(b2gp_ctx* ctx, int cfg, int64_t m, int64_t n,
         case 3: rc = launch_gemm_cfg<128, 128, 4, 2, 4, 1>(ctx, st, a); break;
         case 4: rc = launch_gemm_cfg<128, 128, 2, 8, 4, 1>(ctx, st, a); break;
         case 5: rc = launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a); break;
+        // the latency-bound and lower-only configurations of gemm_nt
+        case 6: rc = launch_gemm_cfg<32, 128, 1, 8, 3, 2>(ctx, st, a); break;
+        case 7: rc = launch_gemm_cfg<64, 128, 2, 4, 3, 2>(ctx, st, a); break;
+        case 8: rc = launch_gemm_cfg<64, 64, 2, 4, 4, 2>(ctx, st, a); break;
         default: break;
     }
     RET_IF(rc);
@@ -1709,6 +1713,28 @@ extern "C" int b2gp_debug_i8_peak(b2gp_ctx* ctx, int iters, int reps, double* to
         if (r > 0 && ms < best) best = ms;
     }
     *tops_out = 2.0 * 64 * 256 * 32 * (OZ_PEAK_THREADS / 128) * (double)iters * ctx->sm_count / (best * 1e-3) / 1e12;
+    if (ms_out) *ms_out = best;
+    return B2GP_OK;
+}
+
+// Development aid: the measured fp64 tensor ceiling in TFLOP/s of one DMMA shape (see dmma_peak_kernel; 0: m8n8k4,
+// 1: m16n8k4, 2: m16n8k8, 3: m16n8k16), best of `reps`.
+extern "C" int b2gp_debug_dmma_peak(b2gp_ctx* ctx, int shape, int iters, int reps, double* tflops_out, double* ms_out) {
+    if (!ctx || !tflops_out || shape < 0 || shape > 3 || iters < 4 || reps < 1) return B2GP_ERR_ARG;
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->slots[0].stream;
+    void (*const kern[4])(int, double*) = {dmma_peak_kernel<0>, dmma_peak_kernel<1>, dmma_peak_kernel<2>, dmma_peak_kernel<3>};
+    double best = 1e30;
+    for (int r = 0; r < reps + 1; ++r) {
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
+        RET_IF(launch(ctx, st, ctx->sm_count, DMMA_PEAK_THREADS, 0, kern[shape], iters, nullptr));
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
+        CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_b));
+        float ms = 0.f;
+        CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+        if (r > 0 && ms < best) best = ms;
+    }
+    *tflops_out = 2.0 * dmma_peak_fma(shape) * DMMA_PEAK_ACC * (DMMA_PEAK_THREADS / 32) * (double)iters * ctx->sm_count / (best * 1e-3) / 1e12;
     if (ms_out) *ms_out = best;
     return B2GP_OK;
 }

@@ -5,8 +5,10 @@
 // epilogue cov = k_pp - V^T V.  It stands where the reference calls jnp.matmul on the outputs of
 // jnp.linalg.inv (gpax/models/gp.py:271-273).
 //
-// The fp64 tensor instruction used here is `mma.sync.m8n8k4.f64` (DMMA; sm_90 has no fp64 wgmma).  Both operands are K-major (rows contiguous in k), so
-// one shared-memory layout and one fragment pattern serve A and B:
+// The fp64 tensor instruction used here is `mma.sync.m16n8k4.f64` (DMMA.16x8x4; sm_90 has no fp64 wgmma).  On the
+// H100 it issues at twice the rate of the Ampere shape m8n8k4 (DESIGN.md 4.3, tools/dmma_peak.py), with the same
+// operand registers: an m16 A fragment is rows g and g + 8, i.e. two m8 fragments (dmma_slice16).  Both operands are
+// K-major (rows contiguous in k), so one shared-memory layout and one fragment pattern serve A and B:
 //     a = As[(row0 + g) * LDS + 4*kk + t]      b = Bs[(col0 + g) * LDS + 4*kk + t]
 // with g = lane/4, t = lane%4.  LDS = 20 doubles (160 B) makes the 8 rows x 32 B a half-warp reads
 // land in 8 distinct 32-B bank groups -> conflict-free LDS.64.
@@ -49,10 +51,91 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
 }
 
+// Fragments (PTX ISA, "Matrix Fragments for mma.m8n8k4 / m16n8k4 / m16n8k8 / m16n8k16", .f64), g = lane/4, t = lane%4:
+//   m8n8k4    a: (row g, k t)                     b: (k t, col g)                 c0,c1: (row g, cols 2t, 2t+1)
+//   m16n8k4   a0: (g, t)   a1: (g+8, t)           b: (k t, col g)                 c0,c1: row g;  c2,c3: row g+8
+//   m16n8k8   a[2j]: (g, t+4j)  a[2j+1]: (g+8, t+4j)   b[j]: (k t+4j, col g)     c as m16n8k4
+//   m16n8k16  as m16n8k8 with j = 0..3
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
     asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
         : "+d"(c0), "+d"(c1)
         : "d"(a), "d"(b));
+}
+// c0, c1 = rows g of the 16x8 block, c2, c3 = rows g + 8
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b0) {
+    asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+        : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+        : "d"(a0), "d"(a1), "d"(b0));
+}
+__device__ __forceinline__ void dmma1688(double& c0, double& c1, double& c2, double& c3, const double (&a)[4], const double (&b)[2]) {
+    asm("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+        : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+}
+__device__ __forceinline__ void dmma16816(double& c0, double& c1, double& c2, double& c3, const double (&a)[8], const double (&b)[4]) {
+    asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, "
+        "{%0,%1,%2,%3};\n"
+        : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]), "d"(b[2]),
+          "d"(b[3]));
+}
+
+// One 16-deep k-slice of a warp tile of MI x NI blocks of 8 x 8 on m16n8k4, the shape every fp64 GEMM kernel here issues
+// (gemm_nt_kernel, gemm_tma_kernel, trsm_strip_kernel): the same instructions in the same k order, so the kernels agree
+// bit for bit.  `lda(i, q)` returns A at row i*8 + g, k 4q + t (q = 0..3); `ldb(j, q)` B at column j*8 + g, k 4q + t.
+// acc[i][j] keeps the m8n8 fragment (row i*8 + g, columns 2t, 2t+1): 8-row blocks 2i' and 2i'+1 are the c0,c1 and
+// c2,c3 halves of m16 tile i', and their A values are its a0 and a1.  So the operand registers are those of m8n8k4, at
+// twice its rate on Hopper (DESIGN.md 4.3).  Each instruction spans k 4q .. 4q+3 of the zero-filled slice.
+template <int MI, int NI, class LA, class LB>
+__device__ __forceinline__ void dmma_slice16(double (&acc)[MI][NI][2], LA lda, LB ldb) {
+    static_assert(MI % 2 == 0, "m16 tiles");
+#pragma unroll
+    for (int q = 0; q < GEMM_BK / 4; ++q) {
+        double a[MI], b[NI];
+#pragma unroll
+        for (int i = 0; i < MI; ++i) a[i] = lda(i, q);
+#pragma unroll
+        for (int j = 0; j < NI; ++j) b[j] = ldb(j, q);
+#pragma unroll
+        for (int i = 0; i < MI / 2; ++i)
+#pragma unroll
+            for (int j = 0; j < NI; ++j)
+                dmma1684(acc[2 * i][j][0], acc[2 * i][j][1], acc[2 * i + 1][j][0], acc[2 * i + 1][j][1], a[2 * i], a[2 * i + 1], b[j]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- peak probe
+// The fp64 tensor-pipe ceiling of each instruction shape, measured instead of assumed: every CTA (one per SM, eight
+// warps, two per SM sub-partition) issues `iters` rounds of DMMA_PEAK_ACC independent MMAs of one shape on
+// register-resident operands (no shared memory, no epilogue).  SHAPE 0: m8n8k4, 1: m16n8k4, 2: m16n8k8, 3: m16n8k16.
+constexpr int DMMA_PEAK_THREADS = 256;
+constexpr int DMMA_PEAK_ACC = 8;
+__host__ __device__ constexpr int dmma_peak_fma(int shape) { return shape == 0 ? 8 * 8 * 4 : 16 * 8 * (4 << (shape - 1)); }
+
+template <int SHAPE>
+__global__ void __launch_bounds__(DMMA_PEAK_THREADS, 1) dmma_peak_kernel(int iters, double* sink) {
+    const double x = 1.0 + 1e-3 * (double)(threadIdx.x & 31);
+    double a[8], b[4], acc[DMMA_PEAK_ACC][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) a[i] = x * 1e-3 * (double)(i + 1);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) b[j] = x - 1e-2 * (double)j;
+#pragma unroll
+    for (int u = 0; u < DMMA_PEAK_ACC; ++u) acc[u][0] = acc[u][1] = acc[u][2] = acc[u][3] = 0.0;
+    for (int it = 0; it < iters; ++it) {
+#pragma unroll
+        for (int u = 0; u < DMMA_PEAK_ACC; ++u) {
+            double* c = acc[u];
+            if (SHAPE == 0) dmma884(c[0], c[1], a[0], b[0]);
+            if (SHAPE == 1) dmma1684(c[0], c[1], c[2], c[3], a[0], a[1], b[0]);
+            if (SHAPE == 2) dmma1688(c[0], c[1], c[2], c[3], reinterpret_cast<const double(&)[4]>(a), reinterpret_cast<const double(&)[2]>(b));
+            if (SHAPE == 3) dmma16816(c[0], c[1], c[2], c[3], a, b);
+        }
+    }
+    double s = 0.0;
+#pragma unroll
+    for (int u = 0; u < DMMA_PEAK_ACC; ++u) s += acc[u][0] + acc[u][1] + acc[u][2] + acc[u][3];
+    if (sink) sink[blockIdx.x * blockDim.x + threadIdx.x] = s;   // keeps the accumulators observable
 }
 
 // Load ROWS x 16 doubles (rows [row0, row0+ROWS) of a row-major matrix, columns [k0, k0+16)) into
@@ -149,18 +232,8 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
         }
         const double* As = smem + (kt % STAGES) * STAGE_ELEMS + (wm * WTM + g) * GEMM_LDS + t4;
         const double* Bs = smem + (kt % STAGES) * STAGE_ELEMS + BM * GEMM_LDS + (wn * WTN + g) * GEMM_LDS + t4;
-#pragma unroll
-        for (int kk = 0; kk < GEMM_BK / 4; ++kk) {
-            double a[MI], b[NI];
-#pragma unroll
-            for (int i = 0; i < MI; ++i) a[i] = As[i * 8 * GEMM_LDS + kk * 4];
-#pragma unroll
-            for (int j = 0; j < NI; ++j) b[j] = Bs[j * 8 * GEMM_LDS + kk * 4];
-#pragma unroll
-            for (int i = 0; i < MI; ++i)
-#pragma unroll
-                for (int j = 0; j < NI; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
-        }
+        dmma_slice16(acc, [&](int i, int q) { return As[i * 8 * GEMM_LDS + q * 4]; },
+                     [&](int j, int q) { return Bs[j * 8 * GEMM_LDS + q * 4]; });
     }
     cp_async_wait<0>();
 
@@ -257,8 +330,8 @@ static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t
         RET_IF(gemm_nt(ctx, st, n, n, k, alpha, A, lda, B, ldb, beta, C, ldc, true));
         return gemm_nt(ctx, st, m - n, n, k, alpha, A + n * lda, lda, B, ldb, beta, C + n * ldc, ldc, false);
     }
-    // Tile choice.  A 128x128 tile keeps one SM busy for 128*128*k/64 cycles (DMMA: 64 fp64 FMA/clk/SM),
-    // i.e. ~17 us per k = 128, however few tiles there are; when the 128x128 grid would leave most of
+    // Tile choice.  A 128x128 tile keeps one SM busy for at least 128*128*k/128 cycles (DMMA.16x8x4: 128 fp64
+    // FMA/clk/SM measured on the H100), i.e. ~8 us per k = 128, however few tiles there are; when the 128x128 grid would leave most of
     // the SMs idle, spend the same flops on more, smaller tiles.  The in-place triangular-solve
     // use (C aliases A, n <= 128) needs a single column tile, which all three configurations give.
     const int64_t tm128 = ceil_div(m, 128), tn128 = ceil_div(n, 128);

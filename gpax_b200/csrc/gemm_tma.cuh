@@ -10,6 +10,7 @@
 //     releases the slot with one arrive on `empty[stage]` (count 8) -- warps drift apart and keep the pipe busy;
 //   * CTAs are persistent (grid = SM count): while the consumers run a tile's epilogue (read-modify-write of C)
 //     the producer is already filling the ring with the next tile's first k-slices.
+// The consumers issue the same m16n8k4 DMMA in the same k order as gemm_nt_kernel (dmma_slice16), so both give the same bits.
 // Shared-memory tile = 128 rows x 128 B, 16-byte chunks XOR-swizzled with (row & 7) by the TMA unit; a fragment
 // element (row r, column c) lives at  r*128 + (((c>>1) ^ (r&7)) << 4) + (c&1)*8.
 #pragma once
@@ -145,12 +146,12 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const int wm = cw >> 2, wn = cw & 3;
     const int g = lane >> 2, t4 = lane & 3;
     constexpr int MI = 8, NI = 4;
-    // byte offsets inside a [128 x 128 B] swizzled box for this lane: row part and the 4 swizzled k positions
-    uint32_t xoff[4];
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) xoff[kk] = ((uint32_t)((2 * kk + (t4 >> 1)) ^ g) << 4) + ((uint32_t)(t4 & 1) << 3);
-    const uint32_t a_row = (uint32_t)(wm * 64 + g) * 128u;
-    const uint32_t b_row = (uint32_t)(wn * 32 + g) * 128u;
+    // byte offsets inside a [128 x 128 B] swizzled box for this lane: row part, and the swizzled position of k = t4.
+    // k = 4q + t4 is 16-byte chunk 2q + (t4 >> 1) XOR g, i.e. at x0 ^ (q << 5); the row bases are 128-byte aligned, so
+    // the XOR can be applied to the whole row-base + x0 offset (one register instead of four).
+    const uint32_t x0 = ((uint32_t)((t4 >> 1) ^ g) << 4) + ((uint32_t)(t4 & 1) << 3);
+    const uint32_t a_row = (uint32_t)(wm * 64 + g) * 128u + x0;
+    const uint32_t b_row = (uint32_t)(wn * 32 + g) * 128u + x0;
     const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
 
     uint32_t it = 0;
@@ -169,22 +170,11 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             mbar_wait(bars + 8 * s, ph);
 #pragma unroll
             for (int sub = 0; sub < KSUB; ++sub) {
-                const uint8_t* As = sgen + s * STAGE_BYTES + sub * TG_SUB_BYTES + a_row;
-                const uint8_t* Bs = sgen + s * STAGE_BYTES + (KSUB + sub) * TG_SUB_BYTES + b_row;
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    double a[MI], b[NI];
-#pragma unroll
-                    for (int i = 0; i < MI; ++i)
-                        a[i] = *reinterpret_cast<const double*>(As + i * 1024 + xoff[kk]);
-#pragma unroll
-                    for (int j = 0; j < NI; ++j)
-                        b[j] = *reinterpret_cast<const double*>(Bs + j * 1024 + xoff[kk]);
-#pragma unroll
-                    for (int i = 0; i < MI; ++i)
-#pragma unroll
-                        for (int j = 0; j < NI; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
-                }
+                const uint8_t* box = sgen + s * STAGE_BYTES + sub * TG_SUB_BYTES;
+                dmma_slice16(acc, [&](int i, int q) { return *reinterpret_cast<const double*>(box + (a_row ^ (q << 5)) + i * 1024); },
+                             [&](int j, int q) {
+                                 return *reinterpret_cast<const double*>(box + KSUB * TG_SUB_BYTES + (b_row ^ (q << 5)) + j * 1024);
+                             });
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(bars + 8 * (STAGES + s));
