@@ -22,6 +22,7 @@ FLAG_DEVICE_PTRS = 1 << 0
 FLAG_LOWER_ONLY = 1 << 1
 FLAG_F32 = 1 << 2
 OUT_MEAN, OUT_VAR, OUT_COV, OUT_SAMPLE = 1 << 4, 1 << 5, 1 << 6, 1 << 7
+OUT_DMEAN, OUT_DVAR = 1 << 8, 1 << 9
 
 
 class B200GPError(RuntimeError):
@@ -73,6 +74,8 @@ SIGNATURES = {
     "b2gp_posterior_batch": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int,
                                        C.c_int64, _vp, _vp, C.c_int64, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp,
                                        C.c_int64, _vp, _vp, C.POINTER(Timing)]),
+    "b2gp_posterior_grad": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int, C.c_int64,
+                                      _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mll_v": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _ip]),
     "b2gp_sparse_posterior": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
                                         _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
@@ -383,6 +386,34 @@ class Context:
             _ptr(theta), _ptr(nv), nvs, int(bool(noiseless)), float(jitter), flags, _ptr(mean), _ptr(var), _ptr(cov), _ptr(eps),
             n_samp, _ptr(samp), info.ctypes.data_as(_vp), C.byref(t) if timing else None))
         out = {"mean": mean, "var": var, "cov": cov, "y_sampled": samp, "info": info}
+        if timing:
+            out["timing"] = t.as_dict()
+        return out
+
+    def posterior_grad(self, kind, Xtr, yres, Xnew, theta, noiseless=False, jitter=1e-6,
+                       want=("mean", "var", "dmean", "dvar"), timing=False):
+        """The posterior mean / variance and their gradients w.r.t. the test inputs (b2gp_posterior_grad).  Xtr [N, d],
+        Xnew [P, d], theta [S, d+3], yres [N] or [S, N]; fp64 host arrays.  Returns a dict with mean / var [S, P],
+        dmean / dvar [S, P, d] (None where not in `want`) and info [S]."""
+        Xtr, Xnew = _f64(Xtr), _f64(Xnew)
+        N, d = Xtr.shape
+        P = Xnew.shape[0]
+        theta = _f64(theta).reshape(-1, d + 3)
+        S = theta.shape[0]
+        yres = _f64(yres)
+        stride = 0 if yres.ndim == 1 else yres.shape[1]
+        bits = {"mean": (OUT_MEAN, (S, P)), "var": (OUT_VAR, (S, P)), "dmean": (OUT_DMEAN, (S, P, d)), "dvar": (OUT_DVAR, (S, P, d))}
+        flags, out = 0, {}
+        for name, (bit, shape) in bits.items():
+            out[name] = np.empty(shape) if name in want else None
+            flags |= bit if name in want else 0
+        info = np.zeros(S, dtype=np.int32)
+        t = Timing()
+        self._check(self.lib.b2gp_posterior_grad(
+            self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(Xtr), N, _ptr(yres), stride, _ptr(Xnew), P, d, S,
+            _ptr(theta), int(bool(noiseless)), float(jitter), flags, _ptr(out["mean"]), _ptr(out["var"]), _ptr(out["dmean"]),
+            _ptr(out["dvar"]), info.ctypes.data_as(_vp), C.byref(t) if timing else None))
+        out["info"] = info
         if timing:
             out["timing"] = t.as_dict()
         return out

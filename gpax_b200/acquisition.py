@@ -1,7 +1,7 @@
 """
-acquisition.py -- acquisition functions with the reference's surface: EI / UCB / POI / UE / KG
-(gpax/acquisition/acquisition.py:50-500 over base_acq.py:20-232) and the q-batch forms qEI / qUCB / qPOI
-(gpax/acquisition/batch_acquisition.py:60-260).  The arithmetic runs on the GPU as epilogues of the posterior
+acquisition.py -- acquisition functions with the reference's surface: EI / UCB / POI / UE / KG / Thompson
+(gpax/acquisition/acquisition.py:50-524 over base_acq.py:20-232), the q-batch forms qEI / qUCB / qPOI / qKG
+(gpax/acquisition/batch_acquisition.py:60-282) and optimize_acq over a continuous box (gpax/acquisition/optimize.py).  The arithmetic runs on the GPU as epilogues of the posterior
 (b2gp_acq_moments / b2gp_acq_samples / b2gp_kg, gpax_b200/csrc/acq.cuh); the penalties of
 gpax/acquisition/penalties.py are O(P * recent) host arithmetic and stay on the host, as in the reference.
 """
@@ -12,7 +12,8 @@ import numpy as np
 from . import prng
 from .utils import posterior_eps
 
-__all__ = ["EI", "UCB", "POI", "UE", "KG", "qEI", "qUCB", "qPOI", "ei", "ucb", "poi", "ue", "compute_penalty"]
+__all__ = ["EI", "UCB", "POI", "UE", "KG", "Thompson", "qEI", "qUCB", "qPOI", "qKG", "optimize_acq", "ei", "ucb", "poi", "ue",
+           "compute_penalty"]
 
 
 # ------------------------------------------------------------------ base functions on moments (base_acq.py:20-155)
@@ -192,6 +193,12 @@ def _q_acq(kind, rng_key, model, X, best_f, param, maximize, noiseless, maximize
         out = model._posterior_batched(Xq, samples, True, noiseless, ("mean", "var"), **kwargs)
         return model.ctx.acq_moments(kind, out["mean"], out["var"], best_f, param, maximize)
 
+    return _q_select(rows, rng_key, model, X, maximize_distance, subsample_size, n_evals, indices)
+
+
+def _q_select(rows, rng_key, model, X, maximize_distance, subsample_size, n_evals, indices):
+    """batch_acquisition.py:34-57: rows(samples, X) of one random subsample of the draws, or of the subsample (out of
+    n_evals) whose per-draw maximisers lie farthest apart"""
     if not maximize_distance:
         return rows(_subsample(model.get_samples(), subsample_size, rng_key), X)
     X_ = np.asarray(indices) if indices is not None else X
@@ -223,3 +230,189 @@ def qPOI(rng_key, model, X, best_f: float = None, xi: float = 0.01, maximize: bo
     """batch_acquisition.py:178-232."""
     return _q_acq("POI", rng_key, model, X, best_f, xi, maximize, noiseless, maximize_distance, subsample_size, n_evals,
                   indices, **kwargs)
+
+
+def qKG(rng_key, model, X, n: int = 10, maximize: bool = False, noiseless: bool = False, maximize_distance: bool = False,
+        subsample_size: int = 1, n_evals: int = 10, indices=None, **kwargs):
+    """batch_acquisition.py:235-282: kg() of each sub-sampled posterior draw, one row per draw ([subsample_size, P]),
+    with the draw sub-sampling and the `maximize_distance` selection of the other q-batch functions.  Every draw's kg()
+    uses `rng_key` for its simulated observations, as the reference's single_acq does."""
+    if getattr(model, "mcmc", None) is None:
+        raise ValueError("The model needs to be fully Bayesian")
+    X = np.asarray(X)
+    X = X[:, None] if X.ndim < 2 else X
+
+    def rows(samples, Xq):
+        S = len(next(iter(samples.values())))
+        return np.stack([kg(model, Xq, {k: np.asarray(v)[s] for k, v in samples.items()}, rng_key, n, maximize, noiseless,
+                            **kwargs) for s in range(S)])
+
+    return _q_select(rows, rng_key, model, X, maximize_distance, subsample_size, n_evals, indices)
+
+
+# ------------------------------------------------------------------ Thompson sampling (acquisition.py:487-524)
+def Thompson(rng_key, model, X, n: int = 1, noiseless: bool = False, **kwargs):
+    """Thompson sampling -- acquisition.py:487-524.  MCMC model: one hyper-parameter draw picked by
+    `prng.randint(rng_key, (1,), 0, S)` (jax.random.randint), then `predict` with that draw and `rng_key`; the n samples
+    are averaged when n > 1.  Otherwise the reference calls `model.sample_from_posterior`, which ExactGP and viGP do
+    not have (there as here), so they raise AttributeError."""
+    if getattr(model, "mcmc", None) is not None:
+        posterior_samples = model.get_samples()
+        idx = prng.randint(prng.as_key(rng_key), (1,), 0, len(posterior_samples["k_length"]))
+        samples = {k: np.asarray(v)[idx] for k, v in posterior_samples.items()}
+        _, tsample = model.predict(rng_key, X, samples, n, noiseless=noiseless, **kwargs)
+        if n > 1:
+            tsample = tsample.mean(1).squeeze()
+        return tsample
+    _, tsample = model.sample_from_posterior(rng_key, X, n=1, noiseless=noiseless, **kwargs)
+    return tsample
+
+
+# ------------------------------------------------------------------ optimize_acq (optimize.py)
+def ensure_array(x):
+    """optimize.py:91-97: a float becomes [x]; a list, tuple or array becomes an array; anything else (an int included)
+    is a TypeError."""
+    if isinstance(x, np.ndarray):
+        return x
+    if isinstance(x, (list, tuple, float)):
+        return np.array([x]) if isinstance(x, float) else np.array(x)
+    raise TypeError(f"Expected input to be a list, tuple, float, or jnp.ndarray, got {type(x)} instead.")
+
+
+def _pdf(u):
+    return np.exp(-0.5 * u * u - 0.9189385332046727)
+
+
+def acq_value_grad(kind, mean, var, dmean, dvar, eps=None, best_f=None, param=0.0, maximize=False):
+    """Value and gradient w.r.t. x of the acquisition function `kind` ('EI', 'UCB', 'POI', 'UE') at ONE test point x.
+
+    mean, var [S] and dmean, dvar [S, d] are the per-draw posterior moments at x and their gradients.  eps None: S == 1
+    and the moments are used directly (the viGP / MAP branch of acquisition.py:35).  eps [S, n]: the reference's
+    reparameterised samples y[s, i] = mean[s] + sqrt(var[s]) eps[s, i] (chol of the 1 x 1 covariance is sqrt(var)) are
+    pooled into their mean and population variance (acquisition.py:31-34), and both are differentiated through the
+    samples.  best_f None is the moments' own mean, as base_acq.py:59-60 takes it over one point, and is differentiated
+    too (so EI's u is 0 and its value sigma * phi(0), as jax.grad of the reference gives).  param is beta (UCB) or
+    xi (POI).  Returns (value, gradient [d])."""
+    from scipy.special import ndtr
+    mean, var = np.asarray(mean, np.float64).reshape(-1), np.asarray(var, np.float64).reshape(-1)
+    dmean, dvar = np.asarray(dmean, np.float64).reshape(mean.size, -1), np.asarray(dvar, np.float64).reshape(mean.size, -1)
+    if eps is None:
+        M, V, dM, dV = mean[0], var[0], dmean[0], dvar[0]
+    else:
+        eps = np.asarray(eps, np.float64).reshape(mean.size, -1)
+        sd = np.sqrt(var)
+        y = mean[:, None] + sd[:, None] * eps                                        # [S, n]
+        dy = dmean[:, None, :] + (dvar / (2.0 * sd[:, None]))[:, None, :] * eps[:, :, None]   # [S, n, d]
+        R = y.size
+        M = y.mean()
+        V = ((y - M) ** 2).mean()
+        dM = dy.reshape(R, -1).mean(0)
+        dV = 2.0 * ((y - M).reshape(R, 1) * (dy.reshape(R, -1) - dM)).mean(0)
+    sigma = np.sqrt(V)
+    dsigma = dV / (2.0 * sigma)
+    sgn = 1.0 if maximize else -1.0
+    if kind == "UE":                                                                 # base_acq.py:129-130
+        return sigma, dsigma
+    if kind == "UCB":                                                                # base_acq.py:97-103
+        delta = np.sqrt(param * V)
+        ddelta = param * dV / (2.0 * delta)
+        return sgn * M + delta, sgn * dM + ddelta
+    best, dbest = (M, dM) if best_f is None else (float(best_f), 0.0)
+    if kind == "EI":                                                                 # base_acq.py:59-69
+        u = sgn * (M - best) / sigma
+        return sigma * (_pdf(u) + u * ndtr(u)), dsigma * _pdf(u) + sgn * ndtr(u) * (dM - dbest)
+    if kind == "POI":                                                                # base_acq.py:148-155
+        u = sgn * (M - best - param) / sigma
+        du = sgn * (dM - dbest) / sigma - u * dsigma / sigma
+        return ndtr(u), _pdf(u) * du
+    raise ValueError(f"no analytic gradient for {kind}")
+
+
+# the acquisition functions with an analytic gradient, and the keyword that carries their parameter
+_ANALYTIC = {"EI": None, "UCB": "beta", "POI": "xi", "UE": None}
+_DEFAULT_PARAM = {"EI": 0.0, "UCB": 0.25, "POI": 0.01, "UE": 0.0}
+
+
+def _analytic_kind(acq_fn, model, kwargs):
+    """'EI' / 'UCB' / 'POI' / 'UE' when acq_fn is one of them and the gradient can be had in closed form, else None.
+
+    Only a plain ExactGP or viGP qualifies: their predict() is the exact-GP posterior that b2gp_posterior_grad
+    differentiates.  Every subclass (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, or a user's own) predicts
+    something else, so it takes the finite-difference branch even though it inherits _posterior_grad."""
+    from .gp import ExactGP
+    from .vigp import viGP
+    kind = {EI: "EI", UCB: "UCB", POI: "POI", UE: "UE"}.get(acq_fn)
+    if kind is None or kwargs.get("penalty") or type(model) not in (ExactGP, viGP):
+        return None
+    if model.mean_fn is not None or model._fused is None:
+        return None
+    return kind
+
+
+def _analytic_objective(kind, rng_key, model, d, kwargs):
+    """x [d] -> (acq(x), d acq / dx) through one b2gp_posterior_grad call per evaluation"""
+    from .gp import _eps_dtype
+    kw = dict(kwargs)
+    n = int(kw.pop("n", 1))
+    noiseless = bool(kw.pop("noiseless", False))
+    maximize = bool(kw.pop("maximize", False))
+    best_f = kw.pop("best_f", None) if kind in ("EI", "POI") else None
+    pname = _ANALYTIC[kind]
+    param = float(kw.pop(pname, _DEFAULT_PARAM[kind])) if pname else 0.0
+    for k in ("penalty", "recent_points", "grid_indices", "penalty_factor"):
+        kw.pop(k, None)
+    if kind == "UE":
+        maximize = False
+    mcmc = getattr(model, "mcmc", None) is not None
+    samples = model.get_samples()
+    S = len(next(iter(samples.values()))) if mcmc else 1
+    eps = posterior_eps(rng_key, S, n, 1, _eps_dtype())[:, :, 0] if mcmc else None
+
+    def f(x):
+        mean, var, dmean, dvar = model._posterior_grad(np.asarray(x, np.float64).reshape(1, d), samples, mcmc, noiseless, **kw)
+        return acq_value_grad(kind, mean[:, 0], var[:, 0], dmean[:, 0, :], dvar[:, 0, :], eps, best_f, param, maximize)
+    return f
+
+
+def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, upper_bound, **kwargs):
+    """Maximise `acq_fn` over the box [lower_bound, upper_bound] -- gpax/acquisition/optimize.py:19-88.
+
+    The acquisition is evaluated at `num_initial_guesses` uniform points (jax.random.uniform on `rng_key`, float32
+    unless x64 is enabled), and L-BFGS-B (scipy.optimize.minimize, the routine jaxopt's ScipyBoundedMinimize wraps;
+    maxiter 500 as jaxopt's default) minimises -acq(x) from the best of them, x shaped (1, d) for each evaluation.
+
+    The reference differentiates the acquisition w.r.t. x with JAX.  Here EI, UCB, POI and UE without a penalty, on a
+    model with a built-in kernel and no mean function, get the same gradient in closed form from the posterior's own
+    derivatives w.r.t. the test input (b2gp_posterior_grad: one posterior call per evaluation, value and gradient
+    together).  Every other acquisition (KG, Thompson, the q-batch functions, penalties, user callables, mean
+    functions) is handed to L-BFGS-B without a gradient: SciPy then takes finite differences, d + 1 posterior calls per
+    gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
+    guess, [d], or a 0-d array in one dimension."""
+    from scipy.optimize import minimize
+    from .utils import x64_enabled
+    lower_bound = ensure_array(lower_bound)
+    upper_bound = ensure_array(upper_bound)
+    dt = np.float64 if x64_enabled() else np.float32
+    d = lower_bound.shape[0]
+    guesses = prng.uniform(prng.as_key(rng_key), (num_initial_guesses, d), dt,
+                           np.asarray(lower_bound, dt), np.asarray(upper_bound, dt))
+    initial_acq_vals = np.asarray(acq_fn(rng_key, model, guesses, **kwargs))
+    x0 = np.asarray(guesses[initial_acq_vals.argmax()]).squeeze()
+    shape = x0.shape
+    bounds = list(zip(np.broadcast_to(lower_bound, (d,)).astype(float), np.broadcast_to(upper_bound, (d,)).astype(float)))
+    kind = _analytic_kind(acq_fn, model, kwargs)
+    if kind is not None:
+        f = _analytic_objective(kind, rng_key, model, d, kwargs)
+
+        def fun(x):
+            v, g = f(x)
+            return -float(v), -np.asarray(g, np.float64).reshape(-1)
+        res = minimize(fun, np.asarray(x0, np.float64).reshape(-1), jac=True, method="L-BFGS-B", bounds=bounds,
+                       options={"maxiter": 500})
+    else:
+        def fun(x):   # optimize.py:70-74
+            x = np.array([x]).reshape(1, -1)
+            return -float(np.asarray(acq_fn(rng_key, model, x, **kwargs)).reshape(()))
+        res = minimize(fun, np.asarray(x0, np.float64).reshape(-1), jac=None, method="L-BFGS-B", bounds=bounds,
+                       options={"maxiter": 500})
+    return np.asarray(res.x, dtype=dt).reshape(shape)

@@ -12,6 +12,7 @@
 #include "gram.cuh"
 #include "mll.cuh"
 #include "posterior.cuh"
+#include "grad.cuh"
 #include "potrf.cuh"
 #include "sparse_elbo.cuh"
 #include "acq.cuh"
@@ -577,11 +578,13 @@ __global__ void add_diag_vec_kernel(double* A, int64_t ld, int64_t n, const doub
 // The posterior with everything that may vary per draw: the training inputs (xtr_stride doubles between draws; 0 =
 // shared), the test inputs (xnew_stride), the targets (yres_stride) and an optional vector of per-point noise variances
 // added to the diagonal of k_XX (nv_stride between draws; 0 = shared).  b2gp_posterior is the all-shared special case.
+// With B2GP_OUT_DMEAN / B2GP_OUT_DVAR (b2gp_posterior_grad only) the P*d derivative rows of grad.cuh ride under
+// [k_pX; y^T] through the same factorisation or solve, and dmean / dvar [S, P, d] are their row dots.
 static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xtr_stride, int64_t N, const double* yres,
                           int64_t yres_stride, const double* Xnew, int64_t xnew_stride, int64_t P, int d, int64_t S,
                           const double* theta, const double* noise_vec, int64_t nv_stride, int noiseless, double jitter,
                           unsigned flags, double* mean, double* var, double* cov, const double* eps, int64_t n_samp,
-                          double* y_sampled, int* info, b2gp_timing* timing) {
+                          double* y_sampled, int* info, b2gp_timing* timing, double* dmean_out = nullptr, double* dvar_out = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, xtr_stride == 0 || xtr_stride >= N * d);
@@ -592,6 +595,11 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     ARG_CHECK(ctx, yres_stride == 0 || yres_stride >= N);
     const bool want_mean = flags & B2GP_OUT_MEAN, want_var = flags & B2GP_OUT_VAR;
     const bool want_cov = flags & B2GP_OUT_COV, want_samp = flags & B2GP_OUT_SAMPLE;
+    const bool want_dmean = flags & B2GP_OUT_DMEAN, want_dvar = flags & B2GP_OUT_DVAR;
+    ARG_CHECK(ctx, !want_dmean || dmean_out);
+    ARG_CHECK(ctx, !want_dvar || dvar_out);
+    // rows of the slot's right-hand side block: [k_pX (P); y^T (1); D (G = P*d derivative rows, gradient calls only)]
+    const int64_t G = (want_dmean || want_dvar) ? P * d : 0, R = P + 1 + G;
     ARG_CHECK(ctx, !want_mean || mean);
     ARG_CHECK(ctx, !want_var || var);
     ARG_CHECK(ctx, !want_cov || cov);
@@ -619,7 +627,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
 
     // ---- outputs
-    double *dmean = mean, *dvar = var, *dcov = cov, *dsamp = y_sampled;
+    double *dmean = mean, *dvar = var, *dcov = cov, *dsamp = y_sampled, *ddmean = dmean_out, *ddvar = dvar_out;
     if (!dev || f32) {
         if (want_mean) {
             RET_IF(ensure(ctx, ctx->d_out[0], (size_t)S * P * 8));
@@ -637,6 +645,15 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             RET_IF(ensure(ctx, ctx->d_out[3], (size_t)S * n_samp * P * 8));
             dsamp = (double*)ctx->d_out[3].p;
         }
+        // a gradient call has no covariance or samples: their staging buffers take dmean / dvar
+        if (want_dmean) {
+            RET_IF(ensure(ctx, ctx->d_out[2], (size_t)S * P * d * 8));
+            ddmean = (double*)ctx->d_out[2].p;
+        }
+        if (want_dvar) {
+            RET_IF(ensure(ctx, ctx->d_out[3], (size_t)S * P * d * 8));
+            ddvar = (double*)ctx->d_out[3].p;
+        }
     }
     RET_IF(ensure(ctx, ctx->d_info, (size_t)2 * S * sizeof(int)));
     int* dinfo = (int*)ctx->d_info.p;
@@ -649,7 +666,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     const bool need_cov = want_cov || want_samp;
     for (int q = 0; q < nslots; ++q) {
         Slot& sl = ctx->slots[q];
-        const size_t needA = (size_t)(N + P + 1) * ldA * 8;
+        const size_t needA = (size_t)(N + R) * ldA * 8;
         if (q == 0 && ctx->fcache.valid && ctx->fcache.N == N && sl.A.p && sl.A.cap < needA) {
             // slot 0's matrix holds the cached factor and this call brings more test points than the one that made it:
             // grow the buffer AROUND the factor (a plain ensure() would free it and the reuse below would read garbage)
@@ -727,6 +744,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             // k_pX = kernel(X_new, X_train, params, jitter=0.0)  (gp.py:268); same-shape inputs add 0 there
             RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, 0.0, 0.0, 0, 0, Vt, ldV));
             CUDA_TRY(ctx, cudaMemcpyAsync(Vt + P * ldV, dy + (yres_stride ? s * yres_stride : 0), (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
+            if (G) RET_IF(launch_gram_dx(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, Vt + (P + 1) * ldV, ldV));
             return B2GP_OK;
         };
         if (!reuse) {
@@ -738,7 +756,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
             if (fused_solve) count_path(ctx, PATH_POTRF_TALL);
             if (fused_solve)
-                RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, P + 1, Linv, inf, 0, keepU ? (double*)ctx->Ukeep.p : nullptr));
+                RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, R, Linv, inf, 0, keepU ? (double*)ctx->Ukeep.p : nullptr));
             else
                 RET_IF(potrf_rec(ctx, st, A, ldA, N, Linv, inf, 0));
         } else {
@@ -751,9 +769,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         // [V^T; w^T] = [k_pX; y^T] L^{-T}
         if (!fused_solve) {
             if (reuse && ctx->fcache.U_nb > 0 && ctx->fcache.U_nb == ctx->panel && ctx->ozaki != 0)
-                RET_IF(trsm_tall(ctx, st, Vt, ldV, P + 1, A, ldA, N, (const double*)ctx->Ukeep.p, ctx->fcache.U_nb));
+                RET_IF(trsm_tall(ctx, st, Vt, ldV, R, A, ldA, N, (const double*)ctx->Ukeep.p, ctx->fcache.U_nb));
             else
-                RET_IF(trsm_rec(ctx, st, Vt, ldV, P + 1, A, ldA, N, Linv));
+                RET_IF(trsm_rec(ctx, st, Vt, ldV, R, A, ldA, N, Linv));
         }
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[4], st));
         // mean / var
@@ -761,6 +779,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         if (want_mean || want_var || want_samp)
             RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, kind, d, th, noise_mult_new, jitter, inf, mean_s,
                           want_var ? dvar + s * P : nullptr));
+        if (G)
+            RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_grad_kernel, Vt, ldV, N, P, d, inf,
+                          want_dmean ? ddmean + s * P * d : nullptr, want_dvar ? ddvar + s * P * d : nullptr));
         if (need_cov) {
             sl.oz_planes = 7;
             // cov = k_pp - V^T V  (gp.py:267, 272), lower tiles then mirrored -> exactly symmetric
@@ -820,6 +841,8 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     if (want_var) RET_IF(store_out(ctx, st0, ctx->f32_out[1], var, P, dvar, P, S, P, dev, f32));
     if (want_cov) RET_IF(store_out(ctx, st0, ctx->f32_out[2], cov, P, dcov, P, S * P, P, dev, f32));
     if (want_samp) RET_IF(store_out(ctx, st0, ctx->f32_out[3], y_sampled, P, dsamp, P, S * n_samp, P, dev, f32));
+    if (want_dmean) RET_IF(store_out(ctx, st0, ctx->f32_out[2], dmean_out, P * d, ddmean, P * d, S, P * d, dev, f32));
+    if (want_dvar) RET_IF(store_out(ctx, st0, ctx->f32_out[3], dvar_out, P * d, ddvar, P * d, S, P * d, dev, f32));
     CUDA_TRY(ctx, cudaEventRecord(ev_d, st0));
     RET_IF(tm.end(st0, nullptr));
     for (int q = 0; q < B2GP_MAX_STREAMS; ++q) ctx->slots[q].oz_planes = 7;   // other entry points: the conservative count
@@ -862,6 +885,10 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     const double n = (double)N, p = (double)P;
     t.flops = (double)S * (n * n * n / 3.0 + n * n * (p + 1.0) + 4.0 * n * p + (need_cov ? n * p * p : 0.0));
     t.gram_bytes = (double)S * (8.0 * n * n / 2.0 + 8.0 * n * p + (need_cov ? 8.0 * p * p : 0.0));
+    if (G) {   // the derivative rows: their solve and row dots, and the bytes gram_dx_kernel writes
+        t.flops += (double)S * (n * n * (double)G + 4.0 * n * (double)G);
+        t.gram_bytes += (double)S * 8.0 * n * (double)G;
+    }
     if (timing) *timing = t;
     return B2GP_OK;
 }
@@ -870,8 +897,8 @@ extern "C" int b2gp_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, int64_
                               const double* Xnew, int64_t P, int d, int64_t S, const double* theta, int noiseless, double jitter,
                               unsigned flags, double* mean, double* var, double* cov, const double* eps, int64_t n_samp,
                               double* y_sampled, int* info, b2gp_timing* timing) {
-    return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
-                          var, cov, eps, n_samp, y_sampled, info, timing);
+    return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter,
+                          flags & ~(unsigned)(B2GP_OUT_DMEAN | B2GP_OUT_DVAR), mean, var, cov, eps, n_samp, y_sampled, info, timing);
 }
 
 extern "C" int b2gp_posterior_batch(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xtr_stride, int64_t N, const double* yres,
@@ -880,7 +907,22 @@ extern "C" int b2gp_posterior_batch(b2gp_ctx* ctx, int kind, const double* Xtr, 
                                     double jitter, unsigned flags, double* mean, double* var, double* cov, const double* eps,
                                     int64_t n_samp, double* y_sampled, int* info, b2gp_timing* timing) {
     return posterior_impl(ctx, kind, Xtr, xtr_stride, N, yres, yres_stride, Xnew, xnew_stride, P, d, S, theta, noise_vec,
-                          noise_vec_stride, noiseless, jitter, flags, mean, var, cov, eps, n_samp, y_sampled, info, timing);
+                          noise_vec_stride, noiseless, jitter, flags & ~(unsigned)(B2GP_OUT_DMEAN | B2GP_OUT_DVAR), mean, var, cov,
+                          eps, n_samp, y_sampled, info, timing);
+}
+
+// The posterior and its gradient w.r.t. the test inputs (grad.cuh); the derivative rows share the factorisation (or the
+// cached factor) with [k_pX; y^T].  fp64 arrays only, shared inputs, no covariance or samples.
+extern "C" int b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t N, const double* yres, int64_t yres_stride,
+                                   const double* Xnew, int64_t P, int d, int64_t S, const double* theta, int noiseless, double jitter,
+                                   unsigned flags, double* mean, double* var, double* dmean, double* dvar, int* info,
+                                   b2gp_timing* timing) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (flags & (B2GP_FLAG_F32 | B2GP_OUT_COV | B2GP_OUT_SAMPLE))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_posterior_grad", "fp64 arrays, outputs mean / var / dmean / dvar only",
+                       __FILE__, __LINE__);
+    return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
+                          var, nullptr, nullptr, 0, nullptr, info, timing, dmean, dvar);
 }
 
 // ------------------------------------------------------------------------------------------ sparse posterior

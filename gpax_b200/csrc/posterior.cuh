@@ -53,6 +53,62 @@ rowdot_kernel(const double* __restrict__ Vt, int64_t ldv, int64_t N, int64_t P, 
     }
 }
 
+// Gradients w.r.t. the test inputs (grad.cuh): the solved derivative rows G = Vt + (P + 1) * ldv, row p*d + k being
+// L^{-1} dk(X, x_p)/dx_p[k]; dmean[p, k] = <G[p*d+k], w>, dvar[p, k] = -2 <G[p*d+k], V_p>.  One CTA per test point, the
+// same fixed-order reduction as rowdot_kernel (deterministic), GRD_KC derivative rows per pass over V_p and w.
+constexpr int GRD_KC = 4;
+__global__ void __launch_bounds__(RD_THREADS)
+rowdot_grad_kernel(const double* __restrict__ Vt, int64_t ldv, int64_t N, int64_t P, int d, const int* __restrict__ info,
+                   double* __restrict__ dmean, double* __restrict__ dvar) {
+    __shared__ double red1[GRD_KC][RD_THREADS / 32], red2[GRD_KC][RD_THREADS / 32];
+    const int64_t p = blockIdx.x;
+    const double* v = Vt + p * ldv;
+    const double* w = Vt + P * ldv;
+    const double* G = Vt + (P + 1 + p * d) * ldv;
+    const bool bad = (*info != 0);
+    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    for (int k0 = 0; k0 < d; k0 += GRD_KC) {
+        double s1[GRD_KC], s2[GRD_KC];
+#pragma unroll
+        for (int j = 0; j < GRD_KC; ++j) s1[j] = s2[j] = 0.0;
+        for (int64_t i = threadIdx.x; i < N; i += RD_THREADS) {
+            const double wi = w[i], vi = v[i];
+#pragma unroll
+            for (int j = 0; j < GRD_KC; ++j) {
+                if (k0 + j < d) {
+                    const double g = G[(int64_t)(k0 + j) * ldv + i];
+                    s1[j] = fma(g, wi, s1[j]);
+                    s2[j] = fma(g, vi, s2[j]);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < GRD_KC; ++j) {
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                s1[j] += __shfl_xor_sync(0xffffffffu, s1[j], o);
+                s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], o);
+            }
+            if ((threadIdx.x & 31) == 0) {
+                red1[j][threadIdx.x >> 5] = s1[j];
+                red2[j][threadIdx.x >> 5] = s2[j];
+            }
+        }
+        __syncthreads();
+        if (threadIdx.x < GRD_KC && k0 + (int)threadIdx.x < d) {
+            const int j = threadIdx.x;
+            double a = 0.0, b = 0.0;
+            for (int i = 0; i < RD_THREADS / 32; ++i) {
+                a += red1[j][i];
+                b += red2[j][i];
+            }
+            if (dmean) dmean[p * d + k0 + j] = bad ? nan : a;
+            if (dvar) dvar[p * d + k0 + j] = bad ? nan : -2.0 * b;
+        }
+        __syncthreads();
+    }
+}
+
 // C[j][i] = C[i][j] for j < i
 __global__ void mirror_lower_kernel(double* C, int64_t ld, int64_t n) {
     const int64_t i = (int64_t)blockIdx.y * 32 + threadIdx.y;

@@ -175,6 +175,20 @@ class ExactGP:
                 out["y_sampled"] = out["y_sampled"] + (pm[:, None, :] if pm.ndim == 2 else pm)
         return out
 
+    def _posterior_grad(self, X_new, params, batched, noiseless, **kwargs):
+        """Per-draw posterior mean [S, P], variance [S, P] and their gradients w.r.t. the test inputs dmean, dvar
+        [S, P, d] (b2gp_posterior_grad): what jax.grad through the acquisition w.r.t. x needs (optimize.py:70-88).  fp32
+        inputs are cast to fp64 here.  A model with a mean function has no analytic gradient (the mean function is an
+        arbitrary host callable), nor has a user kernel callable.  Subclasses inherit this method but predict a different
+        posterior; acquisition.optimize_acq uses it for ExactGP and viGP only."""
+        if self.mean_fn is not None or self._fused is None:
+            raise NotImplementedError("posterior gradients need a built-in kernel and no mean function")
+        X, y = self._train_arrays()
+        Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
+        theta = _theta_rows(params, X.shape[1], batched)
+        out = self.ctx.posterior_grad(self._fused, X, y, Xn, theta, noiseless, float(kwargs.get("jitter", 1e-6)))
+        return out["mean"], out["var"], out["dmean"], out["dvar"]
+
     def get_mvn_posterior(self, X_new, params: Dict[str, np.ndarray], noiseless: bool = False,
                           **kwargs: float) -> Tuple[np.ndarray, np.ndarray]:
         """

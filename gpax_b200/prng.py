@@ -119,6 +119,24 @@ def uniform(key, shape, dtype=np.float32, minval=0.0, maxval=1.0, partitionable:
     return np.maximum(lo, floats * (hi - lo) + lo).astype(dtype)
 
 
+def randint(key, shape, minval, maxval, partitionable: bool = False) -> np.ndarray:
+    """jax.random.randint for int32 results (the JAX 0.4 algorithm): split the key, draw two 32-bit words hi and lo, and
+    reduce ((hi % span) * ((2**16 % span)**2 % span) + lo % span) % span in uint32 arithmetic, plus minval; span = 1
+    when maxval <= minval (every draw is minval).  JAX is not installed here, so unlike split / normal this restatement
+    is not pinned to a value JAX published; it follows the algorithm, not a known answer."""
+    shape = tuple(int(s) for s in shape)
+    minval, maxval = int(minval), int(maxval)
+    k1, k2 = split(key, 2, partitionable)
+    hi = random_bits(k1, 32, shape, partitionable)
+    lo = random_bits(k2, 32, shape, partitionable)
+    span = _U32(maxval - minval if maxval > minval else 1)
+    with np.errstate(over="ignore"):
+        mult = _U32(2 ** 16) % span
+        mult = (mult * mult) % span
+        off = ((hi % span) * mult + lo % span) % span
+    return (off.astype(np.int64) + minval).astype(np.int32)
+
+
 def normal(key, shape, dtype=np.float32, partitionable: bool = False) -> np.ndarray:
     """jax.random.normal: sqrt(2) * erfinv(u), u uniform on (-1, 1)."""
     dtype = np.dtype(dtype)

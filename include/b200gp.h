@@ -60,7 +60,9 @@ enum {
     B2GP_OUT_MEAN         = 1u << 4, /* b2gp_posterior: produce mean[S,P]                                    */
     B2GP_OUT_VAR          = 1u << 5, /* ... var[S,P] = diag(cov)     (viGP.predict, vigp.py:184-185)         */
     B2GP_OUT_COV          = 1u << 6, /* ... cov[S,P,P]               (get_mvn_posterior, gp.py:272)          */
-    B2GP_OUT_SAMPLE       = 1u << 7  /* ... y_sampled[S,n,P] = mean + chol(cov) eps   (gp.py:292)            */
+    B2GP_OUT_SAMPLE       = 1u << 7, /* ... y_sampled[S,n,P] = mean + chol(cov) eps   (gp.py:292)            */
+    B2GP_OUT_DMEAN        = 1u << 8, /* b2gp_posterior_grad: dmean[S,P,d] = d mean[s,p] / d Xnew[p,:]        */
+    B2GP_OUT_DVAR         = 1u << 9  /* ... dvar[S,P,d] = d var[s,p] / d Xnew[p,:]                            */
 };
 
 /* per-call device timing (CUDA events on the library's own streams), filled when non-NULL.
@@ -192,6 +194,22 @@ int  b2gp_posterior_batch(b2gp_ctx* ctx, int kind,
                           double* mean, double* var, double* cov,
                           const double* eps, int64_t n_samp, double* y_sampled,
                           int* info, b2gp_timing* timing);
+
+/* The posterior and its gradient w.r.t. the test inputs -- what jax.grad of the acquisition w.r.t. x needs in
+ * gpax/acquisition/optimize.py:70-88 (optimize_acq).  Arguments as b2gp_posterior; flags: any of B2GP_OUT_MEAN,
+ * B2GP_OUT_VAR, B2GP_OUT_DMEAN, B2GP_OUT_DVAR, plus B2GP_FLAG_DEVICE_PTRS.  B2GP_FLAG_F32, B2GP_OUT_COV and B2GP_OUT_SAMPLE
+ * give B2GP_ERR_UNSUPPORTED.  Kinds RBF, Matern-5/2, Periodic.
+ *   dmean[S,P,d]  d mean[s,p] / d Xnew[p,k]
+ *   dvar[S,P,d]   d var[s,p]  / d Xnew[p,k]   (k(x, x) is constant, so the same with and without noiseless)
+ * The P*d rows d k(Xnew[p], X) / d Xnew[p,k] are solved with the factor of k_XX like k_pX.  mean and var are those of
+ * b2gp_posterior for the same inputs, bit for bit under the default "ozaki" = 0.  Under the int8 options (ozaki != 0) the
+ * extra rows can move a GEMM of the factorisation or solve to the other side of a dispatch threshold (trsm_rec's
+ * 1024-row panel route, the "oz_min_tiles" tile count); mean and var then agree within the digit-plane error.  NaN
+ * outputs where info[s] != 0.  Single-draw host-pointer calls share the factor cache of b2gp_posterior.              */
+int  b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t N, const double* yres, int64_t yres_stride,
+                         const double* Xnew, int64_t P, int d, int64_t S, const double* theta, int noiseless, double jitter,
+                         unsigned flags, double* mean, double* var, double* dmean, double* dvar,
+                         int* info, b2gp_timing* timing);
 
 /* Nystrom / VFE sparse posterior for one theta -- replaces viSparseGP.get_mvn_posterior
  * (gpax/models/sparse_gp.py:173-223).  Xu[M,d] inducing points; theta[d+3] as above;
