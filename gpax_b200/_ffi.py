@@ -76,6 +76,11 @@ SIGNATURES = {
                                        C.c_int64, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_posterior_grad": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int, C.c_int64,
                                       _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
+    "b2gp_posterior_multitask": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int, C.c_int,
+                                           C.c_int, C.c_int, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp,
+                                           _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
+    "b2gp_mll_multitask": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp,
+                                     C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _ip]),
     "b2gp_mll_v": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _ip]),
     "b2gp_sparse_posterior": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
                                         _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
@@ -438,6 +443,63 @@ class Context:
                                         _ptr(theta), _ptr(nv), float(jitter), 0, C.byref(val), _ptr(grad), _ptr(alpha), _ptr(gnv),
                                         C.byref(info)))
         return val.value, grad, alpha, info.value, gnv
+
+    def posterior_multitask(self, kind, Xtr, task_tr, yres, Xnew, task_new, theta, B, noise, group=1, noiseless=False, jitter=1e-6,
+                            want=("mean", "cov"), eps=None, timing=False, flags=0):
+        """The LCM posterior of MultiTaskGP / CoregGP (b2gp_posterior_multitask).  Xtr [N, d] and task_tr [N], Xnew [P, d] and
+        task_new [P] count rows (the Kronecker form is expanded by the caller, group = T); theta [S, L, d+2] rows
+        (lengthscale[d], k_scale, period), B [S, L, T, T], noise [S, T]; yres [N] or [S, N].  Outputs as posterior()."""
+        Xtr, Xnew = _f64(Xtr), _f64(Xnew)
+        N, d = Xtr.shape
+        P = Xnew.shape[0]
+        B = _f64(B)
+        S, L, T = B.shape[0], B.shape[1], B.shape[2]
+        theta, noise = _f64(theta, (S, L, d + 2)), _f64(noise, (S, T))
+        ttr, tnew = np.ascontiguousarray(task_tr, dtype=np.int32), np.ascontiguousarray(task_new, dtype=np.int32)
+        yres = _f64(yres)
+        stride = 0 if yres.ndim == 1 else yres.shape[1]
+        mean = var = cov = samp = None
+        if "mean" in want:
+            flags |= OUT_MEAN
+            mean = np.empty((S, P))
+        if "var" in want:
+            flags |= OUT_VAR
+            var = np.empty((S, P))
+        if "cov" in want:
+            flags |= OUT_COV
+            cov = np.empty((S, P, P))
+        n_samp = 0
+        if eps is not None:
+            eps = _f64(eps).reshape(S, -1, P)
+            n_samp = eps.shape[1]
+            flags |= OUT_SAMPLE
+            samp = np.empty((S, n_samp, P))
+        info = np.zeros(S, dtype=np.int32)
+        t = Timing()
+        self._check(self.lib.b2gp_posterior_multitask(
+            self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(Xtr), _ptr(ttr), N, _ptr(yres), stride, _ptr(Xnew), _ptr(tnew),
+            P, d, int(group), T, L, S, _ptr(theta), _ptr(B), _ptr(noise), int(bool(noiseless)), float(jitter), flags, _ptr(mean),
+            _ptr(var), _ptr(cov), _ptr(eps), n_samp, _ptr(samp), info.ctypes.data_as(_vp), C.byref(t) if timing else None))
+        out = {"mean": mean, "var": var, "cov": cov, "y_sampled": samp, "info": info}
+        if timing:
+            out["timing"] = t.as_dict()
+        return out
+
+    def mll_multitask(self, kind, X, task, yres, theta, B, noise, group=1, jitter=1e-6, want_grad=True, want_alpha=False, flags=0):
+        """The multi-task log marginal likelihood (b2gp_mll_multitask): X [N, d], task [N], theta [L, d+2], B [L, T, T],
+        noise [T].  Returns (value, grad_theta [L, d+2] (d/dlog), grad_B [L, T, T], grad_noise [T] (d/dlog), alpha, info)."""
+        X, yres, B = _f64(X), _f64(yres), _f64(B)
+        N, d = X.shape
+        L, T = B.shape[0], B.shape[1]
+        theta, noise = _f64(theta, (L, d + 2)), _f64(noise, (T,))
+        task = np.ascontiguousarray(task, dtype=np.int32)
+        val, info = C.c_double(0.0), C.c_int(0)
+        gt, gB, gn = (np.zeros((L, d + 2)), np.zeros((L, T, T)), np.zeros(T)) if want_grad else (None, None, None)
+        alpha = np.zeros(N) if want_alpha else None
+        self._check(self.lib.b2gp_mll_multitask(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(X), _ptr(task), N,
+                                                _ptr(yres), d, int(group), T, L, _ptr(theta), _ptr(B), _ptr(noise), float(jitter),
+                                                flags, C.byref(val), _ptr(gt), _ptr(gB), _ptr(gn), _ptr(alpha), C.byref(info)))
+        return val.value, gt, gB, gn, alpha, info.value
 
     def sparse_elbo(self, kind, Xu, X, yres, theta, jitter=1e-6):
         """VFE bound of the sparse GP, its gradient w.r.t. log(lengthscale[d], k_scale, noise, period) and w.r.t. Xu"""

@@ -13,6 +13,7 @@
 #include "mll.cuh"
 #include "posterior.cuh"
 #include "grad.cuh"
+#include "mtgp.cuh"
 #include "potrf.cuh"
 #include "sparse_elbo.cuh"
 #include "acq.cuh"
@@ -575,6 +576,16 @@ __global__ void add_diag_vec_kernel(double* A, int64_t ld, int64_t n, const doub
     if (i < n) A[i * ld + i] += v[i];
 }
 
+// The LCM covariance of MultiTaskGP / CoregGP (mtgp.cuh) in place of the single-task kernel: host arrays, task ids
+// validated by the caller.  nullptr for every single-task entry.
+struct MtDesc {
+    const int* task_tr;    // [N]
+    const int* task_new;   // [P] (posterior only)
+    int group, T, L;
+    const double* B;       // [S, L, T, T]
+    const double* noise;   // [S, T]
+};
+
 // The posterior with everything that may vary per draw: the training inputs (xtr_stride doubles between draws; 0 =
 // shared), the test inputs (xnew_stride), the targets (yres_stride) and an optional vector of per-point noise variances
 // added to the diagonal of k_XX (nv_stride between draws; 0 = shared).  b2gp_posterior is the all-shared special case.
@@ -584,7 +595,8 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                           int64_t yres_stride, const double* Xnew, int64_t xnew_stride, int64_t P, int d, int64_t S,
                           const double* theta, const double* noise_vec, int64_t nv_stride, int noiseless, double jitter,
                           unsigned flags, double* mean, double* var, double* cov, const double* eps, int64_t n_samp,
-                          double* y_sampled, int* info, b2gp_timing* timing, double* dmean_out = nullptr, double* dvar_out = nullptr) {
+                          double* y_sampled, int* info, b2gp_timing* timing, double* dmean_out = nullptr, double* dvar_out = nullptr,
+                          const MtDesc* mt = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, xtr_stride == 0 || xtr_stride >= N * d);
@@ -613,7 +625,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     auto slot_stream = [&](int q) { return ctx->slots[q].stream; };
 
     // ---- inputs
-    const int nth = d + 3;
+    const int nth = mt ? mt->L * (d + 2) : d + 3;
     const double *dXtr, *dy, *dXnew, *dtheta, *deps = nullptr, *dnv = nullptr;
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st0));
     // with B2GP_FLAG_F32 the data arrays (X, y, X_new, noise_vec, eps) are floats; theta stays double
@@ -623,6 +635,24 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     if (noise_vec) RET_IF(stage_in_t(ctx, st0, ctx->d_in[6], ctx->f32_in[6], noise_vec, (size_t)(nv_stride ? S * nv_stride : N), dev, f32, &dnv));
     RET_IF(stage_in(ctx, st0, ctx->d_in[3], theta, (size_t)S * nth * 8, dev, &dtheta));
     if (want_samp) RET_IF(stage_in_t(ctx, st0, ctx->d_in[4], ctx->f32_in[4], eps, (size_t)S * n_samp * P, dev, f32, &deps));
+    // multi-task: [B (S*L*T*T) | noise (S*T) | d+3 zeros] and the task ids [task_tr (N) | task_new (P)]
+    const double* dmt = nullptr;
+    const int* dtask = nullptr;
+    std::vector<double> hmt;
+    std::vector<int> htask;
+    if (mt) {
+        const size_t nb = (size_t)S * mt->L * mt->T * mt->T, nn = (size_t)S * mt->T;
+        hmt.assign(nb + nn + d + 3, 0.0);
+        memcpy(hmt.data(), mt->B, nb * 8);
+        memcpy(hmt.data() + nb, mt->noise, nn * 8);
+        htask.resize((size_t)(N + P));
+        memcpy(htask.data(), mt->task_tr, (size_t)N * 4);
+        memcpy(htask.data() + N, mt->task_new, (size_t)P * 4);
+        RET_IF(stage_in(ctx, st0, ctx->d_in[5], hmt.data(), hmt.size() * 8, false, &dmt));
+        const double* dt = nullptr;
+        RET_IF(stage_in(ctx, st0, ctx->d_in[7], htask.data(), htask.size() * 4, false, &dt));
+        dtask = (const int*)dt;
+    }
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st0));
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
 
@@ -680,7 +710,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
         if (need_cov) RET_IF(ensure(ctx, sl.cov, (size_t)P * ldC * 8));
         if (want_samp) RET_IF(ensure(ctx, sl.LinvC, (size_t)linv_bytes(P)));
-        if (!want_mean) RET_IF(ensure(ctx, sl.misc, (size_t)P * 8));
+        if (!want_mean || (mt && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)(mt ? 2 * P : P) * 8));
     }
     // inputs and the memset of dinfo were queued on st0: order the other streams behind them
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
@@ -689,7 +719,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
 
     // host copy of theta: the accuracy-aware digit-plane count of the int8 path is chosen per draw (oz_auto_planes)
     std::vector<double> htheta;
-    if (ctx->ozaki == -1) {
+    if (ctx->ozaki == -1 && !mt) {
         htheta.resize((size_t)S * nth);
         if (dev) {
             CUDA_TRY(ctx, cudaMemcpyAsync(htheta.data(), dtheta, (size_t)S * nth * 8, cudaMemcpyDeviceToHost, st0));
@@ -708,7 +738,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     // leaves it so, and it is re-validated -- together with the factor's `info` -- only after the call's work has
     // completed on the device (end of this function).
     bool reuse = false;
-    const bool cacheable = (S == 1 && !dev && !noise_vec);
+    const bool cacheable = (S == 1 && !dev && !noise_vec && !mt);
     if (cacheable) {
         auto& fc = ctx->fcache;
         const size_t xbytes = (size_t)N * d * (f32 ? 4 : 8);
@@ -739,17 +769,27 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             CUDA_TRY(ctx, cudaEventRecord(sev[s].e[0], st));
         }
         // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7
-        sl.oz_planes = (htheta.empty() || noise_vec) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
+        sl.oz_planes = (htheta.empty() || noise_vec || mt) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
+        const int T = mt ? mt->T : 0, L = mt ? mt->L : 0, grp = mt ? mt->group : 0;
+        const double* Bs = mt ? dmt + s * L * T * T : nullptr;
+        const double* ns = mt ? dmt + (size_t)S * L * T * T + s * T : nullptr;
+        const int *dtr = dtask, *dtn = mt ? dtask + N : nullptr;
         auto rhs_rows = [&]() -> int {
             // k_pX = kernel(X_new, X_train, params, jitter=0.0)  (gp.py:268); same-shape inputs add 0 there
-            RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, 0.0, 0.0, 0, 0, Vt, ldV));
+            if (mt)
+                RET_IF(launch_gram_lcm(ctx, st, LCM_RECT, kind, dXnew_s, dtn, P, dXtr_s, dtr, N, d, T, L, grp, th, Bs, ns, 0.0, 0.0, Vt, ldV));
+            else
+                RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, 0.0, 0.0, 0, 0, Vt, ldV));
             CUDA_TRY(ctx, cudaMemcpyAsync(Vt + P * ldV, dy + (yres_stride ? s * yres_stride : 0), (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
             if (G) RET_IF(launch_gram_dx(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, Vt + (P + 1) * ldV, ldV));
             return B2GP_OK;
         };
         if (!reuse) {
             // k_XX = kernel(X_train, X_train, params, noise, jitter)  (gp.py:269) -- lower triangle only
-            RET_IF(launch_gram(ctx, st, kind, dXtr_s, N, dXtr_s, N, d, th, 1.0, jitter, 1, 1, A, ldA));
+            if (mt)
+                RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dXtr_s, dtr, N, dXtr_s, dtr, N, d, T, L, grp, th, Bs, ns, 1.0, jitter, A, ldA));
+            else
+                RET_IF(launch_gram(ctx, st, kind, dXtr_s, N, dXtr_s, N, d, th, 1.0, jitter, 1, 1, A, ldA));
             if (dnv) RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ldA, N, dnv + s * nv_stride));
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
@@ -776,9 +816,21 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[4], st));
         // mean / var
         double* mean_s = want_mean ? dmean + s * P : (double*)sl.misc.p;
-        if (want_mean || want_var || want_samp)
+        if (mt) {   // var = prior diagonal - |V^T[p,:]|^2: rowdot_kernel on a zero prior (a periodic kernel of scale 0), then the LCM diagonal
+            const double* zero = dmt + (size_t)S * L * T * T + (size_t)S * T;
+            if (want_mean || want_var || want_samp)
+                RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, (int)B2GP_KERNEL_PERIODIC, d, zero, 0.0, 0.0, inf,
+                              mean_s, want_var ? dvar + s * P : nullptr));
+            if (want_var) {
+                double* prior = (double*)sl.misc.p + P;
+                RET_IF(launch_gram_lcm(ctx, st, LCM_DIAG, kind, dXnew_s, dtn, P, nullptr, nullptr, 0, d, T, L, grp, th, Bs, ns, noise_mult_new,
+                                       jitter, prior, 1));
+                RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, add_vec_kernel, dvar + s * P, (const double*)prior, P));
+            }
+        } else if (want_mean || want_var || want_samp) {
             RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, kind, d, th, noise_mult_new, jitter, inf, mean_s,
                           want_var ? dvar + s * P : nullptr));
+        }
         if (G)
             RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_grad_kernel, Vt, ldV, N, P, d, inf,
                           want_dmean ? ddmean + s * P * d : nullptr, want_dvar ? ddvar + s * P * d : nullptr));
@@ -787,7 +839,11 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             // cov = k_pp - V^T V  (gp.py:267, 272), lower tiles then mirrored -> exactly symmetric
             double* C = want_cov ? dcov + s * P * P : (double*)sl.cov.p;
             const int64_t ldc = want_cov ? P : ldC;
-            RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXnew_s, P, d, th, noise_mult_new, jitter, 1, 1, C, ldc));
+            if (mt)
+                RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dXnew_s, dtn, P, dXnew_s, dtn, P, d, T, L, grp, th, Bs, ns, noise_mult_new,
+                                       jitter, C, ldc));
+            else
+                RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXnew_s, P, d, th, noise_mult_new, jitter, 1, 1, C, ldc));
             RET_IF(gemm_nt(ctx, st, P, P, N, -1.0, Vt, ldV, Vt, ldV, 1.0, C, ldc, true));
             dim3 g2((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), b2(32, 32);
             RET_IF(launch(ctx, st, g2, b2, 0, mirror_lower_kernel, C, ldc, P));
@@ -923,6 +979,38 @@ extern "C" int b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, i
                        __FILE__, __LINE__);
     return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
                           var, nullptr, nullptr, 0, nullptr, info, timing, dmean, dvar);
+}
+
+// the common checks of the two multi-task entries: limits, host fp64 arrays, task ids in [0, T) (so that no kernel can
+// index B out of bounds) -- all before any launch
+static int mt_check(b2gp_ctx* ctx, const char* who, int kind, unsigned flags, int d, int group, int T, int L, const int* task1,
+                    int64_t n1, const int* task2, int64_t n2) {
+    if (flags & (B2GP_FLAG_DEVICE_PTRS | B2GP_FLAG_F32))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, who, "host fp64 arrays only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+    ARG_CHECK(ctx, T >= 1 && T <= MT_MAX_T && L >= 1 && L <= MT_MAX_L && d >= 1 && d <= MLL_MAX_D && group >= 1);
+    ARG_CHECK(ctx, task1 && n1 % group == 0 && (!task2 || n2 % group == 0));
+    for (int64_t i = 0; i < n1; ++i)
+        if (task1[i] < 0 || task1[i] >= T) return set_err(ctx, B2GP_ERR_ARG, who, "task id outside [0, T)", __FILE__, __LINE__);
+    for (int64_t i = 0; task2 && i < n2; ++i)
+        if (task2[i] < 0 || task2[i] >= T) return set_err(ctx, B2GP_ERR_ARG, who, "task id outside [0, T)", __FILE__, __LINE__);
+    return B2GP_OK;
+}
+
+// MultiTaskGP / CoregGP.get_mvn_posterior / predict (gp.py:253-293 with the LCM kernel, mtkernels.py:197-233): the
+// posterior of b2gp_posterior with the three Gram builds and the prior variance taken from gram_lcm_kernel.
+extern "C" int b2gp_posterior_multitask(b2gp_ctx* ctx, int kind, const double* Xtr, const int* task_tr, int64_t N, const double* yres,
+                                        int64_t yres_stride, const double* Xnew, const int* task_new, int64_t P, int d, int group, int T,
+                                        int L, int64_t S, const double* theta, const double* B, const double* noise, int noiseless,
+                                        double jitter, unsigned flags, double* mean, double* var, double* cov, const double* eps,
+                                        int64_t n_samp, double* y_sampled, int* info, b2gp_timing* timing) {
+    if (!ctx) return B2GP_ERR_ARG;
+    ARG_CHECK(ctx, B && noise && task_new && N >= 1 && P >= 1);
+    RET_IF(mt_check(ctx, "b2gp_posterior_multitask", kind, flags, d, group, T, L, task_tr, N, task_new, P));
+    const MtDesc mt{task_tr, task_new, group, T, L, B, noise};
+    return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter,
+                          flags & ~(unsigned)(B2GP_OUT_DMEAN | B2GP_OUT_DVAR), mean, var, cov, eps, n_samp, y_sampled, info, timing,
+                          nullptr, nullptr, &mt);
 }
 
 // ------------------------------------------------------------------------------------------ sparse posterior
@@ -1276,7 +1364,7 @@ __global__ void mll_diag_grad_kernel(const double* __restrict__ alpha, const dou
 
 static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, const double* theta,
                     const double* noise_vec, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
-                    double* grad_noise_vec, int* info) {
+                    double* grad_noise_vec, int* info, const MtDesc* mt = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, !grad_noise_vec || grad);
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
@@ -1289,18 +1377,36 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     cudaStream_t st = sl.stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
-    const int nth = d + 3;
-    const double *dX, *dy, *dth, *dnv = nullptr;
+    // multi-task: theta [L, d+2]; the gradient is [L, d+2] | [L, T, T] | [T] and the per-block partial sums of
+    // mll_lcm_grad_kernel are nout wide, L blocks of tiles^2
+    const int T = mt ? mt->T : 0, L = mt ? mt->L : 0;
+    const int nth = mt ? L * (d + 2) : d + 3;
+    const int ngrad = mt ? L * (d + 2) + L * T * T + T : nth, nout = d + 2 + T * T + T;
+    const double *dX, *dy, *dth, *dnv = nullptr, *dmt = nullptr;
+    const int* dtask = nullptr;
+    std::vector<double> hmt;
     RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, dev, &dX));
     RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)N * 8, dev, &dy));
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
     if (noise_vec) RET_IF(stage_in(ctx, st, ctx->d_in[6], noise_vec, (size_t)N * 8, dev, &dnv));
+    if (mt) {
+        hmt.resize((size_t)L * T * T + T);
+        memcpy(hmt.data(), mt->B, (size_t)L * T * T * 8);
+        memcpy(hmt.data() + (size_t)L * T * T, mt->noise, (size_t)T * 8);
+        RET_IF(stage_in(ctx, st, ctx->d_in[5], hmt.data(), hmt.size() * 8, false, &dmt));
+        const double* dt = nullptr;
+        RET_IF(stage_in(ctx, st, ctx->d_in[7], mt->task_tr, (size_t)N * 4, false, &dt));
+        dtask = (const int*)dt;
+    }
     const int64_t ld = round_up(N, 8);
     const int64_t tiles = ceil_div(N, MLL_TILE);
     RET_IF(ensure(ctx, sl.A, (size_t)(N + 1) * ld * 8));
     RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
     RET_IF(ensure(ctx, ctx->d_info, 64));
-    RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * nth) * 8));
+    if (mt)
+        RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + L * tiles * tiles * nout + L * nout) * 8));
+    else
+        RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * nth) * 8));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 8, st));
     double* A = (double*)sl.A.p;
@@ -1309,7 +1415,12 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     double* alpha = (double*)sl.misc.p + ld;   // K^{-1} y
     double* sc = alpha + ld;             // [0] sum log L_ii, [1] |w|^2, [8..8+nth) grad
     double* partial = sc + 64;
-    RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, dth, 1.0, jitter, 1, 1, A, ld));
+    double* gmt = partial + (size_t)L * tiles * tiles * nout;   // multi-task: per-latent column sums of the partials
+    if (mt)
+        RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dX, dtask, N, dX, dtask, N, d, T, L, mt->group, dth, dmt, dmt + (size_t)L * T * T, 1.0,
+                               jitter, A, ld));
+    else
+        RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, dth, 1.0, jitter, 1, 1, A, ld));
     if (dnv)   // k + diag(measured_noise) / k + diag(exp(log_var)): mngp.py:96, hskgp.py:147
         RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ld, N, dnv));
     CUDA_TRY(ctx, cudaMemcpyAsync(w, dy, (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
@@ -1331,9 +1442,17 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
             // K^{-1} = L^{-T} L^{-1} accumulated onto zeros: beta = 1 is what the int8 tensor-core path takes (7 planes here)
             CUDA_TRY(ctx, cudaMemsetAsync(Kinv, 0, (size_t)N * ld * 8, st));
             RET_IF(gemm_nt(ctx, st, N, N, N, 1.0, Bt, ld, Bt, ld, 1.0, Kinv, ld, true));
-            RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv, ld,
-                          partial));
-            RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8));
+            if (mt) {
+                RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles, (unsigned)L), MLL_THREADS, 0, mll_lcm_grad_kernel, dX, dtask, N,
+                              d, kind, T, L, mt->group, dth, (const double*)dmt, (const double*)(dmt + (size_t)L * T * T), jitter,
+                              (const double*)alpha, (const double*)Kinv, ld, partial));
+                RET_IF(launch(ctx, st, (unsigned)(L * nout), MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial,
+                              tiles * tiles, nout, gmt));
+            } else {
+                RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv,
+                              ld, partial));
+                RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8));
+            }
             if (grad_noise_vec) {
                 RET_IF(launch(ctx, st, grid_for(N), 256, 0, mll_diag_grad_kernel, alpha, Kinv, ld, N, w));   // w is free again
                 CUDA_TRY(ctx, cudaMemcpyAsync(grad_noise_vec, w, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
@@ -1344,14 +1463,27 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     CUDA_TRY(ctx, cudaMemcpyAsync(hsc, sc, sizeof hsc, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, st));
     if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, alpha, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
+    std::vector<double> colsum(mt ? (size_t)L * nout : 0);
+    if (grad && mt) CUDA_TRY(ctx, cudaMemcpyAsync(colsum.data(), gmt, colsum.size() * 8, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
+    if (grad && mt) {   // grad_theta [L, d+2] | grad_B [L, T, T] (symmetrised) | grad_noise [T]  (mtgp.cuh)
+        const int nth1 = d + 2;
+        for (int q = 0; q < L; ++q) {
+            const double* c = colsum.data() + (size_t)q * nout;
+            for (int k = 0; k < nth1; ++k) grad[q * nth1 + k] = c[k];
+            for (int a = 0; a < T; ++a)
+                for (int b = 0; b < T; ++b)
+                    grad[L * nth1 + (q * T + a) * T + b] = 0.5 * (c[nth1 + a * T + b] + c[nth1 + b * T + a]);
+        }
+        for (int t = 0; t < T; ++t) grad[L * nth1 + L * T * T + t] = colsum[nth1 + T * T + t];
+    }
     *value = -0.5 * hsc[1] - hsc[0] - 0.5 * (double)N * 1.8378770664093453;  // log(2 pi)
-    if (grad)
+    if (grad && !mt)
         for (int k = 0; k < nth; ++k) grad[k] = hsc[8 + k];
     if (*info != 0) {
         *value = NAN;
         if (grad)
-            for (int k = 0; k < nth; ++k) grad[k] = NAN;
+            for (int k = 0; k < ngrad; ++k) grad[k] = NAN;
         if (grad_noise_vec)
             for (int64_t i = 0; i < N; ++i) grad_noise_vec[i] = NAN;
     }
@@ -1368,6 +1500,28 @@ extern "C" int b2gp_mll_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, c
                           const double* noise_vec, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
                           double* grad_noise_vec, int* info) {
     return mll_impl(ctx, kind, X, N, yres, d, theta, noise_vec, jitter, flags, value, grad, alpha_out, grad_noise_vec, info);
+}
+
+// MultiTaskGP / CoregGP.model's likelihood (mtgp.py:147-167, corgp.py:66-98) with the LCM kernel and its gradient
+extern "C" int b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, const int* task, int64_t N, const double* yres, int d,
+                                  int group, int T, int L, const double* theta, const double* B, const double* noise, double jitter,
+                                  unsigned flags, double* value, double* grad_theta, double* grad_B, double* grad_noise,
+                                  double* alpha_out, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    ARG_CHECK(ctx, B && noise && N >= 1);
+    ARG_CHECK(ctx, (grad_theta != nullptr) == (grad_B != nullptr) && (grad_B != nullptr) == (grad_noise != nullptr));
+    RET_IF(mt_check(ctx, "b2gp_mll_multitask", kind, flags, d, group, T, L, task, N, nullptr, 0));
+    const MtDesc mt{task, nullptr, group, T, L, B, noise};
+    std::vector<double> g;
+    if (grad_theta) g.resize((size_t)L * (d + 2) + (size_t)L * T * T + T);
+    RET_IF(mll_impl(ctx, kind, X, N, yres, d, theta, nullptr, jitter, flags, value, grad_theta ? g.data() : nullptr, alpha_out, nullptr,
+                    info, &mt));
+    if (grad_theta) {
+        memcpy(grad_theta, g.data(), (size_t)L * (d + 2) * 8);
+        memcpy(grad_B, g.data() + (size_t)L * (d + 2), (size_t)L * T * T * 8);
+        memcpy(grad_noise, g.data() + (size_t)L * (d + 2) + (size_t)L * T * T, (size_t)T * 8);
+    }
+    return B2GP_OK;
 }
 
 // value and gradient of the VFE bound of the sparse GP (see sparse_elbo.cuh): d/dlog(lengthscale[d], k_scale, noise, period)

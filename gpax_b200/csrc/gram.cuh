@@ -72,6 +72,12 @@ __device__ __forceinline__ double nngp_pair(bool relu, double xz, double xx, dou
     return k12;
 }
 
+// sin(pi (x - z) / period) / ell: one feature of the periodic kernel's sum (kernels.py:111-113), the expression gram_kernel
+// writes inline (routing gram_kernel through this helper changes its register allocation and SASS, which stay as they are)
+__device__ __forceinline__ double periodic_arg(double x, double z, double period, double ell) {
+    return sin(3.141592653589793 * (x - z) / period) / ell;
+}
+
 __global__ void __launch_bounds__(GRAM_THREADS) gram_kernel(const GramArgs p) {
     extern __shared__ __align__(16) double sm[];
     // layout: Xs[GRAM_BM][d] | x2[GRAM_BM] | Zt[d][GRAM_BN] | z2[GRAM_BN] | ell[d]

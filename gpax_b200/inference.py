@@ -212,11 +212,18 @@ class ProgramLogJoint:
                                              want_alpha=self.has_mean_params)
         return val, g, alpha, info
 
+    def _valid(self, th):
+        return np.all(np.isfinite(th)) and np.all(th[:self.d + 2] > 0)
+
+    def _dval_dth(self, th, g):
+        """d value / d theta from the likelihood's gradient g, which is d/dlog(theta); unused entries carry g = 0"""
+        return g / th
+
     def __call__(self, u, jacobian):
         u = np.asarray(u, dtype=np.float64)
         th, mean, sites = self._run(u)
         self.n_evals += 1
-        if not (np.all(np.isfinite(th)) and np.all(th[:self.d + 2] > 0)):
+        if not self._valid(th):
             return -np.inf, np.zeros(self.dim)
         yres = self.y0 if mean is None else self.y0 - mean
         val, g, alpha, info = self._lik(th, yres)
@@ -226,7 +233,7 @@ class ProgramLogJoint:
         lp, grad = self._log_prior(u, sites, jacobian, want_grad=not self.hierarchical)
         # chain rule through the host programs by central differences
         h = self.FD_STEP
-        dval_dth = g / th                                   # g is d/dlog(theta); unused entries of theta carry g = 0
+        dval_dth = self._dval_dth(th, g)
         if self.has_mean_params and alpha is None:
             raise NotImplementedError("this likelihood does not return d value / d mean: no probabilistic mean function")
         for k in range(self.dim):
@@ -252,6 +259,113 @@ class ProgramLogJoint:
             for s in self.sites:
                 out[s.name][r] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
                 o += s.size
+        return out
+
+
+def mtgp_model_program(m, d, T, R, L):
+    """the host side of MultiTaskGP.model (gpax/models/mtgp.py:92-142, 147-207): every statement except the likelihood,
+    sites in the reference's order.  Returns (kernel-parameter dict, noise, mean-function parameter dict or None)."""
+    if m.data_kernel_prior is not None:
+        kp = dict(m.data_kernel_prior())
+    else:                                                              # mtgp.py:187-207
+        squeeze = (lambda x: np.squeeze(x)) if L > 1 else (lambda x: x)
+        with P.plate("latent_plate_data", L, dim=-2):
+            with P.plate("ard", d, dim=-1):
+                length = P.sample("k_length", m.lengthscale_prior_dist or P.LogNormal(0.0, 1.0))
+            if m.output_scale:
+                scale = P.sample("k_scale", P.LogNormal(0.0, 1.0))
+            else:
+                scale = P.deterministic("k_scale", np.ones(L))
+            period = P.sample("period", P.LogNormal(0.0, 1.0)) if m.data_kernel_name == "Periodic" else None
+        kp = {"k_length": squeeze(length), "k_scale": squeeze(scale), "period": None if period is None else squeeze(period)}
+    with P.plate("latent_plate_task", L):                              # mtgp.py:164-185
+        kp["W"] = P.sample("W", m.W_prior_dist or P.Normal(0.0, 10.0).expand((L, T, R)))
+        kp["v"] = P.sample("v", m.v_prior_dist or P.LogNormal(0.0, 1.0).expand((L, T)))
+    if m.noise_prior is not None:
+        noise = m.noise_prior()
+    else:                                                              # mtgp.py:147-157
+        noise = P.sample("noise", m.noise_prior_dist or P.LogNormal(0.0, 1.0).expand((T,)))
+    mp = m.mean_fn_prior() if (m.mean_fn is not None and m.mean_fn_prior is not None) else None
+    return kp, noise, mp
+
+
+def corgp_model_program(m, d, T, R):
+    """the host side of CoregGP.model (gpax/models/corgp.py:57-113 with gp.py:229-247 for the data kernel)"""
+    if m.data_kernel_prior is not None:
+        kp = dict(m.data_kernel_prior())
+    else:
+        with P.plate("ard", d):
+            length = P.sample("k_length", m.lengthscale_prior_dist or P.LogNormal(0.0, 1.0))
+        kp = {"k_length": length, "k_scale": P.deterministic("k_scale", np.array(1.0)),
+              "period": P.sample("period", P.LogNormal(0.0, 1.0)) if m.data_kernel_name == "Periodic" else None}
+    if m.task_kernel_prior is not None:
+        kp.update(m.task_kernel_prior())
+    else:                                                              # corgp.py:105-113
+        kp["W"] = P.sample("W", P.Normal(0.0, 10.0).expand((T, R)))
+        kp["v"] = P.sample("v", P.LogNormal(0.0, 1.0).expand((T,)))
+    if m.noise_prior is not None:
+        noise = m.noise_prior()
+    else:                                                              # corgp.py:82-88
+        noise = P.sample("noise", P.LogNormal(0.0, 1.0).expand((T,)))
+    mp = m.mean_fn_prior() if (m.mean_fn is not None and m.mean_fn_prior is not None) else None
+    return kp, noise, mp
+
+
+class MTLogJoint(ProgramLogJoint):
+    """ProgramLogJoint of MultiTaskGP / CoregGP: the model program yields the flat parameter vector
+    p = (theta [L, d+2], B [L, T, T], noise [T]) of the LCM covariance, the GPU (b2gp_mll_multitask) returns the value,
+    d value / d(log theta, B, log noise) and alpha; d p / du and d mean / du are central differences of the program, so
+    custom data_kernel_prior / task_kernel_prior / noise_prior / mean_fn_prior and every *_prior_dist work unchanged."""
+
+    def __init__(self, model, jitter=1e-6):
+        self.T, self.R, self.L = model._num_tasks(), model._rank(), model._num_latents()
+        super().__init__(model, jitter)
+        self.rows = model._rows(self.X)
+        self.nth = self.L * (model.kernel_dim + 2)
+
+    def _model_program(self):
+        return self.m._model_program(self.T, self.R, self.L)
+
+    def _run(self, u):
+        vals, o = {}, 0
+        for s in self.sites:
+            vals[s.name] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
+            o += s.size
+        (kp, noise, mp), sites, _ = P.run_program(self._model_program, vals)
+        theta, B, nz = self.m._pack(dict(kp, noise=noise), batched=False)
+        p = np.concatenate([theta.ravel(), B.ravel(), nz.ravel()])
+        mean = None
+        if self.has_mean_params:
+            mean = np.asarray(self.m.mean_fn(self.X, mp), dtype=np.float64).squeeze()
+        elif self.fixed_mean is not None:
+            mean = self.fixed_mean
+        return p, mean, sites
+
+    def _split(self, p):
+        nb = self.L * self.T * self.T
+        return p[:self.nth], p[self.nth:self.nth + nb], p[self.nth + nb:]
+
+    def _valid(self, p):
+        th, _, nz = self._split(p)
+        return np.all(np.isfinite(p)) and np.all(th > 0) and np.all(nz > 0)
+
+    def _dval_dth(self, p, g):
+        th, _, nz = self._split(p)
+        gth, gB, gn = self._split(g)
+        return np.concatenate([gth / th, gB, gn / nz])
+
+    def _lik(self, p, yres):
+        th, B, nz = self._split(p)
+        Xd, task, group = self.rows
+        val, gt, gB, gn, alpha, info = self.m.ctx.mll_multitask(
+            self.m._fused, Xd, task, yres, th.reshape(self.L, -1), B.reshape(self.L, self.T, self.T), nz, group, self.jitter,
+            want_grad=True, want_alpha=self.has_mean_params)
+        return val, np.concatenate([gt.ravel(), gB.ravel(), gn]), alpha, info
+
+    def to_dict(self, U):
+        out = super().to_dict(U)
+        if "k_scale" not in out and self.m.data_kernel_prior is None:    # numpyro.deterministic sites are in the samples
+            out["k_scale"] = np.ones((np.atleast_2d(U).shape[0],) + self.m._scale_shape())
         return out
 
 

@@ -250,6 +250,7 @@ class _Run:
         self.rng = rng
         self.sites = OrderedDict()
         self.plates = []
+        self.plate_dims = []
         self.deterministic = OrderedDict()
 
 
@@ -271,7 +272,7 @@ def sample(name, fn, obs=None, rng_key=None, sample_shape=()):
     run = _current()
     if name in run.sites:
         raise ValueError(f"site '{name}' is sampled twice")
-    shape = tuple(sample_shape) + tuple(p for p in run.plates if not fn.shape) + tuple(fn.shape)
+    shape = tuple(sample_shape) + (_plate_shape(run) if not fn.shape else ()) + tuple(fn.shape)
     if name in run.values:
         v = np.asarray(run.values[name], dtype=np.float64)
         if v.shape != shape:
@@ -291,18 +292,38 @@ def deterministic(name, value):
     return value
 
 
-class plate:
-    """numpyro.plate(name, size): sample sites inside gain a leading batch dimension (gp.py:237 uses it for ARD)"""
+def _plate_shape(run):
+    """batch shape of a scalar site inside the open plates: one leading dimension per plate, outermost first; when a
+    plate names its `dim` (numpyro.plate(..., dim=-2)), NumPyro's layout -- the named dims at their place counted from the
+    right, the others at the rightmost free places, size 1 elsewhere (mtgp.py:198-203 gives `period` the shape (L, 1))"""
+    if all(dm is None for dm in run.plate_dims):
+        return tuple(run.plates)
+    rank = max([len(run.plates)] + [-dm for dm in run.plate_dims if dm is not None])
+    shape = [1] * rank
+    for size, dm in zip(run.plates, run.plate_dims):
+        if dm is not None:
+            shape[rank + dm] = size
+    free = [i for i in range(rank - 1, -1, -1) if i not in {rank + dm for dm in run.plate_dims if dm is not None}]
+    for size, dm in zip(run.plates, run.plate_dims):
+        if dm is None:
+            shape[free.pop(0)] = size
+    return tuple(shape)
 
-    def __init__(self, name, size, **_):
-        self.name, self.size = name, int(size)
+
+class plate:
+    """numpyro.plate(name, size, dim=None): sample sites inside gain a batch dimension (gp.py:237 uses it for ARD)"""
+
+    def __init__(self, name, size, dim=None, **_):
+        self.name, self.size, self.dim = name, int(size), dim
 
     def __enter__(self):
         _current().plates.append(self.size)
+        _current().plate_dims.append(self.dim)
         return np.arange(self.size)
 
     def __exit__(self, *exc):
         _current().plates.pop()
+        _current().plate_dims.pop()
         return False
 
 

@@ -211,6 +211,27 @@ int  b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t N, 
                          unsigned flags, double* mean, double* var, double* dmean, double* dvar,
                          int* info, b2gp_timing* timing);
 
+/* The posterior of MultiTaskGP / CoregGP -- gp.py:253-293 (get_mvn_posterior / _predict) with the linear model of
+ * coregionalisation of gpax/kernels/mtkernels.py:197-233 in place of the single-task kernel (gpax/models/mtgp.py,
+ * corgp.py).  For latent q = 0..L-1, with B_q = W_q W_q^T + diag(v_q) (mtkernels.py:60-63):
+ *     K[i,j] = sum_q (k_q(x_i, x_j) + jitter [same point]) B_q[t_i, t_j]  +  [i == j] L (noise[t_i] + jitter)
+ * -- the noise and jitter are added once per latent, as the reference's vmap over the latents does (:228-231); k_pX
+ * carries no diagonal term (gp.py:268); noiseless scales only the noise of k_pp (gp.py:260-267).
+ *   Xtr[N,d], task_tr[N]    training inputs and their task ids (int32 in [0, T), checked before any launch)
+ *   Xnew[P,d], task_new[P]  test inputs and their task ids.  N and P count rows: the Kronecker form of
+ *                           MultivariateKernel (mtkernels.py:163-192) repeats every input T times, task index cycling
+ *                           fastest, with group = T (`group` consecutive rows are one data point); group = 1 otherwise
+ *   theta[S,L,d+2]          per draw and latent: lengthscale[d], k_scale, period (read for Periodic only)
+ *   B[S,L,T,T], noise[S,T]  task covariances and per-task noise variances
+ * Other arguments and outputs as b2gp_posterior.  Limits: T <= 8, L <= 4, d <= 16.  Kinds RBF, Matern-5/2, Periodic.
+ * Host fp64 arrays only: B2GP_FLAG_DEVICE_PTRS and B2GP_FLAG_F32 give B2GP_ERR_UNSUPPORTED.  The call does not use or
+ * fill the factor cache of b2gp_posterior; under "ozaki" = -1 it takes 7 digit planes.                                */
+int  b2gp_posterior_multitask(b2gp_ctx* ctx, int kind, const double* Xtr, const int* task_tr, int64_t N, const double* yres,
+                              int64_t yres_stride, const double* Xnew, const int* task_new, int64_t P, int d, int group, int T,
+                              int L, int64_t S, const double* theta, const double* B, const double* noise, int noiseless,
+                              double jitter, unsigned flags, double* mean, double* var, double* cov, const double* eps,
+                              int64_t n_samp, double* y_sampled, int* info, b2gp_timing* timing);
+
 /* Nystrom / VFE sparse posterior for one theta -- replaces viSparseGP.get_mvn_posterior
  * (gpax/models/sparse_gp.py:173-223).  Xu[M,d] inducing points; theta[d+3] as above;
  * outputs mean[P] and var[P] (B2GP_OUT_VAR) and/or cov[P,P] (B2GP_OUT_COV).                        */
@@ -237,6 +258,20 @@ int  b2gp_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double*
 int  b2gp_mll_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d,
                 const double* theta, const double* noise_vec, double jitter, unsigned flags,
                 double* value, double* grad, double* alpha_out, double* grad_noise_vec, int* info);
+
+/* The likelihood of MultiTaskGP.model / CoregGP.model (gpax/models/mtgp.py:147-167, corgp.py:66-98): log N(yres; 0, K)
+ * with K the LCM covariance of b2gp_posterior_multitask (X[N,d], task[N], group, T, L, theta[L,d+2], B[L,T,T], noise[T]
+ * as there, one draw), and its gradient (HOST outputs, all three or none):
+ *   grad_theta[L,d+2]  d value / d log(lengthscale_q[k], k_scale_q, period_q)
+ *   grad_B[L,T,T]      d value / d B_q[a,b] with the entries of B_q taken as independent (symmetric); the chain rule to
+ *                      W_q and v_q is (grad_B_q + grad_B_q^T) W_q and diag(grad_B_q)
+ *   grad_noise[T]      d value / d log noise[t]
+ * and alpha_out[N] = K^{-1} yres.  The reduction runs in a fixed order: identical calls give identical bits.  Limits,
+ * kinds and refused flags as b2gp_posterior_multitask; NaN value and gradient where info != 0.                         */
+int  b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, const int* task, int64_t N, const double* yres, int d,
+                        int group, int T, int L, const double* theta, const double* B, const double* noise, double jitter,
+                        unsigned flags, double* value, double* grad_theta, double* grad_B, double* grad_noise,
+                        double* alpha_out, int* info);
 
 /* Fit side of the sparse GP: the VFE bound of viSparseGP.model (gpax/models/sparse_gp.py:62-114)
  *   log LowRankMVN(yres; 0, W^T W + noise I) - 1/2 clip(sum_n (Kff_nn - Qff_nn) / noise, 0),  W = Luu^{-1} K(Xu, X)
