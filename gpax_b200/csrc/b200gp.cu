@@ -1645,9 +1645,10 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     grad_theta[d] += (T > 0.0) ? -0.5 * n * kd / noise : 0.0;
     const double trSinv = (n - m + hs2[4]) / noise;
     grad_theta[d + 1] = noise * (-0.5 * trSinv + 0.5 * hs2[5] + ((T > 0.0) ? 0.5 * T / (noise * noise) : 0.0));
-    if (*info != 0) {
+    if (*info != 0) {   // grad_Xu too: it was reduced from the failed factor and would otherwise come back finite
         *value = NAN;
         for (int k = 0; k < nth; ++k) grad_theta[k] = NAN;
+        for (int64_t i = 0; i < M * d; ++i) grad_Xu[i] = NAN;
     }
     return B2GP_OK;
 }

@@ -277,7 +277,9 @@ int  b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, const int* tas
  *   log LowRankMVN(yres; 0, W^T W + noise I) - 1/2 clip(sum_n (Kff_nn - Qff_nn) / noise, 0),  W = Luu^{-1} K(Xu, X)
  * and its gradient w.r.t. (log lengthscale[d], log k_scale, log noise, log period) in grad_theta[d+3] and w.r.t. the
  * inducing inputs in grad_Xu[M,d] (the reference differentiates the same expression with JAX; Xu is a numpyro.param,
- * sparse_gp.py:69-70).  theta is a HOST pointer; value / grads are HOST outputs; Xu, X, yres follow `flags`. d <= 16.  */
+ * sparse_gp.py:69-70).  theta is a HOST pointer; value / grads are HOST outputs; Xu, X, yres follow `flags`. d <= 16.
+ * info = the first bad pivot of Kuu + jitter I, or minus that of I + W W^T / noise; NaN value, grad_theta and grad_Xu
+ * where info != 0.                                                                                                    */
 int  b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N,
                       const double* yres, int d, const double* theta, double jitter, unsigned flags,
                       double* value, double* grad_theta, double* grad_Xu, int* info);

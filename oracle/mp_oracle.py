@@ -12,6 +12,11 @@ import numpy as np
 mp.mp.dps = 60
 
 
+def _mpf(v):
+    """an input coordinate as an mpf: float inputs exactly, mpf entries (of an object array) as they are"""
+    return v if isinstance(v, mp.mpf) else mp.mpf(float(v))
+
+
 def _gram(kind, X, Z, ell, scale, period, diag):
     n, m, d = X.shape[0], Z.shape[0], X.shape[1]
     K = mp.matrix(n, m)
@@ -20,12 +25,12 @@ def _gram(kind, X, Z, ell, scale, period, diag):
             if kind == "Periodic":                                  # kernels.py:94-117
                 s = mp.mpf(0)
                 for k in range(d):
-                    s += (mp.sin(mp.pi * (mp.mpf(float(X[i, k])) - mp.mpf(float(Z[j, k]))) / period) / ell[k]) ** 2
+                    s += (mp.sin(mp.pi * (_mpf(X[i, k]) - _mpf(Z[j, k])) / period) / ell[k]) ** 2
                 v = scale * mp.exp(-2 * s)
             else:
                 r2 = mp.mpf(0)
                 for k in range(d):
-                    r2 += ((mp.mpf(float(X[i, k])) - mp.mpf(float(Z[j, k]))) / ell[k]) ** 2
+                    r2 += ((_mpf(X[i, k]) - _mpf(Z[j, k])) / ell[k]) ** 2
                 if kind == "RBF":                                   # kernels.py:44-65
                     v = scale * mp.exp(-r2 / 2)
                 else:                                               # Matern-5/2, kernels.py:68-91 (r from r2 + 1e-12)
