@@ -155,6 +155,11 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
         ctx->tall_min = (int)value;
         return B2GP_OK;
     }
+    if (strcmp(key, "tall_min_fp64") == 0) {
+        ARG_CHECK(ctx, value >= 256);
+        ctx->tall_min_fp64 = (int)value;
+        return B2GP_OK;
+    }
     if (strcmp(key, "oz_debug") == 0) {   // timing experiments only: != 0 skips the C read-modify-write
         ARG_CHECK(ctx, value >= 0 && value <= 2);
         ctx->oz_debug = (int)value;
@@ -180,6 +185,7 @@ extern "C" int b2gp_get_option(b2gp_ctx* ctx, const char* key, int64_t* value) {
     } tab[] = {{"streams", ctx->n_streams},       {"ozaki", ctx->ozaki},         {"trsm_strip", ctx->trsm_strip},
                {"oz_cluster", ctx->oz_cluster},   {"enqueue_threads", ctx->enqueue_threads}, {"big_grid", ctx->big_grid},
                {"oz_min_tiles", ctx->oz_min_tiles}, {"panel", ctx->panel},       {"tall_min", ctx->tall_min},
+               {"tall_min_fp64", ctx->tall_min_fp64},
                {"oz_debug", ctx->oz_debug},       {"tma", ctx->use_tma}};
     for (const auto& e : tab)
         if (strcmp(key, e.key) == 0) {
@@ -761,7 +767,8 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         const double* th = dtheta + s * nth;
         const double* dXtr_s = dXtr + s * xtr_stride;
         const double* dXnew_s = dXnew + s * xnew_stride;
-        const bool fused_solve = !reuse && use_tall(ctx, N);   // the P-side solve rides along with the factorisation
+        // the P-side solve rides along with the factorisation (int8 or fp64 route of the tall-panel scheme)
+        const bool fused_solve = !reuse && (use_tall(ctx, N) || use_tall_fp64(ctx, N));
         int* inf = dinfo + s;
         int* inf2 = dinfo + S + s;
         if (timing) {
@@ -794,7 +801,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
             // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
-            if (fused_solve) count_path(ctx, PATH_POTRF_TALL);
+            if (fused_solve) count_tall_entry(ctx, use_tall(ctx, N));
             if (fused_solve)
                 RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, R, Linv, inf, 0, keepU ? (double*)ctx->Ukeep.p : nullptr));
             else

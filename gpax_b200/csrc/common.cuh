@@ -107,7 +107,8 @@ enum PathCounter {
     PATH_POTRF_DIAG,    // potrf_diag_kernel launches (128-wide leaves)
     PATH_PANEL_SOLVE,   // panel_solve_all_rows calls
     PATH_TRSM_TALL,     // trsm_tall calls
-    PATH_POTRF_TALL,    // factorisations that took potrf_tall (top-level entries, not its recursion)
+    PATH_POTRF_TALL,    // factorisations that took potrf_tall on the int8 route (top-level entries, not its recursion)
+    PATH_POTRF_TALL_FP64,  // factorisations that took potrf_tall on the fp64 DMMA route (ozaki = 0), top-level entries
     PATH_COUNT
 };
 
@@ -124,7 +125,8 @@ struct b2gp_ctx {
     int trsm_strip = 256;  // widest factor solved by the one-launch strip kernel (0: recurse down to the 128 leaves)
     int oz_cluster = 2;  // 2: CTA pairs (a cluster of 2) share the A digit planes by TMA multicast; 1: independent CTAs
     int panel = 1024;      // diagonal-block width of the tall-panel factorisation (potrf_tall); 0: recursive potrf_rec / trsm_rec only
-    int tall_min = 2048;   // smallest N factored by potrf_tall
+    int tall_min = 2048;   // smallest N factored by potrf_tall on the int8 route
+    int tall_min_fp64 = 8192;  // smallest N factored by potrf_tall on the fp64 route (ozaki = 0); DESIGN.md 4.2
     int oz_debug = 0;  // see OzArgs::debug (0 in production)
     // 0: fp64 DMMA only; 6 / 7: large rank-k updates through the int8 wgmma path with that many base-256 digit planes
     // (46 / 54 bits per operand); -1: 6 or 7 per factorisation from a bound on cond(K), see oz_auto_planes().

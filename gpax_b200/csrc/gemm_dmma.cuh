@@ -163,7 +163,9 @@ __device__ __forceinline__ void load_slice(double* sm, const double* __restrict_
     }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, bool ALIGNED, int MINB>
+// KTRI: the in-place k-triangular panel solve of gemm_panel_solve -- one CTA per BM-row strip, column tiles from right to
+// left, tile j with k < BN (j + 1) (as gemm_tma_kernel<.., true>, which explains why that order is race-free).
+template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, bool ALIGNED, int MINB, bool KTRI = false>
 __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(const GemmArgs p) {
     constexpr int NT = WARPS_M * WARPS_N * 32;
     constexpr int WTM = BM / WARPS_M, WTN = BN / WARPS_N;
@@ -191,19 +193,26 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
             if (p.lower_only && tj > ti) return;
         }
     }
-    const int row0 = ti * BM, col0 = tj * BN;
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
     const int wm = warp / WARPS_N, wn = warp % WARPS_N;
     const int g = lane >> 2, t4 = lane & 3;
+    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
 
+    for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
+    if (KTRI) {
+        ti = (int)blockIdx.x;
+        tj = p.tiles_n - 1 - jj;
+        if (jj > 0) __syncthreads();   // every warp is done with the stages of the previous tile before the prologue refills them
+    }
+    const int row0 = ti * BM, col0 = tj * BN;
     double acc[MI][NI][2];
 #pragma unroll
     for (int i = 0; i < MI; ++i)
 #pragma unroll
         for (int j = 0; j < NI; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
 
-    const int KT = (p.k + GEMM_BK - 1) / GEMM_BK;
+    const int KT = KTRI ? min((p.k + GEMM_BK - 1) / GEMM_BK, ((tj + 1) * BN + GEMM_BK - 1) / GEMM_BK) : (p.k + GEMM_BK - 1) / GEMM_BK;
 
     // prologue
 #pragma unroll
@@ -238,7 +247,6 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
     cp_async_wait<0>();
 
     // epilogue: C = beta*C + alpha*acc.  Fragment (i,j): row g, columns 2*t4, 2*t4+1.
-    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
 #pragma unroll
     for (int i = 0; i < MI; ++i) {
         const int r = row0 + wm * WTM + i * 8 + g;
@@ -268,19 +276,20 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
             }
         }
     }
+    }
 }
 
-template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, int MINB>
+template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, int MINB, bool KTRI = false>
 static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     constexpr int smem_bytes = STAGES * (BM + BN) * GEMM_LDS * (int)sizeof(double);
     const bool aligned = ((a.lda & 1) == 0) && ((a.ldb & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.A) & 15) == 0) &&
                          ((reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
     a.tiles_m = (a.m + BM - 1) / BM;
     a.tiles_n = (a.n + BN - 1) / BN;
-    int64_t grid = a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
+    int64_t grid = KTRI ? (int64_t)a.tiles_m : a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
     if (grid <= 0) return B2GP_OK;
-    auto kern = aligned ? gemm_nt_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, true, MINB>
-                        : gemm_nt_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, false, MINB>;
+    auto kern = aligned ? gemm_nt_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, true, MINB, KTRI>
+                        : gemm_nt_kernel<BM, BN, WARPS_M, WARPS_N, STAGES, false, MINB, KTRI>;
     static PerDeviceOnce attr_set[2];
     if (attr_set[aligned ? 1 : 0].need(ctx->device)) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -289,7 +298,8 @@ static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     return launch(ctx, PATH_GEMM_NT, st, (unsigned)grid, WARPS_M * WARPS_N * 32, smem_bytes, kern, a);
 }
 
-static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);  // gemm_tma.cuh
+static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);        // gemm_tma.cuh
+static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);  // gemm_tma.cuh
 static int ozaki_dispatch(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
                           const double* B, int64_t ldb, double* C, int64_t ldc, bool lower_only, bool overwrite, bool transB,
                           bool ktri);  // ozaki.cuh
@@ -356,4 +366,41 @@ static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t
     if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2>(ctx, st, a);
     if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2>(ctx, st, a);
     return launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a);
+}
+
+// The fp64 panel solve of the tall-panel factorisation (potrf.cuh, panel_solve_all_rows):  rows (m x n) <- rows Li^T,
+// in place, with Li = L_bb^{-1} (n x n, lower, row-major, zero above the diagonal).  The k-triangular extent (column tile
+// j needs k < 128 (j + 1)) makes it cost m n^2 flops, the triangular solve's count.  C overwrites A's columns, so a CTA
+// owns a whole row strip and walks its column tiles from right to left (gemm_tma_kernel, KTRI) instead of solving into
+// scratch and copying back.  128-row strips on the persistent TMA kernel from 16 strips up: with draws in flight on other
+// streams the SMs a thin solve leaves idle run their work (DESIGN.md 4.3); below that gemm_nt's latency rule in row strips.
+static int gemm_panel_solve(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, double* rows, int64_t ldr, const double* Li,
+                            int64_t ldli) {
+    if (m <= 0 || n <= 0) return B2GP_OK;
+    GemmArgs a;
+    a.m = (int)m;
+    a.n = (int)n;
+    a.k = (int)n;
+    a.A = rows;
+    a.lda = ldr;
+    a.B = Li;
+    a.ldb = ldli;
+    a.C = rows;
+    a.ldc = ldr;
+    a.alpha = 1.0;
+    a.beta = 0.0;
+    a.lower_only = 0;
+    const int64_t tm128 = ceil_div(m, 128);
+    if (tm128 >= 16) {
+        if (ctx->use_tma) {
+            const int rc = gemm_tma_panel_dispatch(ctx, st, a);
+            if (rc != B2GP_ERR_UNSUPPORTED) return rc;
+        }
+        return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a);
+    }
+    const int64_t c128 = ceil_div(tm128, ctx->sm_count) * 4, c64 = ceil_div(ceil_div(m, 64), 2 * ctx->sm_count) * 2,
+                  c32 = ceil_div(ceil_div(m, 32), 2 * ctx->sm_count);
+    if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2, true>(ctx, st, a);
+    if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2, true>(ctx, st, a);
+    return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a);
 }

@@ -94,7 +94,12 @@ __device__ __forceinline__ void tile_of(int x, int lower_only, int tiles_n, int&
     }
 }
 
-template <int STAGES, int KSUB>
+// KTRI: the in-place panel solve  C = A <- A B^T  with B lower triangular (B = L_bb^{-1}, see gemm_panel_solve in
+// gemm_dmma.cuh).  A work unit is then a whole 128-row strip: its CTA walks the column tiles from right to left, and
+// column tile j stops at k = 128 (j + 1) (B is zero beyond its diagonal block).  Tile j reads columns < 128 (j + 1) and
+// writes columns 128 j .. 128 j + 127, so nothing a later tile of the strip reads has been overwritten, and no other CTA
+// touches the strip's rows.  Right to left is also heaviest first.
+template <int STAGES, int KSUB, bool KTRI = false>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GemmArgs p, int num_tiles) {
     constexpr int BK = 16 * KSUB;
@@ -120,11 +125,18 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         // ------------------------------------------------------------ producer
         if (lane == 0) {
             uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
+            for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
                 int ti, tj;
-                tile_of(tile, p.lower_only, p.tiles_n, ti, tj);
+                if (KTRI) {
+                    ti = tile;
+                    tj = p.tiles_n - 1 - jj;
+                } else {
+                    tile_of(tile, p.lower_only, p.tiles_n, ti, tj);
+                }
                 const int row0 = ti * TG_BM, col0 = tj * TG_BN;
-                for (int kt = 0; kt < KT; ++kt, ++it) {
+                const int KTt = KTRI ? min(KT, ((tj + 1) * TG_BN + BK - 1) / BK) : KT;
+                for (int kt = 0; kt < KTt; ++kt, ++it) {
                     const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
                     mbar_wait(bars + 8 * (STAGES + s), ph ^ 1u);
                     const uint32_t full = bars + 8 * s;
@@ -155,17 +167,24 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
 
     uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
+    for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
         int ti, tj;
-        tile_of(tile, p.lower_only, p.tiles_n, ti, tj);
+        if (KTRI) {
+            ti = tile;
+            tj = p.tiles_n - 1 - jj;
+        } else {
+            tile_of(tile, p.lower_only, p.tiles_n, ti, tj);
+        }
         const int row0 = ti * TG_BM, col0 = tj * TG_BN;
+        const int KTt = KTRI ? min(KT, ((tj + 1) * TG_BN + BK - 1) / BK) : KT;   // the producer's count
         double acc[MI][NI][2];
 #pragma unroll
         for (int i = 0; i < MI; ++i)
 #pragma unroll
             for (int j = 0; j < NI; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
 
-        for (int kt = 0; kt < KT; ++kt, ++it) {
+        for (int kt = 0; kt < KTt; ++kt, ++it) {
             const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
             mbar_wait(bars + 8 * s, ph);
 #pragma unroll
@@ -180,7 +199,7 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             if (lane == 0) mbar_arrive(bars + 8 * (STAGES + s));
         }
 
-        // epilogue (identical to gemm_nt_kernel)
+        // epilogue (identical to gemm_nt_kernel); the panel solve (KTRI) has alpha = 1, beta = 0 and no lower-only map
 #pragma unroll
         for (int i = 0; i < MI; ++i) {
             const int r = row0 + wm * 64 + i * 8 + g;
@@ -189,22 +208,22 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             for (int j = 0; j < NI; ++j) {
                 const int c = col0 + wn * 32 + j * 8 + t4 * 2;
                 if (c >= p.n) continue;
-                if (p.lower_only && c > r) continue;
+                if (!KTRI && p.lower_only && c > r) continue;
                 double* dst = p.C + (int64_t)r * p.ldc + c;
-                const bool two = (c + 1 < p.n) && !(p.lower_only && c + 1 > r);
+                const bool two = (c + 1 < p.n) && !(!KTRI && p.lower_only && c + 1 > r);
                 double v0 = p.alpha * acc[i][j][0], v1 = p.alpha * acc[i][j][1];
                 if (two && vec_ok) {
-                    if (p.beta != 0.0) {
+                    if (!KTRI && p.beta != 0.0) {
                         const double2 old = *reinterpret_cast<const double2*>(dst);
                         v0 += p.beta * old.x;
                         v1 += p.beta * old.y;
                     }
                     *reinterpret_cast<double2*>(dst) = make_double2(v0, v1);
                 } else {
-                    if (p.beta != 0.0) v0 += p.beta * dst[0];
+                    if (!KTRI && p.beta != 0.0) v0 += p.beta * dst[0];
                     dst[0] = v0;
                     if (two) {
-                        if (p.beta != 0.0) v1 += p.beta * dst[1];
+                        if (!KTRI && p.beta != 0.0) v1 += p.beta * dst[1];
                         dst[1] = v1;
                     }
                 }
@@ -214,7 +233,7 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 }
 
 // returns B2GP_ERR_UNSUPPORTED when the operands do not meet TMA's alignment rules (caller falls back)
-template <int STAGES, int KSUB>
+template <int STAGES, int KSUB, bool KTRI = false>
 static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     constexpr int smem_bytes = STAGES * 2 * KSUB * TG_SUB_BYTES + 2 * STAGES * 8 + 1024;
     const bool ok = ((a.lda & 1) == 0) && ((a.ldb & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.A) & 15) == 0) &&
@@ -224,11 +243,11 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     if (!make_tmap(&mapA, a.A, a.m, a.k, a.lda) || !make_tmap(&mapB, a.B, a.n, a.k, a.ldb)) return B2GP_ERR_UNSUPPORTED;
     a.tiles_m = (a.m + TG_BM - 1) / TG_BM;
     a.tiles_n = (a.n + TG_BN - 1) / TG_BN;
-    const int64_t tiles = a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
+    const int64_t tiles = KTRI ? (int64_t)a.tiles_m : a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
     if (tiles <= 0) return B2GP_OK;
     static PerDeviceOnce attr;
     if (attr.need(ctx->device)) {
-        CUDA_TRY(ctx, cudaFuncSetAttribute(gemm_tma_kernel<STAGES, KSUB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+        CUDA_TRY(ctx, cudaFuncSetAttribute(gemm_tma_kernel<STAGES, KSUB, KTRI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
         attr.done(ctx->device);
     }
     // Wave quantisation: with T tiles on S SMs the persistent kernel takes ceil(T/S) tile-times.  The T mod S tiles
@@ -241,7 +260,7 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     int64_t main_tiles = tiles;
     if (!inplace && tiles > S && tiles % S != 0) main_tiles = tiles - tiles % S;
     const int grid = (int)(main_tiles < S ? main_tiles : S);
-    RET_IF(launch(ctx, PATH_GEMM_TMA, st, grid, TG_THREADS, smem_bytes, gemm_tma_kernel<STAGES, KSUB>, mapA, mapB, a, (int)main_tiles));
+    RET_IF(launch(ctx, PATH_GEMM_TMA, st, grid, TG_THREADS, smem_bytes, gemm_tma_kernel<STAGES, KSUB, KTRI>, mapA, mapB, a, (int)main_tiles));
     if (main_tiles < tiles) {
         GemmArgs t = a;
         t.tile_base = (int)main_tiles;
@@ -261,3 +280,4 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
 }
 
 static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) { return launch_gemm_tma<3, 2>(ctx, st, a); }
+static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) { return launch_gemm_tma<3, 2, true>(ctx, st, a); }
