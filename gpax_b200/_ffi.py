@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libb200gp.so")
 
 KERNEL_RBF, KERNEL_MATERN52, KERNEL_PERIODIC = 0, 1, 2
 KERNEL_NNGP_ERF, KERNEL_NNGP_RELU = 3, 4
+ACT_RELU, ACT_TANH = 0, 1
 KIND = {"RBF": KERNEL_RBF, "Matern": KERNEL_MATERN52, "Periodic": KERNEL_PERIODIC}
 
 FLAG_DEVICE_PTRS = 1 << 0
@@ -85,6 +86,9 @@ SIGNATURES = {
     "b2gp_sparse_posterior": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
                                         _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _ip]),
+    "b2gp_mlp_forward": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_uint]),
+    "b2gp_dkl_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint,
+                               _dp, _vp, _vp, _vp, _ip]),
     "b2gp_sparse_elbo": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp,
                                    _vp, _ip]),
     "b2gp_dist_unique_id": (C.c_int, [_vp]),
@@ -501,6 +505,51 @@ class Context:
                                                 _ptr(yres), d, int(group), T, L, _ptr(theta), _ptr(B), _ptr(noise), float(jitter),
                                                 flags, C.byref(val), _ptr(gt), _ptr(gB), _ptr(gn), _ptr(alpha), C.byref(info)))
         return val.value, gt, gB, gn, alpha, info.value
+
+    def mlp_forward(self, X, widths, act, params):
+        """Z [S, N, d] = MLP(X) for S weight sets (b2gp_mlp_forward).  X [N, D]: a host array or a DeviceArray; widths [L]:
+        the layers' output widths; act ACT_RELU / ACT_TANH; params [S, P] or [P] in the flat layout (per layer W_l [in, out]
+        row-major, then b_l)."""
+        X, Xp, flags = self._arg(X)
+        N, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        p = _f64(params)
+        p = p.reshape(1, -1) if p.ndim == 1 else p
+        S = p.shape[0]
+        d = int(w[-1]) if w.size else D
+        Z = np.empty((S, N, d))
+        self._check(self.lib.b2gp_mlp_forward(self.h, Xp, N, D, int(w.size), _ptr(w), int(act), _ptr(p) if p.size else None, S,
+                                              p.shape[1], _ptr(Z), flags))
+        return Z
+
+    def dkl_mll(self, kind, X, yres, widths, act, params, theta, jitter=1e-6, want_params=True, want_z=False):
+        """log N(yres; 0, K(MLP(X))) and its gradients (b2gp_dkl_mll).  X [N, D] and yres [N]: both host arrays or both
+        DeviceArrays; params [P] flat layout; theta [d+3].  Returns (value, grad_theta [d+3] (d/dlog), grad_params [P] or
+        None, grad_z [N, d] or None, info)."""
+        X, Xp, flags = self._arg(X)
+        yres, yp, yflags = self._arg(yres)
+        if flags != yflags:
+            raise ValueError("X and yres must both be host arrays or both DeviceArrays")
+        N, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        d = int(w[-1]) if w.size else D
+        theta, p = _f64(theta).reshape(d + 3), _f64(params).reshape(-1)
+        val, info = C.c_double(0.0), C.c_int(0)
+        gt = np.zeros(d + 3)
+        gp = np.zeros(p.size) if want_params else None
+        gz = np.zeros((N, d)) if want_z else None
+        self._check(self.lib.b2gp_dkl_mll(self.h, KIND[kind] if isinstance(kind, str) else kind, Xp, N, D, yp, int(w.size), _ptr(w),
+                                          int(act), _ptr(p) if p.size else None, _ptr(theta), float(jitter), flags, C.byref(val),
+                                          _ptr(gt), _ptr(gp), _ptr(gz), C.byref(info)))
+        return val.value, gt, gp, gz, info.value
+
+    @staticmethod
+    def _arg(a):
+        """(array, pointer, flags) of a host array (made C-contiguous fp64) or a DeviceArray"""
+        if isinstance(a, DeviceArray):
+            return a, a.ptr, FLAG_DEVICE_PTRS
+        a = _f64(a)
+        return a, _ptr(a), 0
 
     def sparse_elbo(self, kind, Xu, X, yres, theta, jitter=1e-6):
         """VFE bound of the sparse GP, its gradient w.r.t. log(lengthscale[d], k_scale, noise, period) and w.r.t. Xu"""

@@ -144,7 +144,8 @@ def kg(model, X_new, sample, rng_key=None, n: int = 10, maximize: bool = True, n
         eps = posterior_eps(key, 1, n, P, np.float32, per_draw_keys=False)
     out = model._posterior_batched(X_new, sample, False, noiseless, ("mean", "cov"), eps=np.asarray(eps).reshape(1, n, P), **kwargs)
     mean, cov, ysim = out["mean"][0], out["cov"][0], out["y_sampled"][0]
-    noise = float(np.asarray(sample["noise"]))
+    kp = sample[1] if isinstance(sample, tuple) else sample          # viDKL's samples: (nn_params, kernel_params)
+    noise = float(np.asarray(kp["noise"]))
     jitter = float(kwargs.get("jitter", 1e-6))
     diag_sub = noise * (0.0 if noiseless else 1.0) + jitter
     return model.ctx.kg(mean, cov, ysim, diag_sub, noise + jitter, maximize)

@@ -18,6 +18,7 @@
 #include "sparse_elbo.cuh"
 #include "acq.cuh"
 #include "dist.cuh"
+#include "dkl.cuh"
 
 // ------------------------------------------------------------------------------------------ helpers
 static inline bool dev_ptrs(unsigned flags) { return (flags & B2GP_FLAG_DEVICE_PTRS) != 0; }
@@ -1371,9 +1372,10 @@ __global__ void mll_diag_grad_kernel(const double* __restrict__ alpha, const dou
 
 static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, const double* theta,
                     const double* noise_vec, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
-                    double* grad_noise_vec, int* info, const MtDesc* mt = nullptr) {
+                    double* grad_noise_vec, int* info, const MtDesc* mt = nullptr, double* grad_x_dev = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, !grad_noise_vec || grad);
+    ARG_CHECK(ctx, !grad_x_dev || (grad && !mt && !noise_vec));
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, X && yres && theta && value && info);
     ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= MLL_MAX_D);
@@ -1459,6 +1461,9 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv,
                               ld, partial));
                 RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8));
+                if (grad_x_dev)   // d value / d X [N, d] on the device (dkl.cuh)
+                    RET_IF(launch(ctx, st, (unsigned)ceil_div(N, DZ_ROWS), DZ_THREADS, 0, mll_dz_kernel, kind, dX, N, d, dth,
+                                  (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
             }
             if (grad_noise_vec) {
                 RET_IF(launch(ctx, st, grid_for(N), 256, 0, mll_diag_grad_kernel, alpha, Kinv, ld, N, w));   // w is free again
@@ -1528,6 +1533,164 @@ extern "C" int b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, cons
         memcpy(grad_B, g.data() + (size_t)L * (d + 2), (size_t)L * T * T * 8);
         memcpy(grad_noise, g.data() + (size_t)L * (d + 2) + (size_t)L * T * T, (size_t)T * 8);
     }
+    return B2GP_OK;
+}
+
+// ------------------------------------------------------------------------------------------ deep kernel learning (dkl.cuh)
+// Layer l maps in[l] -> out[l] features; W_l [in, out] at woff[l] and b_l [out] at boff[l] of the params layout.
+struct MlpShape {
+    int L = 0;
+    int64_t N = 0, d = 0, nparams = 0, max_in = 0, max_out = 0;
+    std::vector<int64_t> in, out, woff, boff;
+};
+
+static int mlp_shape(b2gp_ctx* ctx, int64_t N, int64_t D, int n_layers, const int64_t* widths, int act, MlpShape& s) {
+    ARG_CHECK(ctx, N >= 1 && D >= 1 && n_layers >= 0 && n_layers <= 64);
+    ARG_CHECK(ctx, n_layers == 0 || (widths && (act == B2GP_ACT_RELU || act == B2GP_ACT_TANH)));
+    s.L = n_layers;
+    s.N = N;
+    int64_t in = D, o = 0;
+    for (int l = 0; l < n_layers; ++l) {
+        ARG_CHECK(ctx, widths[l] >= 1 && widths[l] <= (1 << 16));
+        s.in.push_back(in);
+        s.out.push_back(widths[l]);
+        s.woff.push_back(o);
+        o += in * widths[l];
+        s.boff.push_back(o);
+        o += widths[l];
+        s.max_in = std::max(s.max_in, in);
+        s.max_out = std::max(s.max_out, widths[l]);
+        in = widths[l];
+    }
+    s.d = in;
+    s.nparams = o;
+    return B2GP_OK;
+}
+
+// H[0] = X, H[l+1] = act(H[l] W_l + b_l) (no activation on the last layer), each [N, out_l] contiguous, in ctx->mlp[2]
+// after the transposed weights W_l^T [out_l, in_l] that gemm_nt takes as its B operand.  dP: the weights on the device.
+static int mlp_forward_dev(b2gp_ctx* ctx, cudaStream_t st, const MlpShape& s, int act, const double* dX, const double* dP,
+                           std::vector<double*>& H) {
+    std::vector<int64_t> hoff(s.L), toff(s.L);
+    int64_t tot = 0;
+    for (int l = 0; l < s.L; ++l) {
+        toff[l] = tot;
+        tot += round_up(s.out[l] * s.in[l], 8);
+    }
+    for (int l = 0; l < s.L; ++l) {
+        hoff[l] = tot;
+        tot += round_up(s.N * s.out[l], 8);
+    }
+    H.assign(s.L + 1, nullptr);
+    H[0] = const_cast<double*>(dX);
+    if (s.L == 0) return B2GP_OK;
+    RET_IF(ensure(ctx, ctx->mlp[2], (size_t)tot * 8));
+    double* base = (double*)ctx->mlp[2].p;
+    for (int l = 0; l < s.L; ++l) {
+        const int64_t in = s.in[l], out = s.out[l];
+        double* Wt = base + toff[l];
+        H[l + 1] = base + hoff[l];
+        RET_IF(launch_transpose(ctx, st, dP + s.woff[l], out, in, out, Wt, in));
+        RET_IF(gemm_nt(ctx, st, s.N, out, in, 1.0, H[l], in, Wt, in, 0.0, H[l + 1], out, false));
+        RET_IF(launch(ctx, st, grid_for(s.N * out), 256, 0, mlp_bias_act_kernel, H[l + 1], out, s.N, (int)out,
+                      (const double*)(dP + s.boff[l]), l + 1 < s.L ? act : (int)DKL_ACT_NONE));
+    }
+    return B2GP_OK;
+}
+
+extern "C" int b2gp_mlp_forward(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, int n_layers, const int64_t* widths, int act,
+                                const double* params, int64_t S, int64_t params_stride, double* Z, unsigned flags) {
+    if (!ctx) return B2GP_ERR_ARG;
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, X && Z && S >= 1 && !f32_io(flags));
+    ARG_CHECK(ctx, n_layers == 0 || (params && params_stride >= s.nparams));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    CallTimer tm(ctx);
+    RET_IF(tm.begin(st));
+    const double *dX, *dP = nullptr;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev_ptrs(flags), &dX));
+    if (n_layers > 0) RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)((S - 1) * params_stride + s.nparams) * 8, false, &dP));
+    std::vector<double*> H;
+    for (int64_t m = 0; m < S; ++m) {
+        RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP ? dP + m * params_stride : nullptr, H));
+        CUDA_TRY(ctx, cudaMemcpyAsync(Z + m * N * s.d, H[s.L], (size_t)N * s.d * 8, cudaMemcpyDeviceToHost, st));
+    }
+    RET_IF(tm.end(st, nullptr));
+    return B2GP_OK;
+}
+
+// viDKL / DKL's likelihood on z = MLP(X): forward pass, then mll_impl on z (the b2gp_mll route, with d value / dz from
+// mll_dz_kernel), then the backward pass through the layers: per layer the bias gradient (column sum), the weight gradient
+// H_l^T G (gemm_nt on the transposes) and, below the first layer, G W_l^T masked by the activation's derivative.
+extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D, const double* yres, int n_layers,
+                            const int64_t* widths, int act, const double* params, const double* theta, double jitter, unsigned flags,
+                            double* value, double* grad_theta, double* grad_params, double* grad_z, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+    ARG_CHECK(ctx, X && yres && theta && value && grad_theta && info && !f32_io(flags));
+    ARG_CHECK(ctx, s.d <= MLL_MAX_D && (n_layers == 0 || params));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    // b2gp_last_timing reports the whole step: mll_impl's own timer covers only its part, so the call is bracketed by
+    // a second pair of events and its totals replace mll_impl's at the end
+    const auto t0 = std::chrono::steady_clock::now();
+    const int64_t launches0 = ctx->launches;
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
+    const bool dev = dev_ptrs(flags);
+    const double *dX, *dy, *dP = nullptr;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev, &dX));
+    RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)N * 8, dev, &dy));
+    if (n_layers > 0) RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)s.nparams * 8, false, &dP));
+    std::vector<double*> H;
+    RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP, H));
+    const bool back = grad_params && n_layers > 0;
+    // backward scratch: gz [N, d] | grad params | G ping-pong 2 x [N, max_out] | H_l^T [max_in, ldN] | G^T [max_out, ldN]
+    const int64_t ldN = round_up(N, 8);
+    const int64_t o_gp = round_up(N * s.d, 8), o_g0 = o_gp + round_up(s.nparams, 8), o_g1 = o_g0 + round_up(N * s.max_out, 8);
+    const int64_t o_ht = o_g1 + round_up(N * s.max_out, 8), o_gt = o_ht + s.max_in * ldN, tot = o_gt + s.max_out * ldN;
+    RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(back ? tot : o_gp) * 8));
+    double* gz = (double*)ctx->mlp[3].p;
+    const int64_t d = s.d;
+    RET_IF(mll_impl(ctx, kind, H[s.L], N, dy, (int)d, theta, nullptr, jitter, B2GP_FLAG_DEVICE_PTRS, value, grad_theta, nullptr, nullptr,
+                    info, nullptr, (grad_z || back) ? gz : nullptr));
+    const int64_t ngp = grad_params ? s.nparams : 0;
+    if (*info != 0) {
+        for (int64_t i = 0; grad_z && i < N * d; ++i) grad_z[i] = NAN;
+        for (int64_t i = 0; i < ngp; ++i) grad_params[i] = NAN;
+    }
+    if (grad_z && *info == 0) CUDA_TRY(ctx, cudaMemcpyAsync(grad_z, gz, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
+    if (back && *info == 0) {
+        double* base = (double*)ctx->mlp[3].p;
+        double *gp = base + o_gp, *G0 = base + o_g0, *G1 = base + o_g1, *Ht = base + o_ht, *Gt = base + o_gt;
+        double* G = gz;   // d value / d (pre-activation output of layer l), [N, out_l]
+        for (int l = s.L - 1; l >= 0; --l) {
+            const int64_t in = s.in[l], out = s.out[l];
+            RET_IF(launch(ctx, st, (unsigned)out, MLP_SUM_THREADS, 0, mlp_colsum_kernel, (const double*)G, out, N, gp + s.boff[l]));
+            RET_IF(launch_transpose(ctx, st, H[l], in, N, in, Ht, ldN));
+            RET_IF(launch_transpose(ctx, st, G, out, N, out, Gt, ldN));
+            RET_IF(gemm_nt(ctx, st, in, out, N, 1.0, Ht, ldN, Gt, ldN, 0.0, gp + s.woff[l], out, false));
+            if (l > 0) {
+                double* Gn = G == G0 ? G1 : G0;
+                RET_IF(gemm_nt(ctx, st, N, in, out, 1.0, G, out, dP + s.woff[l], out, 0.0, Gn, in, false));
+                RET_IF(launch(ctx, st, grid_for(N * in), 256, 0, mlp_act_grad_kernel, Gn, in, (const double*)H[l], in, N, (int)in, act));
+                G = Gn;
+            }
+        }
+        CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, gp, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
+    CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_b));
+    float ms = 0.f;
+    CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+    ctx->last.total_ms = ms;
+    ctx->last.launches = ctx->launches - launches0;
+    ctx->last.host_enqueue_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return B2GP_OK;
 }
 

@@ -144,6 +144,7 @@ struct b2gp_ctx {
     DevBuf eb[12];     // scratch of b2gp_sparse_elbo
     DevBuf f32_in[8];  // fp32 staging of the inputs / outputs of calls made with B2GP_FLAG_F32
     DevBuf f32_out[4];
+    DevBuf mlp[4];     // b2gp_mlp_forward / b2gp_dkl_mll: staged X and yres | weights | activations | backward scratch
     std::vector<void*> user_allocs;  // b2gp_dev_alloc
     // factor bookkeeping for b2gp_trsm_lower (host-pointer mode keeps the factor resident)
     DevBuf last_linv;

@@ -1,0 +1,198 @@
+// dkl.cuh -- deep kernel learning: the MLP feature extractor z = MLP(X) and the gradient of the exact-GP log marginal
+// likelihood w.r.t. the GP inputs z, which the MLP's backward pass turns into gradients w.r.t. its weights.
+//
+// The reference's models are viDKL (gpax/models/vidkl.py: 3-layer ReLU MLP, haiku) and DKL (gpax/models/dkl.py:167-177: tanh
+// MLP).  Dense layers H_{l+1} = act(H_l W_l + b_l), no activation after the last one.  The products run on gemm_nt (DMMA);
+// here are the pieces around them: the bias + activation epilogue, its backward mask, the bias gradient (a fixed-order
+// column sum) and a transpose for operands in the wrong orientation.
+//
+// mll_dz_kernel:  d/dz_i log N(y; 0, K(z)) = 1/2 sum_jl W_jl dK_jl/dz_i with W = alpha alpha^T - K^{-1}.  z_i enters row i
+// and column i of K, so the 1/2 cancels:
+//     g_i[k] = sum_{j != i} W_ij dk(z_i, z_j)/dz_i[k]
+// (k(z, z) is constant for the three stationary kernels, and the noise and jitter on the diagonal do not depend on z).
+// The derivatives are gram_dx_kernel's (grad.cuh): the reference's formulas as written.  K^{-1} exists as its lower
+// triangle only (mll_impl's SYRK), so W_ij is read at [max(i,j), min(i,j)].  One CTA owns DZ_ROWS rows and walks all
+// columns in tiles: for tiles left of the diagonal the rows of K^{-1} are read, right of it the columns (as rows j,
+// consecutive i) -- both coalesced; every entry of the lower triangle is read twice, N^2 doubles in all.  Each row's sum
+// is accumulated in a fixed order and reduced across the row's threads by a fixed shuffle tree: deterministic, no atomics.
+#pragma once
+#include "common.cuh"
+#include "grad.cuh"
+#include "mll.cuh"
+
+constexpr int DZ_ROWS = 32;      // rows i per CTA
+constexpr int DZ_COLS = 32;      // columns j per tile
+constexpr int DZ_THREADS = 256;  // 8 threads per row, 4 columns each per tile
+constexpr int DZ_TPR = DZ_THREADS / DZ_ROWS;
+
+__global__ void __launch_bounds__(DZ_THREADS)
+mll_dz_kernel(int kind, const double* __restrict__ Z, int64_t N, int d, const double* __restrict__ theta,
+              const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ G) {
+    __shared__ double Ws[DZ_ROWS][DZ_COLS + 1];
+    __shared__ double Zi[DZ_ROWS][MLL_MAX_D];
+    __shared__ double Zj[DZ_COLS][MLL_MAX_D];
+    __shared__ double ell[MLL_MAX_D];
+    const int tid = threadIdx.x;
+    const int64_t i0 = (int64_t)blockIdx.x * DZ_ROWS;
+    const bool periodic = (kind == B2GP_KERNEL_PERIODIC);
+    const double scale = theta[d], period = theta[d + 2];
+    if (tid < d) ell[tid] = theta[tid];
+    __syncthreads();
+    // staged as gram_dx_kernel stages them: divided by the lengthscale for RBF / Matern, raw for periodic
+    for (int idx = tid; idx < DZ_ROWS * d; idx += DZ_THREADS) {
+        const int r = idx / d, k = idx % d;
+        const int64_t gi = i0 + r;
+        const double v = gi < N ? Z[gi * d + k] : 0.0;
+        Zi[r][k] = periodic ? v : v / ell[k];
+    }
+    const int r = tid / DZ_TPR, q = tid % DZ_TPR;
+    const int64_t i = i0 + r;
+    double acc[MLL_MAX_D];
+#pragma unroll
+    for (int k = 0; k < MLL_MAX_D; ++k) acc[k] = 0.0;
+    for (int64_t j0 = 0; j0 < N; j0 += DZ_COLS) {
+        __syncthreads();
+        for (int idx = tid; idx < DZ_ROWS * DZ_COLS; idx += DZ_THREADS) {
+            // left of the diagonal block: consecutive threads along a row of K^{-1}; right of it: along a column
+            const bool left = j0 < i0;
+            const int rr = left ? idx / DZ_COLS : idx % DZ_ROWS, cc = left ? idx % DZ_COLS : idx / DZ_ROWS;
+            const int64_t gi = i0 + rr, gj = j0 + cc;
+            double w = 0.0;
+            if (gi < N && gj < N && gi != gj) {
+                const int64_t hi = gi > gj ? gi : gj, lo = gi > gj ? gj : gi;
+                w = alpha[gi] * alpha[gj] - Kinv[hi * ldk + lo];
+            }
+            Ws[rr][cc] = w;
+        }
+        for (int idx = tid; idx < DZ_COLS * d; idx += DZ_THREADS) {
+            const int c = idx / d, k = idx % d;
+            const int64_t gj = j0 + c;
+            const double v = gj < N ? Z[gj * d + k] : 0.0;
+            Zj[c][k] = periodic ? v : v / ell[k];
+        }
+        __syncthreads();
+        if (i >= N) continue;
+        for (int c = q; c < DZ_COLS; c += DZ_TPR) {
+            const double w = Ws[r][c];
+            if (w == 0.0) continue;     // outside the matrix, the diagonal, or an exact zero: contributes nothing
+            if (periodic) {
+                // gram_dx_kernel's derivative -2 pi sin(2 a_k) / (period l_k^2) k: one sincos per dimension, the terms kept
+                // in registers (fully unrolled) until the exponent is known
+                double s = 0.0, t[MLL_MAX_D];
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k) {
+                    t[k] = 0.0;
+                    if (k < d) {
+                        double sa, ca;
+                        sincos(3.141592653589793 * (Zi[r][k] - Zj[c][k]) / period, &sa, &ca);
+                        const double a = sa / ell[k];
+                        s += a * a;
+                        t[k] = -(4.0 * 3.141592653589793) * sa * ca / (period * ell[k] * ell[k]);
+                    }
+                }
+                const double wk = w * (scale * exp(-2.0 * s));
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k)
+                    if (k < d) acc[k] = fma(wk, t[k], acc[k]);
+                continue;
+            }
+            double x2 = 0.0, xz = 0.0, z2 = 0.0;
+#pragma unroll
+            for (int k = 0; k < MLL_MAX_D; ++k) {
+                if (k < d) {
+                    x2 = fma(Zi[r][k], Zi[r][k], x2);
+                    xz = fma(Zi[r][k], Zj[c][k], xz);
+                    z2 = fma(Zj[c][k], Zj[c][k], z2);
+                }
+            }
+            const double wg = w * stationary_dk_dr2(kind, (x2 - 2.0 * xz) + z2, scale);
+#pragma unroll
+            for (int k = 0; k < MLL_MAX_D; ++k)
+                if (k < d) acc[k] = fma(wg, 2.0 * (Zi[r][k] - Zj[c][k]) / ell[k], acc[k]);
+        }
+    }
+    // the DZ_TPR threads of a row are consecutive lanes: a fixed xor tree
+#pragma unroll
+    for (int k = 0; k < MLL_MAX_D; ++k) {
+        if (k < d) {
+            double v = acc[k];
+#pragma unroll
+            for (int o = DZ_TPR / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+            acc[k] = v;
+        }
+    }
+    if (q == 0 && i < N) {
+#pragma unroll
+        for (int k = 0; k < MLL_MAX_D; ++k)
+            if (k < d) G[i * d + k] = acc[k];
+    }
+}
+
+// ---- MLP pieces.  Row-major [rows, cols] with leading dimension ld.
+enum { DKL_ACT_NONE = -1 };   // the last layer; B2GP_ACT_RELU / B2GP_ACT_TANH otherwise
+
+// H = act(H + b)
+__global__ void mlp_bias_act_kernel(double* __restrict__ H, int64_t ld, int64_t rows, int cols, const double* __restrict__ b, int act) {
+    const int64_t total = rows * cols;
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = idx / cols;
+        const int j = (int)(idx % cols);
+        double v = H[i * ld + j] + b[j];
+        if (act == B2GP_ACT_RELU) v = v > 0.0 ? v : 0.0;
+        else if (act == B2GP_ACT_TANH) v = tanh(v);
+        H[i * ld + j] = v;
+    }
+}
+
+// G *= act'(pre-activation), from the stored activation H: ReLU (h > 0), tanh (1 - h^2)
+__global__ void mlp_act_grad_kernel(double* __restrict__ G, int64_t ldg, const double* __restrict__ H, int64_t ldh, int64_t rows,
+                                    int cols, int act) {
+    const int64_t total = rows * cols;
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = idx / cols;
+        const int j = (int)(idx % cols);
+        const double h = H[i * ldh + j];
+        const double m = act == B2GP_ACT_RELU ? (h > 0.0 ? 1.0 : 0.0) : 1.0 - h * h;
+        G[i * ldg + j] *= m;
+    }
+}
+
+// out[j] = sum_i G[i, j]: one CTA per column, strided partial sums then a fixed tree (deterministic)
+constexpr int MLP_SUM_THREADS = 256;
+__global__ void __launch_bounds__(MLP_SUM_THREADS)
+mlp_colsum_kernel(const double* __restrict__ G, int64_t ld, int64_t rows, double* __restrict__ out) {
+    __shared__ double red[MLP_SUM_THREADS];
+    const int j = blockIdx.x;
+    double s = 0.0;
+    for (int64_t i = threadIdx.x; i < rows; i += MLP_SUM_THREADS) s += G[i * ld + j];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = MLP_SUM_THREADS / 2; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) out[j] = red[0];
+}
+
+// B[c, r] = A[r, c]  (A [rows, cols] with lda, B [cols, rows] with ldb), 32 x 32 tiles through shared memory
+__global__ void mlp_transpose_kernel(const double* __restrict__ A, int64_t lda, int64_t rows, int64_t cols, double* __restrict__ B,
+                                     int64_t ldb) {
+    __shared__ double t[32][33];
+    const int64_t r0 = (int64_t)blockIdx.y * 32, c0 = (int64_t)blockIdx.x * 32;
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+        const int64_t r = r0 + y, c = c0 + threadIdx.x;
+        if (r < rows && c < cols) t[y][threadIdx.x] = A[r * lda + c];
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < 32; y += blockDim.y) {
+        const int64_t c = c0 + y, r = r0 + threadIdx.x;
+        if (r < rows && c < cols) B[c * ldb + r] = t[threadIdx.x][y];
+    }
+}
+
+static int launch_transpose(b2gp_ctx* ctx, cudaStream_t st, const double* A, int64_t lda, int64_t rows, int64_t cols, double* B,
+                            int64_t ldb) {
+    if (rows <= 0 || cols <= 0) return B2GP_OK;
+    dim3 grid((unsigned)ceil_div(cols, 32), (unsigned)ceil_div(rows, 32));
+    return launch(ctx, st, grid, dim3(32, 8), 0, mlp_transpose_kernel, A, lda, rows, cols, B, ldb);
+}

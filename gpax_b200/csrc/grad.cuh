@@ -19,6 +19,16 @@
 #include "common.cuh"
 #include "gram.cuh"
 
+// dk/dr2 of RBF / Matern at the unclipped r2 = (x2 - 2 xz) + z2 of lengthscale-scaled inputs (see above); also used by
+// mll_dz_kernel (dkl.cuh), so that the likelihood's input gradient differentiates the same formulas
+__device__ __forceinline__ double stationary_dk_dr2(int kind, double r2raw, double scale) {
+    if (r2raw < 0.0) return 0.0;                         // clipped (kernels.py:41): no gradient flows
+    if (kind == B2GP_KERNEL_RBF) return -0.5 * scale * exp(-0.5 * r2raw);
+    const double r = sqrt(r2raw + 1e-12);
+    const double s5r = 2.23606797749979 * r;
+    return -(5.0 / 6.0) * scale * exp(-s5r) * (1.0 + 2.23606797749979 * r2raw / r);
+}
+
 constexpr int GDX_BN = 128;     // training points (columns) per CTA
 constexpr int GDX_BP = 16;      // test points per CTA
 constexpr int GDX_THREADS = 256;
@@ -84,16 +94,7 @@ gram_dx_kernel(int kind, const double* __restrict__ Xnew, int64_t P, const doubl
             xz = fma(x[k], Zs[k * GDX_BN + c], xz);
         }
         const double r2raw = (x2 - 2.0 * xz) + z2;      // kernels.py:40
-        double g;                                        // dk/dr2
-        if (r2raw < 0.0) {
-            g = 0.0;                                     // clipped (kernels.py:41): no gradient flows
-        } else if (kind == B2GP_KERNEL_RBF) {
-            g = -0.5 * scale * exp(-0.5 * r2raw);
-        } else {
-            const double r = sqrt(r2raw + 1e-12);
-            const double s5r = 2.23606797749979 * r;
-            g = -(5.0 / 6.0) * scale * exp(-s5r) * (1.0 + 2.23606797749979 * r2raw / r);
-        }
+        const double g = stationary_dk_dr2(kind, r2raw, scale);
         for (int k = 0; k < d; ++k) out[k * ldd] = g * 2.0 * (x[k] - Zs[k * GDX_BN + c]) / ell[k];
     }
 }

@@ -382,6 +382,25 @@ class SVIState:
         self.losses, self.guide, self.loc, self.scale = losses, guide, loc, scale
 
 
+def adam(params, objective, num_steps, step_size, progress_bar):
+    """Adam(step_size, b1=0.5), the optimiser of every SVI fit here (vigp.py:108-120, sparse_gp.py:116-171,
+    vidkl.py:134): maximises `objective(params) -> (elbo, grad)` and returns (params, losses = -elbo per step)."""
+    m1, m2 = np.zeros_like(params), np.zeros_like(params)
+    b1, b2, eps = 0.5, 0.999, 1e-8
+    losses = []
+    for t in range(1, int(num_steps) + 1):
+        elbo, grad = objective(params)
+        losses.append(-elbo)
+        if not np.isfinite(elbo):
+            grad = np.zeros_like(params)
+        m1 = b1 * m1 + (1 - b1) * (-grad)
+        m2 = b2 * m2 + (1 - b2) * grad * grad
+        params = params - step_size * (m1 / (1 - b1 ** t)) / (np.sqrt(m2 / (1 - b2 ** t)) + eps)
+        if progress_bar and (t % max(1, num_steps // 10) == 0 or t == num_steps):
+            print(f"svi step {t}/{num_steps}  loss {losses[-1]:.4f}")
+    return params, losses
+
+
 def fit_vi_gp(model, rng_key, num_steps, step_size, progress_bar, **kwargs):
     """vigp.py:108-120: Adam(step_size, b1=0.5), AutoDelta (MAP in the constrained space, no Jacobian) or AutoNormal
     (mean-field normal over u, init scale 0.1, one reparameterised draw per step).  Returns (state, median dict)."""
@@ -391,26 +410,16 @@ def fit_vi_gp(model, rng_key, num_steps, step_size, progress_bar, **kwargs):
     loc = lj.init_u()
     rho = np.full(lj.dim, math.log(0.1))            # log sigma
     params = np.concatenate([loc, rho]) if normal else loc.copy()
-    m1, m2 = np.zeros_like(params), np.zeros_like(params)
-    b1, b2, eps = 0.5, 0.999, 1e-8
-    losses = []
-    for t in range(1, int(num_steps) + 1):
+
+    def objective(params):
         if normal:
             mu, r = params[:lj.dim], params[lj.dim:]
             e = rng.standard_normal(lj.dim)
             val, g = lj(mu + np.exp(r) * e, jacobian=True)
             elbo = val + r.sum() + 0.5 * lj.dim * (1 + math.log(2 * math.pi))
-            grad = np.concatenate([g, g * e * np.exp(r) + 1.0])
-        else:
-            elbo, grad = lj(params, jacobian=False)
-        losses.append(-elbo)
-        if not np.isfinite(elbo):
-            grad = np.zeros_like(params)
-        m1 = b1 * m1 + (1 - b1) * (-grad)
-        m2 = b2 * m2 + (1 - b2) * grad * grad
-        params = params - step_size * (m1 / (1 - b1 ** t)) / (np.sqrt(m2 / (1 - b2 ** t)) + eps)
-        if progress_bar and (t % max(1, num_steps // 10) == 0 or t == num_steps):
-            print(f"svi step {t}/{num_steps}  loss {losses[-1]:.4f}")
+            return elbo, np.concatenate([g, g * e * np.exp(r) + 1.0])
+        return lj(params, jacobian=False)
+    params, losses = adam(params, objective, num_steps, step_size, progress_bar)
     loc = params[:lj.dim]
     med = {k: (v[0] if v.ndim == 1 else v[0]) for k, v in lj.to_dict(loc).items()}   # guide median (vigp.py:125-127)
     return SVIState(np.array(losses), "normal" if normal else "delta", loc, np.exp(params[lj.dim:]) if normal else None), med
@@ -468,10 +477,8 @@ def fit_sparse_gp(model, rng_key, Xu0, num_steps, step_size, progress_bar, **kwa
     head = np.concatenate([loc, rho]) if normal else loc.copy()
     params = np.concatenate([head, lj.Xu.ravel()])
     nh = head.size
-    m1, m2 = np.zeros_like(params), np.zeros_like(params)
-    b1, b2, eps = 0.5, 0.999, 1e-8
-    losses = []
-    for t in range(1, int(num_steps) + 1):
+
+    def objective(params):
         lj.Xu = params[nh:].reshape(lj.Xu.shape)
         if normal:
             mu, r = params[:nu], params[nu:nh]
@@ -481,15 +488,8 @@ def fit_sparse_gp(model, rng_key, Xu0, num_steps, step_size, progress_bar, **kwa
             ghead = np.concatenate([g, g * e * np.exp(r) + 1.0])
         else:
             elbo, ghead = lj(params[:nu], jacobian=False)
-        grad = np.concatenate([ghead, lj.grad_Xu.ravel()])
-        losses.append(-elbo)
-        if not np.isfinite(elbo):
-            grad = np.zeros_like(params)
-        m1 = b1 * m1 + (1 - b1) * (-grad)
-        m2 = b2 * m2 + (1 - b2) * grad * grad
-        params = params - step_size * (m1 / (1 - b1 ** t)) / (np.sqrt(m2 / (1 - b2 ** t)) + eps)
-        if progress_bar and (t % max(1, num_steps // 10) == 0 or t == num_steps):
-            print(f"svi step {t}/{num_steps}  loss {losses[-1]:.4f}")
+        return elbo, np.concatenate([ghead, lj.grad_Xu.ravel()])
+    params, losses = adam(params, objective, num_steps, step_size, progress_bar)
     med = {k: v[0] for k, v in lj.to_dict(params[:nu]).items()}
     med["Xu"] = params[nh:].reshape(lj.Xu.shape)
     return SVIState(np.array(losses), "normal" if normal else "delta", params[:nu], np.exp(params[nu:nh]) if normal else None), med

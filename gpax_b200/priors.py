@@ -231,6 +231,21 @@ class HalfCauchy(Prior):
         return np.abs(self.scale * rng.standard_cauchy(shape))
 
 
+class Cauchy(Normal):
+    """real support, theta = u: the bias prior of DKL / viDKL (dkl.py:160-164, vidkl.py:96)"""
+
+    def log_prob(self, t):
+        z = (t - self.loc) / self.scale
+        return -math.log(math.pi * self.scale) - np.log1p(z * z)
+
+    def dlog_prob(self, t):
+        z = (t - self.loc) / self.scale
+        return -2.0 * z / (self.scale * (1.0 + z * z))
+
+    def sample(self, rng, shape=()):
+        return self.loc + self.scale * rng.standard_cauchy(shape)
+
+
 # ---------------------------------------------------------------------------------------------- prior programs
 distributions = sys.modules[__name__]      # `priors.distributions.LogNormal(...)`, as `numpyro.distributions.LogNormal(...)`
 _tls = threading.local()

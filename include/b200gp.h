@@ -284,6 +284,28 @@ int  b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, cons
                       const double* yres, int d, const double* theta, double jitter, unsigned flags,
                       double* value, double* grad_theta, double* grad_Xu, int* info);
 
+/* ---- deep kernel learning (gpax/models/vidkl.py, gpax/models/dkl.py) ---------------------------------------------
+ * The feature extractor is a dense MLP, H_{l+1} = act(H_l W_l + b_l) with no activation after the last layer.
+ * params, per layer l: W_l[in_l, out_l] row-major (haiku's and dkl.py's orientation), then b_l[out_l];
+ * widths[n_layers] are the output widths, the last one is z_dim = d <= 16; in_0 = D.                                  */
+enum { B2GP_ACT_RELU = 0, B2GP_ACT_TANH = 1 };
+
+/* Z[s] = MLP(X; params + s * params_stride) for S weight sets: Z [S, N, d] (HOST).  X follows `flags`; params and
+ * widths are HOST pointers.  n_layers = 0 copies X (D = d).                                                          */
+int  b2gp_mlp_forward(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, int n_layers, const int64_t* widths, int act,
+                      const double* params, int64_t S, int64_t params_stride, double* Z, unsigned flags);
+
+/* log N(yres; 0, K(z)) on the embedding z = MLP(X) (the likelihood of viDKL.model / DKL.model) with its gradient:
+ *   value, grad_theta[d+3]  as b2gp_mll on the same z (same kernels, same bits), d / dlog theta
+ *   grad_z[N, d]            d value / d z (optional); with n_layers = 0 this is d value / d X
+ *   grad_params             d value / d params in the params layout (optional)
+ * X and yres follow `flags` (a fit uploads X once); theta, params and every output are HOST pointers.  NaN outputs where
+ * info != 0.  The reductions run in a fixed order: identical calls give identical bits.                              */
+int  b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D, const double* yres,
+                  int n_layers, const int64_t* widths, int act, const double* params,
+                  const double* theta, double jitter, unsigned flags,
+                  double* value, double* grad_theta, double* grad_params, double* grad_z, int* info);
+
 /* Samples of S multivariate normals: y[s,i,:] = mean[s,:] + chol(cov[s]) eps[s,i,:], i < n -- replaces
  * numpyro.distributions.MultivariateNormal(mean, cov).sample (gpax/models/gp.py:292, gpax/acquisition/base_acq.py:221)
  * where the caller changed cov after the posterior call (gpax/models/hskgp.py:201-204 adds the predicted noise variance).
