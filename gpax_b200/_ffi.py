@@ -89,6 +89,8 @@ SIGNATURES = {
     "b2gp_mlp_forward": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_uint]),
     "b2gp_dkl_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint,
                                _dp, _vp, _vp, _vp, _ip]),
+    "b2gp_mtdkl_mll": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int,
+                                 _vp, _vp, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _vp, _ip]),
     "b2gp_sparse_elbo": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp,
                                    _vp, _ip]),
     "b2gp_dist_unique_id": (C.c_int, [_vp]),
@@ -114,6 +116,7 @@ SIGNATURES = {
     "b2gp_acq_samples": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, C.c_int, C.c_double, C.c_double, C.c_int, _vp, _vp,
                                    _vp, C.c_uint]),
     "b2gp_kg": (C.c_int, [_vp, _vp, _vp, C.c_int64, _vp, C.c_int64, C.c_double, C.c_double, C.c_int, _vp, C.c_uint]),
+    "b2gp_kg_v": (C.c_int, [_vp, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int, _vp, C.c_uint]),
     "b2gp_copy2d": (C.c_int, [_vp, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int64]),
 }
 
@@ -543,6 +546,33 @@ class Context:
                                           _ptr(gt), _ptr(gp), _ptr(gz), C.byref(info)))
         return val.value, gt, gp, gz, info.value
 
+    def mtdkl_mll(self, kind, X, task, yres, widths, act, params, theta, B, noise, group=1, jitter=1e-6, want_params=True,
+                  want_z=False):
+        """The multi-task likelihood on z = MLP(X) and its gradients (b2gp_mtdkl_mll).  X [N, D] (N points, no task column)
+        and yres [N * group]: both host arrays or both DeviceArrays; task [N * group]; params [P] flat layout; theta [L, d+2],
+        B [L, T, T], noise [T] as mll_multitask.  Returns (value, grad_theta [L, d+2] (d/dlog), grad_B [L, T, T],
+        grad_noise [T] (d/dlog), grad_params [P] or None, grad_z [N, d] or None, info)."""
+        X, Xp, flags = self._arg(X)
+        yres, yp, yflags = self._arg(yres)
+        if flags != yflags:
+            raise ValueError("X and yres must both be host arrays or both DeviceArrays")
+        N, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        d = int(w[-1]) if w.size else D
+        B = _f64(B)
+        L, T = B.shape[0], B.shape[1]
+        theta, noise, p = _f64(theta, (L, d + 2)), _f64(noise, (T,)), _f64(params).reshape(-1)
+        task = np.ascontiguousarray(task, dtype=np.int32)
+        val, info = C.c_double(0.0), C.c_int(0)
+        gt, gB, gn = np.zeros((L, d + 2)), np.zeros((L, T, T)), np.zeros(T)
+        gp = np.zeros(p.size) if want_params else None
+        gz = np.zeros((N, d)) if want_z else None
+        self._check(self.lib.b2gp_mtdkl_mll(self.h, KIND[kind] if isinstance(kind, str) else kind, Xp, _ptr(task), N, D, yp,
+                                            int(group), T, L, int(w.size), _ptr(w), int(act), _ptr(p) if p.size else None,
+                                            _ptr(theta), _ptr(B), _ptr(noise), float(jitter), flags, C.byref(val), _ptr(gt),
+                                            _ptr(gB), _ptr(gn), _ptr(gp), _ptr(gz), C.byref(info)))
+        return val.value, gt, gB, gn, gp, gz, info.value
+
     @staticmethod
     def _arg(a):
         """(array, pointer, flags) of a host array (made C-contiguous fp64) or a DeviceArray"""
@@ -618,12 +648,19 @@ def _acq_samples(self, kind, y, best_f=None, param=0.0, maximize=False):
 
 
 def _kg(self, mean, cov, ysim, diag_sub, noise_plus_jitter, maximize=True):
+    """diag_sub and noise_plus_jitter: scalars (b2gp_kg) or one value per candidate [P] (b2gp_kg_v)"""
     mean, cov, ysim = _f64(mean), _f64(cov), _f64(ysim)
     P = mean.shape[0]
     ysim = ysim.reshape(-1, P)
     out = np.empty(P)
-    self._check(self.lib.b2gp_kg(self.h, _ptr(mean), _ptr(cov), P, _ptr(ysim), ysim.shape[0], float(diag_sub),
-                                 float(noise_plus_jitter), int(bool(maximize)), _ptr(out), 0))
+    if np.ndim(diag_sub) == 0 and np.ndim(noise_plus_jitter) == 0:
+        self._check(self.lib.b2gp_kg(self.h, _ptr(mean), _ptr(cov), P, _ptr(ysim), ysim.shape[0], float(diag_sub),
+                                     float(noise_plus_jitter), int(bool(maximize)), _ptr(out), 0))
+        return out
+    ds = _f64(np.broadcast_to(np.asarray(diag_sub, dtype=np.float64), (P,)))
+    nj = _f64(np.broadcast_to(np.asarray(noise_plus_jitter, dtype=np.float64), (P,)))
+    self._check(self.lib.b2gp_kg_v(self.h, _ptr(mean), _ptr(cov), P, _ptr(ysim), ysim.shape[0], _ptr(ds), _ptr(nj),
+                                   int(bool(maximize)), _ptr(out), 0))
     return out
 
 

@@ -139,14 +139,18 @@ def kg(model, X_new, sample, rng_key=None, n: int = 10, maximize: bool = True, n
     the reference's key: normal(rng_key, (n, P))."""
     X_new = np.asarray(model._set_data(X_new), dtype=np.float64)
     P = X_new.shape[0]
+    jitter = float(kwargs.get("jitter", 1e-6))
+    # models with a noise per task give the rank-1 update's diagonal terms per candidate (viMTDKL._kg_terms)
+    terms = model._kg_terms(X_new, sample, noiseless, jitter) if hasattr(model, "_kg_terms") else None
     if eps is None:
         key = rng_key if rng_key is not None else prng.PRNGKey(0)
         eps = posterior_eps(key, 1, n, P, np.float32, per_draw_keys=False)
     out = model._posterior_batched(X_new, sample, False, noiseless, ("mean", "cov"), eps=np.asarray(eps).reshape(1, n, P), **kwargs)
     mean, cov, ysim = out["mean"][0], out["cov"][0], out["y_sampled"][0]
+    if terms is not None:
+        return model.ctx.kg(mean, cov, ysim, terms[0], terms[1], maximize)
     kp = sample[1] if isinstance(sample, tuple) else sample          # viDKL's samples: (nn_params, kernel_params)
     noise = float(np.asarray(kp["noise"]))
-    jitter = float(kwargs.get("jitter", 1e-6))
     diag_sub = noise * (0.0 if noiseless else 1.0) + jitter
     return model.ctx.kg(mean, cov, ysim, diag_sub, noise + jitter, maximize)
 

@@ -97,12 +97,19 @@ __global__ void sample_moments_kernel(const double* __restrict__ y, int64_t R, i
 //     mean_aug[p] = mean[p] + C0[p, c] (y_sim - mean[c]) / (C0[c, c] + noise + jitter),
 // C0 = k(X_new, X_new) - k_pX K^{-1} k_Xp the posterior covariance of the latent function (the `cov` output with its
 // diagonal term noise_p + jitter removed).  One CTA per candidate c: for each of the n simulations the extremum over p.
-//   cov[P, P] (symmetric; row c is read), ysim[n, P], diag_sub = noise_p + jitter, nj = noise + jitter
+//   cov[P, P] (symmetric; row c is read), ysim[n, P], diag_sub = noise_p + jitter, nj = noise + jitter; or, when
+//   diag_sub_v / nj_v are given, per-candidate values diag_sub_v[c], nj_v[c] (a noise per task: the LCM models)
+template <bool PER_CANDIDATE>
 __global__ void __launch_bounds__(256) kg_kernel(const double* __restrict__ mean, const double* __restrict__ cov, int64_t ldc,
                                                  const double* __restrict__ ysim, int n, int64_t P, double diag_sub, double nj,
+                                                 const double* __restrict__ diag_sub_v, const double* __restrict__ nj_v,
                                                  int maximize, const double* __restrict__ best_mean, double* __restrict__ out) {
     __shared__ double red[8];
     const int64_t c = blockIdx.x;
+    if (PER_CANDIDATE) {
+        diag_sub = diag_sub_v[c];
+        nj = nj_v[c];
+    }
     const double c0cc = cov[c * ldc + c] - diag_sub;
     const double inv_s = 1.0 / (c0cc + nj);
     const double mc = mean[c];

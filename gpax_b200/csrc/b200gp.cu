@@ -1375,7 +1375,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                     double* grad_noise_vec, int* info, const MtDesc* mt = nullptr, double* grad_x_dev = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, !grad_noise_vec || grad);
-    ARG_CHECK(ctx, !grad_x_dev || (grad && !mt && !noise_vec));
+    ARG_CHECK(ctx, !grad_x_dev || (grad && !noise_vec && (!mt || kind != B2GP_KERNEL_PERIODIC)));
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     ARG_CHECK(ctx, X && yres && theta && value && info);
     ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= MLL_MAX_D);
@@ -1457,6 +1457,9 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                               (const double*)alpha, (const double*)Kinv, ld, partial));
                 RET_IF(launch(ctx, st, (unsigned)(L * nout), MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial,
                               tiles * tiles, nout, gmt));
+                if (grad_x_dev)   // d value / d X [N, d] of the LCM covariance on the device (dkl.cuh)
+                    RET_IF(launch(ctx, st, (unsigned)ceil_div(N, DZ_ROWS), DZ_THREADS, 0, mll_lcm_dz_kernel, kind, dX, dtask, N, d, T, L,
+                                  dth, (const double*)dmt, (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
             } else {
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv,
                               ld, partial));
@@ -1622,9 +1625,74 @@ extern "C" int b2gp_mlp_forward(b2gp_ctx* ctx, const double* X, int64_t N, int64
     return B2GP_OK;
 }
 
+// The backward pass's scratch in ctx->mlp[3]: gz [N, d] | grad params | G ping-pong 2 x [N, max_out] | H_l^T [max_in, ldN]
+// | G^T [max_out, ldN].  `tot` with the backward pass, `o_gp` (gz alone) without it.
+struct MlpBack {
+    int64_t ldN, o_gp, o_g0, o_g1, o_ht, o_gt, tot;
+};
+
+static MlpBack mlp_back_layout(const MlpShape& s) {
+    MlpBack b;
+    b.ldN = round_up(s.N, 8);
+    b.o_gp = round_up(s.N * s.d, 8);
+    b.o_g0 = b.o_gp + round_up(s.nparams, 8);
+    b.o_g1 = b.o_g0 + round_up(s.N * s.max_out, 8);
+    b.o_ht = b.o_g1 + round_up(s.N * s.max_out, 8);
+    b.o_gt = b.o_ht + s.max_in * b.ldN;
+    b.tot = b.o_gt + s.max_out * b.ldN;
+    return b;
+}
+
+// The backward pass from gz = d value / dz (at base, the start of mlp[3]) to grad_params (HOST): per layer the bias
+// gradient (column sum), the weight gradient H_l^T G (gemm_nt on the transposes) and, below the first layer, G W_l^T
+// masked by the activation's derivative.
+static int mlp_backward_dev(b2gp_ctx* ctx, cudaStream_t st, const MlpShape& s, const MlpBack& b, int act, const double* dP,
+                            const std::vector<double*>& H, double* base, double* grad_params) {
+    const int64_t N = s.N, ldN = b.ldN;
+    double *gp = base + b.o_gp, *G0 = base + b.o_g0, *G1 = base + b.o_g1, *Ht = base + b.o_ht, *Gt = base + b.o_gt;
+    double* G = base;   // d value / d (pre-activation output of layer l), [N, out_l]
+    for (int l = s.L - 1; l >= 0; --l) {
+        const int64_t in = s.in[l], out = s.out[l];
+        RET_IF(launch(ctx, st, (unsigned)out, MLP_SUM_THREADS, 0, mlp_colsum_kernel, (const double*)G, out, N, gp + s.boff[l]));
+        RET_IF(launch_transpose(ctx, st, H[l], in, N, in, Ht, ldN));
+        RET_IF(launch_transpose(ctx, st, G, out, N, out, Gt, ldN));
+        RET_IF(gemm_nt(ctx, st, in, out, N, 1.0, Ht, ldN, Gt, ldN, 0.0, gp + s.woff[l], out, false));
+        if (l > 0) {
+            double* Gn = G == G0 ? G1 : G0;
+            RET_IF(gemm_nt(ctx, st, N, in, out, 1.0, G, out, dP + s.woff[l], out, 0.0, Gn, in, false));
+            RET_IF(launch(ctx, st, grid_for(N * in), 256, 0, mlp_act_grad_kernel, Gn, in, (const double*)H[l], in, N, (int)in, act));
+            G = Gn;
+        }
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, gp, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
+    return B2GP_OK;
+}
+
+// b2gp_last_timing of a deep-kernel step reports the whole step: mll_impl's own timer covers only its part, so the call
+// is bracketed by a second pair of events and its totals replace mll_impl's at the end
+struct StepTimer {
+    std::chrono::steady_clock::time_point t0;
+    int64_t launches0 = 0;
+    int begin(b2gp_ctx* ctx, cudaStream_t st) {
+        t0 = std::chrono::steady_clock::now();
+        launches0 = ctx->launches;
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
+        return B2GP_OK;
+    }
+    int end(b2gp_ctx* ctx, cudaStream_t st) {
+        CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
+        CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_b));
+        float ms = 0.f;
+        CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
+        ctx->last.total_ms = ms;
+        ctx->last.launches = ctx->launches - launches0;
+        ctx->last.host_enqueue_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        return B2GP_OK;
+    }
+};
+
 // viDKL / DKL's likelihood on z = MLP(X): forward pass, then mll_impl on z (the b2gp_mll route, with d value / dz from
-// mll_dz_kernel), then the backward pass through the layers: per layer the bias gradient (column sum), the weight gradient
-// H_l^T G (gemm_nt on the transposes) and, below the first layer, G W_l^T masked by the activation's derivative.
+// mll_dz_kernel), then the backward pass through the layers (mlp_backward_dev).
 extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D, const double* yres, int n_layers,
                             const int64_t* widths, int act, const double* params, const double* theta, double jitter, unsigned flags,
                             double* value, double* grad_theta, double* grad_params, double* grad_z, int* info) {
@@ -1637,11 +1705,8 @@ extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N,
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     ctx->fcache.valid = false;
     cudaStream_t st = ctx->slots[0].stream;
-    // b2gp_last_timing reports the whole step: mll_impl's own timer covers only its part, so the call is bracketed by
-    // a second pair of events and its totals replace mll_impl's at the end
-    const auto t0 = std::chrono::steady_clock::now();
-    const int64_t launches0 = ctx->launches;
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, st));
+    StepTimer tm;
+    RET_IF(tm.begin(ctx, st));
     const bool dev = dev_ptrs(flags);
     const double *dX, *dy, *dP = nullptr;
     RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev, &dX));
@@ -1650,11 +1715,8 @@ extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N,
     std::vector<double*> H;
     RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP, H));
     const bool back = grad_params && n_layers > 0;
-    // backward scratch: gz [N, d] | grad params | G ping-pong 2 x [N, max_out] | H_l^T [max_in, ldN] | G^T [max_out, ldN]
-    const int64_t ldN = round_up(N, 8);
-    const int64_t o_gp = round_up(N * s.d, 8), o_g0 = o_gp + round_up(s.nparams, 8), o_g1 = o_g0 + round_up(N * s.max_out, 8);
-    const int64_t o_ht = o_g1 + round_up(N * s.max_out, 8), o_gt = o_ht + s.max_in * ldN, tot = o_gt + s.max_out * ldN;
-    RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(back ? tot : o_gp) * 8));
+    const MlpBack b = mlp_back_layout(s);
+    RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(back ? b.tot : b.o_gp) * 8));
     double* gz = (double*)ctx->mlp[3].p;
     const int64_t d = s.d;
     RET_IF(mll_impl(ctx, kind, H[s.L], N, dy, (int)d, theta, nullptr, jitter, B2GP_FLAG_DEVICE_PTRS, value, grad_theta, nullptr, nullptr,
@@ -1665,33 +1727,75 @@ extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N,
         for (int64_t i = 0; i < ngp; ++i) grad_params[i] = NAN;
     }
     if (grad_z && *info == 0) CUDA_TRY(ctx, cudaMemcpyAsync(grad_z, gz, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
-    if (back && *info == 0) {
-        double* base = (double*)ctx->mlp[3].p;
-        double *gp = base + o_gp, *G0 = base + o_g0, *G1 = base + o_g1, *Ht = base + o_ht, *Gt = base + o_gt;
-        double* G = gz;   // d value / d (pre-activation output of layer l), [N, out_l]
-        for (int l = s.L - 1; l >= 0; --l) {
-            const int64_t in = s.in[l], out = s.out[l];
-            RET_IF(launch(ctx, st, (unsigned)out, MLP_SUM_THREADS, 0, mlp_colsum_kernel, (const double*)G, out, N, gp + s.boff[l]));
-            RET_IF(launch_transpose(ctx, st, H[l], in, N, in, Ht, ldN));
-            RET_IF(launch_transpose(ctx, st, G, out, N, out, Gt, ldN));
-            RET_IF(gemm_nt(ctx, st, in, out, N, 1.0, Ht, ldN, Gt, ldN, 0.0, gp + s.woff[l], out, false));
-            if (l > 0) {
-                double* Gn = G == G0 ? G1 : G0;
-                RET_IF(gemm_nt(ctx, st, N, in, out, 1.0, G, out, dP + s.woff[l], out, 0.0, Gn, in, false));
-                RET_IF(launch(ctx, st, grid_for(N * in), 256, 0, mlp_act_grad_kernel, Gn, in, (const double*)H[l], in, N, (int)in, act));
-                G = Gn;
-            }
-        }
-        CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, gp, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
+    if (back && *info == 0) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, gz, grad_params));
+    return tm.end(ctx, st);
+}
+
+// viMTDKL's likelihood: the forward pass on the N points, z expanded to the N * group GP rows (point-major, one device
+// copy per task slot), mll_impl on the rows with the LCM covariance (the b2gp_mll_multitask route, d value / dz from
+// mll_lcm_dz_kernel), each point's rows summed in task order (group_sum_kernel), then the backward pass.
+extern "C" int b2gp_mtdkl_mll(b2gp_ctx* ctx, int kind, const double* X, const int* task, int64_t N, int64_t D, const double* yres,
+                              int group, int T, int L, int n_layers, const int64_t* widths, int act, const double* params,
+                              const double* theta, const double* B, const double* noise, double jitter, unsigned flags,
+                              double* value, double* grad_theta, double* grad_B, double* grad_noise, double* grad_params,
+                              double* grad_z, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, X && yres && theta && B && noise && value && grad_theta && grad_B && grad_noise && info);
+    ARG_CHECK(ctx, group >= 1 && (n_layers == 0 || params));
+    if (kind == B2GP_KERNEL_PERIODIC)
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_mtdkl_mll", "RBF and Matern only (viMTDKL samples no period)", __FILE__,
+                       __LINE__);
+    const int64_t R = N * group;   // GP rows
+    // task ids and limits before any launch; X and yres may be device pointers here, the arrays mt_check sees are host
+    RET_IF(mt_check(ctx, "b2gp_mtdkl_mll", kind, flags & ~B2GP_FLAG_DEVICE_PTRS, (int)s.d, group, T, L, task, R, nullptr, 0));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    StepTimer tm;
+    RET_IF(tm.begin(ctx, st));
+    const bool dev = dev_ptrs(flags);
+    const double *dX, *dy, *dP = nullptr;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev, &dX));
+    RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)R * 8, dev, &dy));
+    if (n_layers > 0) RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)s.nparams * 8, false, &dP));
+    std::vector<double*> H;
+    RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP, H));
+    const bool back = grad_params && n_layers > 0, want_z = grad_z || back;
+    const int64_t d = s.d;
+    // mlp[3]: the backward scratch (gz at its start), then z and d value / dz on the rows when group > 1
+    const MlpBack b = mlp_back_layout(s);
+    const int64_t o_rows = back ? b.tot : b.o_gp, nrow = group > 1 ? round_up(R * d, 8) : 0;
+    RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(o_rows + 2 * nrow) * 8));
+    double* gz = (double*)ctx->mlp[3].p;
+    const double* zr = H[s.L];
+    double* gzr = gz;
+    if (group > 1) {
+        double* zrows = gz + o_rows;
+        gzr = zrows + nrow;
+        for (int t = 0; t < group; ++t)
+            CUDA_TRY(ctx, cudaMemcpy2DAsync(zrows + t * d, (size_t)group * d * 8, H[s.L], (size_t)d * 8, (size_t)d * 8, (size_t)N,
+                                            cudaMemcpyDeviceToDevice, st));
+        zr = zrows;
     }
-    CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, st));
-    CUDA_TRY(ctx, cudaEventSynchronize(ctx->ev_b));
-    float ms = 0.f;
-    CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b));
-    ctx->last.total_ms = ms;
-    ctx->last.launches = ctx->launches - launches0;
-    ctx->last.host_enqueue_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-    return B2GP_OK;
+    const MtDesc mt{task, nullptr, group, T, L, B, noise};
+    std::vector<double> g((size_t)L * (d + 2) + (size_t)L * T * T + T);
+    RET_IF(mll_impl(ctx, kind, zr, R, dy, (int)d, theta, nullptr, jitter, B2GP_FLAG_DEVICE_PTRS, value, g.data(), nullptr, nullptr,
+                    info, &mt, want_z ? gzr : nullptr));
+    memcpy(grad_theta, g.data(), (size_t)L * (d + 2) * 8);
+    memcpy(grad_B, g.data() + (size_t)L * (d + 2), (size_t)L * T * T * 8);
+    memcpy(grad_noise, g.data() + (size_t)L * (d + 2) + (size_t)L * T * T, (size_t)T * 8);
+    const int64_t ngp = grad_params ? s.nparams : 0;
+    if (*info != 0) {
+        for (int64_t i = 0; grad_z && i < N * d; ++i) grad_z[i] = NAN;
+        for (int64_t i = 0; i < ngp; ++i) grad_params[i] = NAN;
+    }
+    if (want_z && group > 1 && *info == 0)
+        RET_IF(launch(ctx, st, grid_for(N * d), 256, 0, group_sum_kernel, (const double*)gzr, N, (int)d, group, gz));
+    if (grad_z && *info == 0) CUDA_TRY(ctx, cudaMemcpyAsync(grad_z, gz, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
+    if (back && *info == 0) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, gz, grad_params));
+    return tm.end(ctx, st);
 }
 
 // value and gradient of the VFE bound of the sparse GP (see sparse_elbo.cuh): d/dlog(lengthscale[d], k_scale, noise, period)
@@ -1940,8 +2044,9 @@ extern "C" int b2gp_acq_samples(b2gp_ctx* ctx, int kind, const double* y, int64_
     return tm.end(st, nullptr);
 }
 
-extern "C" int b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n,
-                       double diag_sub, double noise_plus_jitter, int maximize, double* out, unsigned flags) {
+// The knowledge gradient's rank-1 update on the device; diag_sub_v / nj_v (both or neither) give per-candidate values
+static int kg_impl(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n, double diag_sub,
+                   double noise_plus_jitter, const double* diag_sub_v, const double* nj_v, int maximize, double* out, unsigned flags) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, mean && cov && ysim && out && P >= 1 && n >= 1);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
@@ -1949,10 +2054,14 @@ extern "C" int b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int
     cudaStream_t st = ctx->slots[0].stream;
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
-    const double *dmean, *dcov, *dys;
+    const double *dmean, *dcov, *dys, *dds = nullptr, *dnj = nullptr;
     RET_IF(stage_in(ctx, st, ctx->d_in[0], mean, (size_t)P * 8, dev, &dmean));
     RET_IF(stage_in(ctx, st, ctx->d_in[1], cov, (size_t)P * P * 8, dev, &dcov));
     RET_IF(stage_in(ctx, st, ctx->d_in[2], ysim, (size_t)n * P * 8, dev, &dys));
+    if (diag_sub_v) {
+        RET_IF(stage_in(ctx, st, ctx->d_in[3], diag_sub_v, (size_t)P * 8, dev, &dds));
+        RET_IF(stage_in(ctx, st, ctx->d_in[4], nj_v, (size_t)P * 8, dev, &dnj));
+    }
     double* dout = out;
     if (!dev) {
         RET_IF(ensure(ctx, ctx->d_out[0], (size_t)P * 8));
@@ -1961,9 +2070,26 @@ extern "C" int b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int
     RET_IF(ensure(ctx, ctx->slots[0].misc, 16 * 8));
     double* dbest = (double*)ctx->slots[0].misc.p;
     RET_IF(launch(ctx, st, 1, 256, 0, acq_best_kernel, dmean, P, P, maximize, dbest));
-    RET_IF(launch(ctx, st, (unsigned)P, 256, 0, kg_kernel, dmean, dcov, P, dys, (int)n, P, diag_sub, noise_plus_jitter, maximize, dbest, dout));
+    if (diag_sub_v)
+        RET_IF(launch(ctx, st, (unsigned)P, 256, 0, kg_kernel<true>, dmean, dcov, P, dys, (int)n, P, diag_sub, noise_plus_jitter, dds, dnj,
+                      maximize, dbest, dout));
+    else
+        RET_IF(launch(ctx, st, (unsigned)P, 256, 0, kg_kernel<false>, dmean, dcov, P, dys, (int)n, P, diag_sub, noise_plus_jitter, dds, dnj,
+                      maximize, dbest, dout));
     if (!dev) CUDA_TRY(ctx, cudaMemcpyAsync(out, dout, (size_t)P * 8, cudaMemcpyDeviceToHost, st));
     return tm.end(st, nullptr);
+}
+
+extern "C" int b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n,
+                       double diag_sub, double noise_plus_jitter, int maximize, double* out, unsigned flags) {
+    return kg_impl(ctx, mean, cov, P, ysim, n, diag_sub, noise_plus_jitter, nullptr, nullptr, maximize, out, flags);
+}
+
+extern "C" int b2gp_kg_v(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n,
+                         const double* diag_sub, const double* noise_plus_jitter, int maximize, double* out, unsigned flags) {
+    if (!ctx) return B2GP_ERR_ARG;
+    ARG_CHECK(ctx, diag_sub && noise_plus_jitter);
+    return kg_impl(ctx, mean, cov, P, ysim, n, 0.0, 0.0, diag_sub, noise_plus_jitter, maximize, out, flags);
 }
 
 // ------------------------------------------------------------------------------------------ debug

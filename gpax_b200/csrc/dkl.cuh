@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "grad.cuh"
 #include "mll.cuh"
+#include "mtgp.cuh"
 
 constexpr int DZ_ROWS = 32;      // rows i per CTA
 constexpr int DZ_COLS = 32;      // columns j per tile
@@ -125,6 +126,113 @@ mll_dz_kernel(int kind, const double* __restrict__ Z, int64_t N, int d, const do
 #pragma unroll
         for (int k = 0; k < MLL_MAX_D; ++k)
             if (k < d) G[i * d + k] = acc[k];
+    }
+}
+
+// mll_lcm_dz_kernel: the same gradient for the LCM covariance of gram_lcm_kernel (mtgp.cuh, viMTDKL):
+//     g_i[k] = sum_{j != i} W_ij sum_q B_q[t_i, t_j] dk_q(z_i, z_j)/dz_i[k]
+// with latent q's lengthscales ell_q and scale.  The jitter, the noise (L times on the diagonal) and the same-point jitter
+// block of the Kronecker form do not depend on z; pairs at one point have z_i = z_j and contribute exactly zero.  RBF and
+// Matern only (the reference's viMTDKL samples no period).  mll_dz_kernel's tiling, K^{-1} access and fixed reduction
+// order; theta_q and B_q of every latent staged in shared memory as gram_lcm_kernel does, the row and column tiles once
+// per latent (scaled by 1 / ell_q), the task ids once.
+__global__ void __launch_bounds__(DZ_THREADS)
+mll_lcm_dz_kernel(int kind, const double* __restrict__ Z, const int* __restrict__ task, int64_t N, int d, int T, int L,
+                  const double* __restrict__ theta, const double* __restrict__ B, const double* __restrict__ alpha,
+                  const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ G) {
+    __shared__ double Ws[DZ_ROWS][DZ_COLS + 1];
+    __shared__ double Zi[MT_MAX_L][DZ_ROWS][MLL_MAX_D];
+    __shared__ double Zj[MT_MAX_L][DZ_COLS][MLL_MAX_D];
+    __shared__ double th[MT_MAX_L * (MLL_MAX_D + 2)];
+    __shared__ double Bs[MT_MAX_L * MT_MAX_T * MT_MAX_T];
+    __shared__ int ti[DZ_ROWS], tj[DZ_COLS];
+    const int tid = threadIdx.x, nth = d + 2;
+    const int64_t i0 = (int64_t)blockIdx.x * DZ_ROWS;
+    for (int idx = tid; idx < L * nth; idx += DZ_THREADS) th[idx] = theta[idx];
+    for (int idx = tid; idx < L * T * T; idx += DZ_THREADS) Bs[idx] = B[idx];
+    if (tid < DZ_ROWS) ti[tid] = i0 + tid < N ? task[i0 + tid] : 0;
+    __syncthreads();
+    for (int idx = tid; idx < L * DZ_ROWS * d; idx += DZ_THREADS) {
+        const int q = idx / (DZ_ROWS * d), r = (idx / d) % DZ_ROWS, k = idx % d;
+        const int64_t gi = i0 + r;
+        Zi[q][r][k] = (gi < N ? Z[gi * d + k] : 0.0) / th[q * nth + k];
+    }
+    const int r = tid / DZ_TPR, c0 = tid % DZ_TPR;
+    const int64_t i = i0 + r;
+    double acc[MLL_MAX_D];
+#pragma unroll
+    for (int k = 0; k < MLL_MAX_D; ++k) acc[k] = 0.0;
+    for (int64_t j0 = 0; j0 < N; j0 += DZ_COLS) {
+        __syncthreads();
+        for (int idx = tid; idx < DZ_ROWS * DZ_COLS; idx += DZ_THREADS) {
+            // left of the diagonal block: consecutive threads along a row of K^{-1}; right of it: along a column
+            const bool left = j0 < i0;
+            const int rr = left ? idx / DZ_COLS : idx % DZ_ROWS, cc = left ? idx % DZ_COLS : idx / DZ_ROWS;
+            const int64_t gi = i0 + rr, gj = j0 + cc;
+            double w = 0.0;
+            if (gi < N && gj < N && gi != gj) {
+                const int64_t hi = gi > gj ? gi : gj, lo = gi > gj ? gj : gi;
+                w = alpha[gi] * alpha[gj] - Kinv[hi * ldk + lo];
+            }
+            Ws[rr][cc] = w;
+        }
+        for (int idx = tid; idx < L * DZ_COLS * d; idx += DZ_THREADS) {
+            const int q = idx / (DZ_COLS * d), c = (idx / d) % DZ_COLS, k = idx % d;
+            const int64_t gj = j0 + c;
+            Zj[q][c][k] = (gj < N ? Z[gj * d + k] : 0.0) / th[q * nth + k];
+        }
+        if (tid < DZ_COLS) tj[tid] = j0 + tid < N ? task[j0 + tid] : 0;
+        __syncthreads();
+        if (i >= N) continue;
+        for (int c = c0; c < DZ_COLS; c += DZ_TPR) {
+            const double w = Ws[r][c];
+            if (w == 0.0) continue;     // outside the matrix, the diagonal, or an exact zero: contributes nothing
+            const double* Bp = Bs + ti[r] * T + tj[c];
+            for (int q = 0; q < L; ++q) {
+                const double* zi = Zi[q][r];
+                const double* zj = Zj[q][c];
+                const double* ell = th + q * nth;
+                double x2 = 0.0, xz = 0.0, z2 = 0.0;
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k) {
+                    if (k < d) {
+                        x2 = fma(zi[k], zi[k], x2);
+                        xz = fma(zi[k], zj[k], xz);
+                        z2 = fma(zj[k], zj[k], z2);
+                    }
+                }
+                const double wg = w * Bp[q * T * T] * stationary_dk_dr2(kind, (x2 - 2.0 * xz) + z2, ell[d]);
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k)
+                    if (k < d) acc[k] = fma(wg, 2.0 * (zi[k] - zj[k]) / ell[k], acc[k]);
+            }
+        }
+    }
+    // the DZ_TPR threads of a row are consecutive lanes: a fixed xor tree
+#pragma unroll
+    for (int k = 0; k < MLL_MAX_D; ++k) {
+        if (k < d) {
+            double v = acc[k];
+#pragma unroll
+            for (int o = DZ_TPR / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+            acc[k] = v;
+        }
+    }
+    if (c0 == 0 && i < N) {
+#pragma unroll
+        for (int k = 0; k < MLL_MAX_D; ++k)
+            if (k < d) G[i * d + k] = acc[k];
+    }
+}
+
+// G[p, k] = sum_{t < group} Gr[p * group + t, k]: a point's gradient from its `group` rows (the Kronecker form), in task order
+__global__ void group_sum_kernel(const double* __restrict__ Gr, int64_t n, int d, int group, double* __restrict__ G) {
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n * d; idx += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t p = idx / d;
+        const int k = (int)(idx % d);
+        double s = 0.0;
+        for (int t = 0; t < group; ++t) s += Gr[(p * group + t) * d + k];
+        G[idx] = s;
     }
 }
 

@@ -46,6 +46,13 @@ def _refuse(nn, latent_prior, input_dim, nn_prior_program=None):
     return int(input_dim)
 
 
+def _nn_log_prior(wmask, flat):
+    """log p of the network sites with Normal(0, 1) weights and Cauchy(0, 1) biases (vidkl.py:93-96) and its gradient"""
+    normal, cauchy = P.Normal(0.0, 1.0), P.Cauchy(0.0, 1.0)
+    val = float(np.sum(normal.log_prob(flat[wmask]))) + float(np.sum(cauchy.log_prob(flat[~wmask])))
+    return val, np.where(wmask, normal.dlog_prob(flat), cauchy.dlog_prob(flat))
+
+
 class _MLPModel(ExactGP):
     """What viDKL and DKL share: the layer widths, the kernel sites and the embedding on the GPU."""
 
@@ -174,6 +181,10 @@ class viDKL(_MLPModel):
     def _init_params(self, rng):
         """(u_theta, flat network parameters) at the start of the fit (see the module docstring)"""
         u = np.array([float(pr.inverse(pr.median())) for _, pr, _ in self._kernel_sites()])
+        return u, self._init_network(rng)
+
+    def _init_network(self, rng):
+        """the flat network parameters at the start of the fit"""
         parts = []
         for i, w in self._shapes():
             if self.nn_prior:
@@ -186,15 +197,23 @@ class viDKL(_MLPModel):
                     W[bad] = rng.standard_normal(int(bad.sum()))
                 W, b = W / math.sqrt(i), np.zeros(w)
             parts += [W.ravel(), b]
-        return u, np.concatenate(parts)
+        return np.concatenate(parts)
 
-    def _log_joint(self, Xd, yd, jitter):
+    def _weight_mask(self):
+        """True at the weights, False at the biases of the flat layout"""
+        return np.concatenate([np.r_[np.ones(i * w), np.zeros(w)] for i, w in self._shapes()]).astype(bool)
+
+    def _mlp_inputs(self, X):
+        """the network's input rows of a (2-d) input array"""
+        return X
+
+    def _log_joint(self, X, Xd, yd, jitter):
         """log p(y, sites) over (u_theta, flat) and its gradient; priors on theta in the constrained space without the
-        Jacobian (as fit_vi_gp), Normal(0, 1) weights and Cauchy(0, 1) biases when nn_prior (vidkl.py:93-96)"""
+        Jacobian (as fit_vi_gp), Normal(0, 1) weights and Cauchy(0, 1) biases when nn_prior (vidkl.py:93-96).  X: the
+        host inputs, Xd / yd: the network's inputs and the targets on the device."""
         sites = self._kernel_sites()
         nth = len(sites)
-        wmask = np.concatenate([np.r_[np.ones(i * w), np.zeros(w)] for i, w in self._shapes()]).astype(bool)
-        normal, cauchy = P.Normal(0.0, 1.0), P.Cauchy(0.0, 1.0)
+        wmask = self._weight_mask()
 
         def f(v, jacobian=False):
             u, flat = v[:nth], v[nth:]
@@ -211,8 +230,9 @@ class viDKL(_MLPModel):
                     val += float(pr.log_abs_jac(u[k]))
                     gu[k] += float(pr.dlog_abs_jac(u[k]))
             if self.nn_prior:
-                val += float(np.sum(normal.log_prob(flat[wmask]))) + float(np.sum(cauchy.log_prob(flat[~wmask])))
-                gp = gp + np.where(wmask, normal.dlog_prob(flat), cauchy.dlog_prob(flat))
+                lp, glp = _nn_log_prior(wmask, flat)
+                val += lp
+                gp = gp + glp
             return val, np.concatenate([gu, gp])
         return f, nth
 
@@ -223,9 +243,9 @@ class viDKL(_MLPModel):
         X = np.asarray(self._set_data(X), dtype=np.float64)
         y = np.asarray(y, dtype=np.float64).reshape(-1)
         rng = seed_from_key(rng_key)
-        Xd, yd = self.ctx.to_device(X), self.ctx.to_device(y)       # uploaded once for the whole fit
+        Xd, yd = self.ctx.to_device(self._mlp_inputs(X)), self.ctx.to_device(y)       # uploaded once for the whole fit
         try:
-            f, nth = self._log_joint(Xd, yd, float(kwargs.get("jitter", 1e-6)))
+            f, nth = self._log_joint(X, Xd, yd, float(kwargs.get("jitter", 1e-6)))
             u0, flat0 = self._init_params(rng)
             loc = np.concatenate([u0, flat0])
             dim = loc.size
@@ -506,3 +526,233 @@ class DKL(_MLPModel):
             if k in s:
                 v = np.asarray(s[k])
                 print(f"{k:>12s}  mean {np.mean(v, axis=0)}  std {np.std(v, axis=0)}")
+
+
+# ------------------------------------------------------------------------------------------------------------ viMTDKL
+class viMTDKL(viDKL):
+    """
+    Multi-task deep kernel learning (gpax/models/vi_mtdkl.py): viDKL's ReLU MLP (64, 64, z_dim) embeds the inputs and the
+    GP on the embedding has the LCM covariance of MultiTaskGP, sum_q (k_q(z, z') + jitter [same point]) B_q[t, t'] with
+    B_q = W_q W_q^T + diag(v_q).  The network and the kernel sites are fitted jointly by SVI as in viDKL; the likelihood
+    and its gradient w.r.t. every site and weight come from b2gp_mtdkl_mll, the posterior from b2gp_posterior_multitask
+    on the embeddings.  Both forms of the reference:
+      * multitask form (shared_input_space=False): one row per observation, its task id in the last column of X; the
+        network sees X[:, :-1];
+      * Kronecker form (shared_input_space=True, needs num_tasks): every task observed at every input, y of length N*T
+        in point-major order (point i, task t at i*T + t); predictions have length P*T in the same order.
+
+    Sites (vi_mtdkl.py:163-209): k_length LogNormal(0, 1) [L, z_dim], k_scale Normal(1, 1e-4) [L, 1], W Normal(0, 10)
+    [L, T, rank] (or W_prior_dist), v LogNormal(0, 1) [L, T] (or v_prior_dist), noise LogNormal(0, 1) [T] (or
+    noise_prior_dist).  `kernel_params` carries them in these shapes.  T defaults to the distinct labels of the task
+    column, rank to T - 1.  The kernel sites start at their prior median, except W, whose median 0 is a stationary point
+    of the loss (d/dW = (G + G^T) W = 0 there and the prior's gradient is 0 too): W starts, as the network's weights do,
+    at the element-wise median of INIT_MEDIAN_DRAWS prior draws (numpyro's init_to_median).
+
+    Differences from the reference: `embed` strips the task column of the multitask form before the network (the
+    reference would feed it to the network, whose input width it does not match).  Refused: data_kernel 'Periodic' (the
+    reference samples no period, so its own model fails there), data_kernel_prior / task_kernel_prior programs and custom
+    networks (as viDKL).  Limits of the GPU path: T <= 8, L <= 4, z_dim <= 16.
+
+    Acquisition functions: EI / UCB / POI / UE work through `predict`; KG works in the multitask form, with the
+    candidate's task setting its noise in the rank-1 update (`_kg_terms`), and raises NotImplementedError in the
+    Kronecker form; the q-batch functions (qEI, qUCB, qPOI, qKG) need a fully Bayesian model and raise ValueError, as for
+    viDKL and in the reference; `acquisition.optimize_acq` takes finite differences for this model.
+    """
+
+    def __init__(self, input_dim, z_dim: int = 2, data_kernel: str = "RBF", num_latents: Optional[int] = None,
+                 shared_input_space: bool = False, num_tasks: Optional[int] = None, rank: Optional[int] = None,
+                 data_kernel_prior=None, nn=None, nn_prior: bool = True, guide: str = "delta", W_prior_dist=None,
+                 v_prior_dist=None, task_kernel_prior=None, ctx=None, **kwargs) -> None:
+        if data_kernel == "Periodic":
+            raise NotImplementedError("viMTDKL takes data_kernel 'RBF' or 'Matern': the reference samples no period for "
+                                      "'Periodic', so its own model fails there")
+        if data_kernel not in ("RBF", "Matern"):
+            raise NotImplementedError("viMTDKL takes data_kernel 'RBF' or 'Matern'")
+        if data_kernel_prior is not None or task_kernel_prior is not None:
+            raise NotImplementedError("data_kernel_prior / task_kernel_prior programs are not supported by viMTDKL; use "
+                                      "W_prior_dist, v_prior_dist and noise_prior_dist")
+        super().__init__(input_dim, z_dim, data_kernel, None, nn, nn_prior, None, guide, ctx=ctx, **kwargs)
+        if shared_input_space:                                  # vi_mtdkl.py:85-91
+            if num_tasks is None:
+                raise ValueError("Please specify num_tasks")
+        elif num_latents is None:
+            raise ValueError("Please specify num_latents")
+        self.num_tasks = num_tasks
+        self.num_latents = num_tasks if num_latents is None else num_latents
+        self.rank = rank
+        self.shared_input = bool(shared_input_space)
+        self.W_prior_dist = W_prior_dist
+        self.v_prior_dist = v_prior_dist
+
+    # ---- shapes and sites
+    def _num_tasks(self):
+        if self.num_tasks is None:                              # vi_mtdkl.py:108-109
+            return len(np.unique(np.asarray(self.X_train)[:, -1]))
+        return int(self.num_tasks)
+
+    def _site_list(self):
+        """(name, prior, shape) of the kernel and noise sites in the reference's order (vi_mtdkl.py:130-209)"""
+        L, T, d = int(self.num_latents), self._num_tasks(), self.kernel_dim
+        R = int(self.rank) if self.rank is not None else T - 1
+        return [("k_length", P.LogNormal(0.0, 1.0), (L, d)), ("k_scale", P.Normal(1.0, 1e-4), (L, 1)),
+                ("W", self.W_prior_dist or P.Normal(0.0, 10.0), (L, T, R)),
+                ("v", self.v_prior_dist or P.LogNormal(0.0, 1.0), (L, T)),
+                ("noise", self.noise_prior_dist or P.LogNormal(0.0, 1.0), (T,))]
+
+    def _points(self, X):
+        """(network inputs [n, D], int32 task ids of the GP rows, group) of an input array"""
+        from .mtgp import lcm_points
+        return lcm_points(self._set_data(X), self._num_tasks(), self.shared_input)
+
+    def _mlp_inputs(self, X):
+        return self._points(X)[0]
+
+    def _theta(self, u):
+        """the unconstrained vector of the kernel sites -> {name: constrained value in the site's shape}"""
+        out, o = {}, 0
+        for name, pr, shape in self._site_list():
+            n = int(np.prod(shape))
+            out[name] = np.asarray(pr.transform(u[o:o + n]), dtype=np.float64).reshape(shape)
+            o += n
+        return out
+
+    def _kernel_dict(self, sites):
+        return sites
+
+    def _lcm(self, kp):
+        """a kernel_params dict (one draw) -> theta [L, d+2], B [L, T, T], noise [T] of the C ABI"""
+        from .mtgp import lcm_task_matrix
+        L, T, d = int(self.num_latents), self._num_tasks(), self.kernel_dim
+        theta = np.ones((L, d + 2))
+        theta[:, :d] = np.broadcast_to(np.asarray(kp["k_length"], dtype=np.float64).reshape(L, -1), (L, d))
+        theta[:, d] = np.asarray(kp["k_scale"], dtype=np.float64).reshape(L)
+        B = lcm_task_matrix(np.asarray(kp["W"], dtype=np.float64).reshape(L, T, -1), np.asarray(kp["v"]).reshape(L, T))
+        noise = np.broadcast_to(np.asarray(kp["noise"], dtype=np.float64).reshape(-1), (T,)).copy()
+        return theta, B, noise
+
+    # ---- fit
+    def _init_params(self, rng):
+        """kernel sites at their prior median, W at the median of INIT_MEDIAN_DRAWS prior draws (see the class docstring),
+        then the network as viDKL"""
+        u = []
+        for name, pr, shape in self._site_list():
+            if name == "W":
+                u.append(np.asarray(pr.inverse(np.median(pr.sample(rng, (INIT_MEDIAN_DRAWS,) + shape), axis=0))).ravel())
+            else:
+                u.append(np.full(int(np.prod(shape)), float(pr.inverse(pr.median()))))
+        return np.concatenate(u), self._init_network(rng)
+
+    def _log_joint(self, X, Xd, yd, jitter):
+        """log p(y, sites) over (u of the kernel sites, flat network parameters) and its gradient: b2gp_mtdkl_mll's
+        likelihood, the sites' priors in the constrained space without the Jacobian (as viDKL), the network's prior"""
+        sites = self._site_list()
+        nth = sum(int(np.prod(sh)) for _, _, sh in sites)
+        _, task, group = self._points(X)
+        wmask = self._weight_mask()
+
+        def f(v, jacobian=False):
+            u, flat = v[:nth], v[nth:]
+            kp = self._theta(u)
+            theta, B, noise = self._lcm(kp)
+            val, gt, gB, gn, gp, _, info = self.ctx.mtdkl_mll(self._fused, Xd, task, yd, self.widths, self.act, flat, theta, B,
+                                                              noise, group, jitter)
+            if info != 0 or not np.isfinite(val):
+                return -np.inf, np.zeros_like(v)
+            d = self.kernel_dim
+            # d value / d (constrained site): the C ABI's d/dlog for lengthscales, scale and noise; B's chain rule to W, v
+            g = {"k_length": gt[:, :d] / kp["k_length"], "k_scale": (gt[:, d] / theta[:, d]).reshape(-1, 1),
+                 "W": np.einsum("qab,qbr->qar", gB + gB.transpose(0, 2, 1), kp["W"]), "v": np.diagonal(gB, axis1=1, axis2=2),
+                 "noise": gn / noise}
+            gu, o = np.zeros(nth), 0
+            for name, pr, shape in sites:
+                n = int(np.prod(shape))
+                uk, t = u[o:o + n], kp[name].reshape(-1)
+                dt = np.asarray(pr.dtheta_du(uk), dtype=np.float64)
+                val += float(np.sum(pr.log_prob(t)))
+                gu[o:o + n] = (g[name].reshape(-1) + pr.dlog_prob(t)) * dt
+                if jacobian:
+                    val += float(np.sum(pr.log_abs_jac(uk)))
+                    gu[o:o + n] += pr.dlog_abs_jac(uk)
+                o += n
+            if self.nn_prior:
+                lp, glp = _nn_log_prior(wmask, flat)
+                val += lp
+                gp = gp + glp
+            return val, np.concatenate([gu, gp])
+        return f, nth
+
+    # ---- predict
+    def _posterior_lcm(self, X_new, flat, kp, yres, noiseless, want, eps=None, jitter=1e-6):
+        """the LCM posterior on the embeddings of one weight set: flat [P], kp one draw's kernel_params, yres [rows]"""
+        Xtr, ttr, group = self._points(self.X_train)
+        Xn, tn, _ = self._points(X_new)
+        Ztr = self.ctx.mlp_forward(Xtr, self.widths, self.act, flat)[0]
+        Zn = self.ctx.mlp_forward(Xn, self.widths, self.act, flat)[0]
+        if group > 1:
+            Ztr, Zn = np.repeat(Ztr, group, axis=0), np.repeat(Zn, group, axis=0)
+        theta, B, noise = self._lcm(kp)
+        return self.ctx.posterior_multitask(self._fused, Ztr, ttr, np.asarray(yres, dtype=np.float64).reshape(-1), Zn, tn,
+                                            theta[None], B[None], noise[None], group, noiseless, jitter, want, eps)
+
+    def _channels(self, nn_params, k_params):
+        """[(flat, kernel_params, y)] per channel of y_train"""
+        flat = self.to_flat(nn_params)
+        y = np.asarray(self.y_train, dtype=np.float64)
+        if y.ndim == 1:
+            return [(flat, k_params, y)]
+        return [(flat[c], {k: np.asarray(v)[c] for k, v in k_params.items()}, y[c]) for c in range(y.shape[0])]
+
+    def _posterior_batched(self, X_new, params, batched, noiseless, want, eps=None, **kwargs):
+        """the seam of the acquisition functions: params = (nn_params, kernel_params) of one fit; one channel"""
+        nn_params, kp = params
+        (flat, kpc, y), = self._channels(nn_params, kp)
+        return self._posterior_lcm(X_new, flat, kpc, y, noiseless, want, eps, float(kwargs.get("jitter", 1e-6)))
+
+    def _posterior_grad(self, X_new, params, batched, noiseless, **kwargs):
+        raise NotImplementedError("multi-task models have no analytic posterior gradient; optimize_acq differences them")
+
+    def _kg_terms(self, X_new, params, noiseless, jitter):
+        """acquisition.kg's per-candidate terms of the rank-1 update (b2gp_kg_v) for one fit, multitask form.  With
+        bj = jitter sum_q B_q[t, t] (the data kernel's own jitter on k_pp's diagonal, which the cross-covariance with an
+        appended training row does not carry) and the noise term L (noise[t] + jitter) added once per latent:
+        diag_sub = bj + L (noise_p[t] + jitter) and noise_plus_jitter = bj + L (noise[t] + jitter), t the candidate's task.
+        The Kronecker form is refused: observing a point there observes all T tasks, a rank-T update (the reference's kg
+        appends one y per point and fails on the P*T outputs)."""
+        if self.shared_input:
+            raise NotImplementedError("KG is not supported in the Kronecker form (shared_input_space=True): observing a "
+                                      "point observes every task, which is not the rank-1 update KG evaluates")
+        _, kp = params
+        (_, kpc, _), = self._channels(params[0], kp)
+        _, t, _ = self._points(X_new)
+        _, B, noise = self._lcm(kpc)
+        L = B.shape[0]
+        bj = jitter * B[:, t, t].sum(0)
+        noise_p = noise * (0.0 if noiseless else 1.0)
+        return bj + L * (noise_p[t] + jitter), bj + L * (noise[t] + jitter)
+
+    def get_mvn_posterior(self, X_new, nn_params, k_params, noiseless: bool = False, y_residual=None,
+                          **kwargs) -> Tuple[np.ndarray, np.ndarray]:
+        """vi_mtdkl.py:211-247: mean [P'] and covariance [P', P'] for one set of network weights and kernel parameters
+        (P' = P, or P*T in the Kronecker form)"""
+        y = self.y_train if y_residual is None else y_residual
+        out = self._posterior_lcm(X_new, self.to_flat(nn_params), k_params, y, noiseless, ("mean", "cov"),
+                                  jitter=float(kwargs.get("jitter", 1e-6)))
+        return out["mean"][0], out["cov"][0]
+
+    def predict(self, rng_key, X_new, params=None, noiseless: bool = False, *args, **kwargs) -> Tuple[np.ndarray, np.ndarray]:
+        """vidkl.py:277-318 with the LCM posterior: (mean, var), [P'] or, for C channels, [C, P'] (one posterior per
+        channel)"""
+        nn_params, k_params = (self.nn_params, self.kernel_params) if params is None else params
+        X_new = self._set_data(X_new)
+        res = [self._posterior_lcm(X_new, f, kp, y, noiseless, ("mean", "var"), jitter=float(kwargs.get("jitter", 1e-6)))
+               for f, kp, y in self._channels(nn_params, k_params)]
+        mean, var = np.stack([r["mean"][0] for r in res]), np.stack([r["var"][0] for r in res])
+        if np.asarray(self.y_train).ndim == 2:
+            return mean, var
+        return mean[0], var[0]
+
+    def embed(self, X_new) -> np.ndarray:
+        """vidkl.py:371-384: z [N, d], or [C, N, d] with C channels.  The multitask form's task column is stripped first."""
+        flat = self.to_flat(self.nn_params)
+        Z = self.ctx.mlp_forward(self._points(X_new)[0], self.widths, self.act, np.atleast_2d(flat))
+        return Z if flat.ndim == 2 else Z[0]

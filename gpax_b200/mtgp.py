@@ -25,6 +25,27 @@ def _refuse_kernel(data_kernel):
         raise NotImplementedError("multi-task models take the data kernels 'RBF', 'Matern' and 'Periodic'")
 
 
+def lcm_task_matrix(W, v):
+    """B = W W^T + diag(v) (mtkernels.py:60-63) over any leading axes: W [..., T, R], v [..., T] -> B [..., T, T]"""
+    W, v = np.asarray(W, dtype=np.float64), np.asarray(v, dtype=np.float64)
+    return np.einsum("...tr,...ur->...tu", W, W) + v[..., None] * np.eye(W.shape[-2])
+
+
+def lcm_points(X, T: int, shared: bool):
+    """(data points [n, d], int32 task ids of the GP rows, group) of an input array.  The Kronecker form (shared) observes
+    every point once per task: n * T rows, point-major, task index fastest; the multitask form reads the task id from the
+    last column with astype(int) as the reference does, one row per point.  Task ids outside [0, T) raise ValueError (JAX
+    would clamp the gather into B silently)."""
+    X = np.asarray(X, dtype=np.float64)
+    X = X if X.ndim > 1 else X[:, None]
+    if shared:
+        return X, np.tile(np.arange(T, dtype=np.int32), X.shape[0]), T
+    t = X[:, -1].astype(int)
+    if t.size and (t.min() < 0 or t.max() >= T):
+        raise ValueError(f"task ids must lie in [0, {T}): got {t.min()} .. {t.max()}")
+    return np.ascontiguousarray(X[:, :-1]), t.astype(np.int32), 1
+
+
 class _LCMModel(ExactGP):
     """What MultiTaskGP and CoregGP share: parameter packing, task columns, the posterior and fit."""
 
@@ -46,18 +67,10 @@ class _LCMModel(ExactGP):
         return X.shape[1] if self.shared_input else X.shape[1] - 1
 
     def _rows(self, X):
-        """(data rows, int32 task ids, group) of an input array: the Kronecker form repeats each point once per task
-        (task index fastest); the multitask form reads the task id from the last column with astype(int) as the
-        reference does.  Task ids outside [0, T) raise ValueError (JAX would clamp the gather into B silently)."""
-        X = np.asarray(X, dtype=np.float64)
-        X = X if X.ndim > 1 else X[:, None]
-        T = self._num_tasks()
-        if self.shared_input:
-            return np.repeat(X, T, axis=0), np.tile(np.arange(T, dtype=np.int32), X.shape[0]), T
-        t = X[:, -1].astype(int)
-        if t.size and (t.min() < 0 or t.max() >= T):
-            raise ValueError(f"task ids must lie in [0, {T}): got {t.min()} .. {t.max()}")
-        return np.ascontiguousarray(X[:, :-1]), t.astype(np.int32), 1
+        """(data rows, int32 task ids, group) of an input array (lcm_points, each point repeated once per task in the
+        Kronecker form)"""
+        pts, t, group = lcm_points(X, self._num_tasks(), self.shared_input)
+        return (np.repeat(pts, group, axis=0) if group > 1 else pts), t, group
 
     def _out_len(self, X_new):
         X_new = self._set_data(X_new)
@@ -85,7 +98,7 @@ class _LCMModel(ExactGP):
         theta = np.empty((S, L, d + 2))
         theta[:, :, :d] = ell
         theta[:, :, d], theta[:, :, d + 1] = sc, per
-        B = np.einsum("sltr,slur->sltu", W, W) + v[..., None] * np.eye(T)
+        B = lcm_task_matrix(W, v)
         noise = np.broadcast_to(np.asarray(params["noise"], dtype=np.float64).reshape(S, -1), (S, T)).copy()
         return theta, B, noise
 

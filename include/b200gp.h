@@ -306,6 +306,23 @@ int  b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D
                   const double* theta, double jitter, unsigned flags,
                   double* value, double* grad_theta, double* grad_params, double* grad_z, int* info);
 
+/* The multi-task counterpart (the likelihood of viMTDKL.model, gpax/models/vi_mtdkl.py): log N(yres; 0, K) with K the
+ * LCM covariance of b2gp_mll_multitask on the embedding z = MLP(X), expanded to the GP rows:
+ *   X[N, D]                 the network's inputs, N points, without the task column
+ *   task[N*group], yres[N*group]  the GP rows, point-major: point p is rows p*group .. p*group+group-1 (group = 1: the
+ *                           multitask form, one row per point; group = T: the Kronecker form, task index fastest)
+ *   theta[L,d+2], B[L,T,T], noise[T], group, T, L   as b2gp_mll_multitask (RBF and Matern; d = z_dim)
+ * HOST outputs: value, grad_theta, grad_B, grad_noise as b2gp_mll_multitask on the expanded z (same kernels, same
+ * bits); grad_z[N, d] (optional) d value / dz, each point's rows summed in task order (with n_layers = 0 this is
+ * d value / dX); grad_params (optional) in the params layout.  X and yres follow `flags` (B2GP_FLAG_DEVICE_PTRS allowed,
+ * B2GP_FLAG_F32 refused); task, theta, B, noise, widths and params are HOST pointers.  Task ids are checked before any
+ * launch.  NaN outputs where info != 0.  The reductions run in a fixed order: identical calls give identical bits.   */
+int  b2gp_mtdkl_mll(b2gp_ctx* ctx, int kind, const double* X, const int* task, int64_t N, int64_t D, const double* yres,
+                    int group, int T, int L, int n_layers, const int64_t* widths, int act, const double* params,
+                    const double* theta, const double* B, const double* noise, double jitter,
+                    unsigned flags, double* value, double* grad_theta, double* grad_B, double* grad_noise,
+                    double* grad_params, double* grad_z, int* info);
+
 /* Samples of S multivariate normals: y[s,i,:] = mean[s,:] + chol(cov[s]) eps[s,i,:], i < n -- replaces
  * numpyro.distributions.MultivariateNormal(mean, cov).sample (gpax/models/gp.py:292, gpax/acquisition/base_acq.py:221)
  * where the caller changed cov after the posterior call (gpax/models/hskgp.py:201-204 adds the predicted noise variance).
@@ -333,6 +350,10 @@ int  b2gp_acq_samples(b2gp_ctx* ctx, int kind, const double* y, int64_t R, int64
  * noise_plus_jitter = the diagonal term of the appended training point.  out[P].                                 */
 int  b2gp_kg(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n,
              double diag_sub, double noise_plus_jitter, int maximize, double* out, unsigned flags);
+/* Same with a value per candidate: diag_sub[P], noise_plus_jitter[P] (follow `flags` as the other arrays).  The LCM
+ * models (viMTDKL) carry a noise per task, so both terms depend on the candidate's task.                         */
+int  b2gp_kg_v(b2gp_ctx* ctx, const double* mean, const double* cov, int64_t P, const double* ysim, int64_t n,
+               const double* diag_sub, const double* noise_plus_jitter, int maximize, double* out, unsigned flags);
 
 /* ---- multi-GPU building blocks (SURVEY.md section 8e).  One process per GPU; the exchange steps
  * (panel broadcast, M x M all-reduce) are issued by the host side over NCCL on these same device
