@@ -17,7 +17,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libb200gp.so")
 KERNEL_RBF, KERNEL_MATERN52, KERNEL_PERIODIC = 0, 1, 2
 KERNEL_NNGP_ERF, KERNEL_NNGP_RELU = 3, 4
 ACT_RELU, ACT_TANH = 0, 1
-KIND = {"RBF": KERNEL_RBF, "Matern": KERNEL_MATERN52, "Periodic": KERNEL_PERIODIC}
+KIND = {"RBF": KERNEL_RBF, "Matern": KERNEL_MATERN52, "Periodic": KERNEL_PERIODIC,
+        "NNGP_erf": KERNEL_NNGP_ERF, "NNGP_relu": KERNEL_NNGP_RELU}
 
 FLAG_DEVICE_PTRS = 1 << 0
 FLAG_LOWER_ONLY = 1 << 1
@@ -248,7 +249,7 @@ class Context:
 
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
-             "potrf_tall_fp64")
+             "potrf_tall_fp64", "mll_nngp_grad")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""

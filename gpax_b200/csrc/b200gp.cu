@@ -19,6 +19,7 @@
 #include "acq.cuh"
 #include "dist.cuh"
 #include "dkl.cuh"
+#include "nngp.cuh"
 
 // ------------------------------------------------------------------------------------------ helpers
 static inline bool dev_ptrs(unsigned flags) { return (flags & B2GP_FLAG_DEVICE_PTRS) != 0; }
@@ -605,7 +606,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                           double* y_sampled, int* info, b2gp_timing* timing, double* dmean_out = nullptr, double* dvar_out = nullptr,
                           const MtDesc* mt = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
-    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+    ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
+    const bool nngp = is_nngp(kind);   // NNGP: no multi-task form, no test-input gradient
+    ARG_CHECK(ctx, !nngp || (!mt && !(flags & (B2GP_OUT_DMEAN | B2GP_OUT_DVAR))));
     ARG_CHECK(ctx, xtr_stride == 0 || xtr_stride >= N * d);
     ARG_CHECK(ctx, xnew_stride == 0 || xnew_stride >= P * d);
     ARG_CHECK(ctx, nv_stride == 0 || nv_stride >= N);
@@ -625,6 +628,14 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     ARG_CHECK(ctx, !want_samp || (eps && y_sampled && n_samp >= 1));
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     const bool dev = dev_ptrs(flags), f32 = f32_io(flags);
+    if (nngp) {   // every draw's depth, before any work is queued
+        std::vector<double> hth((size_t)S * (d + 3));
+        if (dev)
+            CUDA_TRY(ctx, cudaMemcpy(hth.data(), theta, hth.size() * 8, cudaMemcpyDeviceToHost));
+        else
+            memcpy(hth.data(), theta, hth.size() * 8);
+        for (int64_t s = 0; s < S; ++s) RET_IF(nngp_check_depth(ctx, "b2gp_posterior", hth[(size_t)s * (d + 3)]));
+    }
     const int nslots = (int)(S < ctx->n_streams ? S : ctx->n_streams);
     cudaStream_t st0 = ctx->slots[0].stream;
     CallTimer tm(ctx);
@@ -642,6 +653,13 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     if (noise_vec) RET_IF(stage_in_t(ctx, st0, ctx->d_in[6], ctx->f32_in[6], noise_vec, (size_t)(nv_stride ? S * nv_stride : N), dev, f32, &dnv));
     RET_IF(stage_in(ctx, st0, ctx->d_in[3], theta, (size_t)S * nth * 8, dev, &dtheta));
     if (want_samp) RET_IF(stage_in_t(ctx, st0, ctx->d_in[4], ctx->f32_in[4], eps, (size_t)S * n_samp * P, dev, f32, &deps));
+    // NNGP: d+3 zeros, the theta of the zero prior the variance epilogue starts from
+    const double* dzero = nullptr;
+    std::vector<double> hzero;
+    if (nngp) {
+        hzero.assign((size_t)d + 3, 0.0);
+        RET_IF(stage_in(ctx, st0, ctx->d_in[5], hzero.data(), hzero.size() * 8, false, &dzero));
+    }
     // multi-task: [B (S*L*T*T) | noise (S*T) | d+3 zeros] and the task ids [task_tr (N) | task_new (P)]
     const double* dmt = nullptr;
     const int* dtask = nullptr;
@@ -717,7 +735,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
         if (need_cov) RET_IF(ensure(ctx, sl.cov, (size_t)P * ldC * 8));
         if (want_samp) RET_IF(ensure(ctx, sl.LinvC, (size_t)linv_bytes(P)));
-        if (!want_mean || (mt && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)(mt ? 2 * P : P) * 8));
+        if (!want_mean || ((mt || nngp) && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)((mt || nngp) ? 2 * P : P) * 8));
     }
     // inputs and the memset of dinfo were queued on st0: order the other streams behind them
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
@@ -776,8 +794,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             for (int e = 0; e < 6; ++e) sev[s].e[e] = ctx->pool.get();
             CUDA_TRY(ctx, cudaEventRecord(sev[s].e[0], st));
         }
-        // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7
-        sl.oz_planes = (htheta.empty() || noise_vec || mt) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
+        // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7.
+        // The bound takes k(x, x) = k_scale, which an NNGP kernel does not satisfy: 7 there.
+        sl.oz_planes = (htheta.empty() || noise_vec || mt || nngp) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
         const int T = mt ? mt->T : 0, L = mt ? mt->L : 0, grp = mt ? mt->group : 0;
         const double* Bs = mt ? dmt + s * L * T * T : nullptr;
         const double* ns = mt ? dmt + (size_t)S * L * T * T + s * T : nullptr;
@@ -833,6 +852,16 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                 double* prior = (double*)sl.misc.p + P;
                 RET_IF(launch_gram_lcm(ctx, st, LCM_DIAG, kind, dXnew_s, dtn, P, nullptr, nullptr, 0, d, T, L, grp, th, Bs, ns, noise_mult_new,
                                        jitter, prior, 1));
+                RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, add_vec_kernel, dvar + s * P, (const double*)prior, P));
+            }
+        } else if (nngp) {   // as the multi-task branch, with the NNGP prior diagonal k(x_p, x_p) + noise_p + jitter
+            if (want_mean || want_var || want_samp)
+                RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, (int)B2GP_KERNEL_PERIODIC, d, dzero, 0.0, 0.0,
+                              inf, mean_s, want_var ? dvar + s * P : nullptr));
+            if (want_var) {
+                double* prior = (double*)sl.misc.p + P;
+                RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, nngp_diag_kernel, dXnew_s, P, d, kind, th, noise_mult_new,
+                              jitter, prior));
                 RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, add_vec_kernel, dvar + s * P, (const double*)prior, P));
             }
         } else if (want_mean || want_var || want_samp) {
@@ -985,6 +1014,7 @@ extern "C" int b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, i
     if (flags & (B2GP_FLAG_F32 | B2GP_OUT_COV | B2GP_OUT_SAMPLE))
         return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_posterior_grad", "fp64 arrays, outputs mean / var / dmean / dvar only",
                        __FILE__, __LINE__);
+    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
                           var, nullptr, nullptr, 0, nullptr, info, timing, dmean, dvar);
 }
@@ -1376,9 +1406,14 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, !grad_noise_vec || grad);
     ARG_CHECK(ctx, !grad_x_dev || (grad && !noise_vec && (!mt || kind != B2GP_KERNEL_PERIODIC)));
-    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+    ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
+    // NNGP: single task, no input gradient; no per-feature accumulator, so the Gram build's d <= 64 is the limit
+    const bool nngp = is_nngp(kind);
+    ARG_CHECK(ctx, !nngp || (!mt && !grad_x_dev));
     ARG_CHECK(ctx, X && yres && theta && value && info);
-    ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= MLL_MAX_D);
+    ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= (nngp ? GRAM_MAX_D : MLL_MAX_D));
+    if (nngp) RET_IF(nngp_check_depth(ctx, "b2gp_mll", theta[0]));
+    const int depth = nngp ? (int)theta[0] : 0;
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     ctx->fcache.valid = false;
     const bool dev = dev_ptrs(flags);
@@ -1414,6 +1449,8 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     RET_IF(ensure(ctx, ctx->d_info, 64));
     if (mt)
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + L * tiles * tiles * nout + L * nout) * 8));
+    else if (nngp)   // partials [tiles^2, 3] | self-chains [N, depth, 3]
+        RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * 3 + N * depth * 3) * 8));
     else
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * nth) * 8));
     int* dinfo = (int*)ctx->d_info.p;
@@ -1460,6 +1497,20 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                 if (grad_x_dev)   // d value / d X [N, d] of the LCM covariance on the device (dkl.cuh)
                     RET_IF(launch(ctx, st, (unsigned)ceil_div(N, DZ_ROWS), DZ_THREADS, 0, mll_lcm_dz_kernel, kind, dX, dtask, N, d, T, L,
                                   dth, (const double*)dmt, (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
+            } else if (nngp) {   // nngp.cuh: self-chains, the cross chain per pair, fixed-order sums -> sc[8..11) = (var_w, noise, var_b)
+                double* chain = partial + tiles * tiles * 3;
+                if (depth > 0) RET_IF(launch(ctx, st, (unsigned)ceil_div(N, (int64_t)256), 256, 0, nngp_self_kernel, dX, N, d, kind, dth, chain));
+                static PerDeviceOnce attr;
+                if (attr.need(ctx->device)) {
+                    CUDA_TRY(ctx, cudaFuncSetAttribute(mll_nngp_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)nngp_grad_smem(GRAM_MAX_D, NNGP_MAX_DEPTH)));
+                    attr.done(ctx->device);
+                }
+                count_path(ctx, (int)PATH_MLL_NNGP_GRAD);
+                RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), NNGP_THREADS, nngp_grad_smem(d, depth),
+                              mll_nngp_grad_kernel, dX, N, d, kind, dth, (const double*)chain, (const double*)alpha, (const double*)Kinv, ld,
+                              partial));
+                RET_IF(launch(ctx, st, 3u, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, tiles * tiles, 3, sc + 8));
             } else {
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv,
                               ld, partial));
@@ -1493,8 +1544,12 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
         for (int t = 0; t < T; ++t) grad[L * nth1 + L * T * T + t] = colsum[nth1 + T * T + t];
     }
     *value = -0.5 * hsc[1] - hsc[0] - 0.5 * (double)N * 1.8378770664093453;  // log(2 pi)
-    if (grad && !mt)
+    if (grad && nngp) {   // [0, d) depth slots: 0; d: log var_w; d+1: log noise; d+2: log var_b
+        for (int k = 0; k < d; ++k) grad[k] = 0.0;
+        for (int k = 0; k < 3; ++k) grad[d + k] = hsc[8 + k];
+    } else if (grad && !mt) {
         for (int k = 0; k < nth; ++k) grad[k] = hsc[8 + k];
+    }
     if (*info != 0) {
         *value = NAN;
         if (grad)

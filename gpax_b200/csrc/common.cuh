@@ -109,6 +109,7 @@ enum PathCounter {
     PATH_TRSM_TALL,     // trsm_tall calls
     PATH_POTRF_TALL,    // factorisations that took potrf_tall on the int8 route (top-level entries, not its recursion)
     PATH_POTRF_TALL_FP64,  // factorisations that took potrf_tall on the fp64 DMMA route (ozaki = 0), top-level entries
+    PATH_MLL_NNGP_GRAD,    // likelihood gradients that took the NNGP route (mll_nngp_grad_kernel, nngp.cuh), one per call
     PATH_COUNT
 };
 

@@ -142,6 +142,10 @@ class ExactGP:
         return np.float32 if np.asarray(X_new).dtype == np.float32 else np.float64
 
     # ------------------------------------------------------------------ the posterior seam
+    def _theta(self, params, d, batched):
+        """the posterior's theta rows [S, d+3] from a parameter dict (the NNGP models pack theirs differently)"""
+        return _theta_rows(params, d, batched)
+
     def _f32_io(self, X_new):
         """the reference's default precision: float32 training data and test inputs go over the C-ABI as float32 and the
         results come back float32 (B2GP_FLAG_F32; gpax/utils/utils.py:19-21) -- no host-side casts of the big arrays"""
@@ -152,14 +156,14 @@ class ExactGP:
         if self._fused is not None and self._f32_io(X_new):
             X = np.asarray(self.X_train)
             X = X if X.ndim > 1 else X[:, None]
-            theta = _theta_rows(params, X.shape[1], batched)
+            theta = self._theta(params, X.shape[1], batched)
             return self.ctx.posterior(self._fused, X, np.asarray(self.y_train).reshape(-1), self._set_data(X_new), theta, noiseless,
                                       float(kwargs.get("jitter", 1e-6)), want, eps, f32=True)
         X, y = self._train_arrays()
         Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
         d = X.shape[1]
         jitter = float(kwargs.get("jitter", 1e-6))
-        theta = _theta_rows(params, d, batched)
+        theta = self._theta(params, d, batched)
         S = theta.shape[0]
         yres = self._residuals(X, y, params, batched, S)
         if self._fused is None:

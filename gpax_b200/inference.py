@@ -17,6 +17,11 @@ from . import priors as P
 from .utils import seed_from_key
 
 
+def _is_nngp(kind):
+    """the fused NNGP kernels (iBNN / vi_iBNN): theta = (depth [d], var_w, noise, var_b)"""
+    return kind in ("NNGP_erf", "NNGP_relu")
+
+
 class LogJoint:
     """log p(y, theta) over the unconstrained vector u, with gradient; theta = (k_length[d], k_scale, noise[, period]).
     Default priors and `*_prior_dist` objects only; `make_log_joint` picks ProgramLogJoint when the model carries prior
@@ -92,11 +97,48 @@ class LogJoint:
         return out
 
 
+class NNGPLogJoint(LogJoint):
+    """LogJoint of iBNN / vi_iBNN with their default priors (ibnn.py:54-61, vi_ibnn.py:53-60): sites var_b, var_w, noise
+    in the reference's order; theta = (depth [d], var_w, noise, var_b).  The depth slots are constants: no site, no
+    gradient, and nothing is divided by them."""
+
+    def __init__(self, model, jitter=1e-6):
+        if model.kernel_prior is not None or model.noise_prior is not None or \
+                (model.mean_fn is not None and model.mean_fn_prior is not None):
+            raise NotImplementedError("prior programs go through ProgramLogJoint (inference.make_log_joint)")
+        self.m, self.jitter = model, float(jitter)
+        X, y = model._train_arrays()
+        self.X, self.d = X, X.shape[1]
+        self.y = y if model.mean_fn is None else y - np.asarray(model.mean_fn(X), dtype=np.float64).squeeze()
+        self.kind = model._fused
+        d = self.d
+        pb, pw = model._nngp_site_priors()
+        self.names = ["var_b", "var_w", "noise"]
+        self.priors = [pb, pw, model.noise_prior_dist or P.LogNormal(0.0, 1.0)]     # gp.py:222-227
+        self.idx = [d + 2, d, d + 1]
+        for pr in self.priors:
+            if not isinstance(pr, P.Prior):
+                raise TypeError("priors must be gpax_b200.priors objects (numpyro distributions cannot be used here)")
+        self.dim = 3
+        self.n_evals = 0
+
+    def theta_of(self, u):
+        th = super().theta_of(u)
+        th[:self.d] = self.m.depth
+        return th
+
+    def to_dict(self, U):
+        th = np.stack([self.theta_of(u) for u in np.atleast_2d(U)])
+        return {"var_b": th[:, self.d + 2], "var_w": th[:, self.d], "noise": th[:, self.d + 1]}
+
+
 def gp_model_program(m, d, kind):
     """the host side of ExactGP.model (gp.py:137-154): every statement except the likelihood.  Runs under
     priors.run_program; returns (kernel-parameter dict, noise, mean-function parameter dict or None)."""
     if m.kernel_prior is not None:
         kp = m.kernel_prior()
+    elif _is_nngp(getattr(m, "_fused", None)):                         # ibnn.py:54-61, vi_ibnn.py:53-60
+        kp = m._sample_kernel_params()
     else:                                                              # gp.py:229-247
         lp = m.lengthscale_prior_dist or P.LogNormal(0.0, 1.0)
         with P.plate("ard", d):
@@ -169,6 +211,9 @@ class ProgramLogJoint:
             o += s.size
         (kp, noise, mp), sites, _ = P.run_program(self._model_program, vals)
         th = np.ones(self.d + 3)
+        if _is_nngp(self.kind):
+            th[:] = self.m._theta(dict(kp, noise=noise), self.d, False)[0]
+            return th, self._mean(mp), sites
         th[:self.d] = np.broadcast_to(np.asarray(kp["k_length"], dtype=np.float64).reshape(-1), (self.d,)) \
             if np.size(kp["k_length"]) in (1, self.d) else np.nan
         th[self.d] = float(np.asarray(kp["k_scale"]).reshape(-1)[0])
@@ -177,12 +222,13 @@ class ProgramLogJoint:
             if kp.get("period") is None:
                 raise ValueError("the Periodic kernel needs 'period' in the dict kernel_prior returns")
             th[self.d + 2] = float(np.asarray(kp["period"]).reshape(-1)[0])
-        mean = None
+        return th, self._mean(mp), sites
+
+    def _mean(self, mp):
+        """the mean-function vector at X for the mean-function parameters mp, or None"""
         if self.has_mean_params:
-            mean = np.asarray(self.m.mean_fn(self.X, mp), dtype=np.float64).squeeze()
-        elif self.fixed_mean is not None:
-            mean = self.fixed_mean
-        return th, mean, sites
+            return np.asarray(self.m.mean_fn(self.X, mp), dtype=np.float64).squeeze()
+        return self.fixed_mean
 
     def init_u(self):
         """init_to_median (gp.py:208)"""
@@ -213,10 +259,16 @@ class ProgramLogJoint:
         return val, g, alpha, info
 
     def _valid(self, th):
+        if _is_nngp(self.kind):     # the depth slots may be 0; var_w, noise and var_b must be positive
+            return np.all(np.isfinite(th)) and np.all(th[self.d:] > 0)
         return np.all(np.isfinite(th)) and np.all(th[:self.d + 2] > 0)
 
     def _dval_dth(self, th, g):
         """d value / d theta from the likelihood's gradient g, which is d/dlog(theta); unused entries carry g = 0"""
+        if _is_nngp(self.kind):     # the depth slots are constants (their g is 0, and the depth may be 0)
+            out = np.zeros_like(th)
+            out[self.d:] = g[self.d:] / th[self.d:]
+            return out
         return g / th
 
     def __call__(self, u, jacobian):
@@ -373,6 +425,8 @@ def make_log_joint(model, jitter=1e-6):
     if model.kernel_prior is not None or model.noise_prior is not None or \
             (model.mean_fn is not None and model.mean_fn_prior is not None):
         return ProgramLogJoint(model, jitter)
+    if _is_nngp(model._fused):
+        return NNGPLogJoint(model, jitter)
     return LogJoint(model, jitter)
 
 

@@ -37,9 +37,11 @@ typedef struct b2gp_ctx b2gp_ctx;
 /* kernel families: gpax/kernels/kernels.py:44-65 (RBF), 68-91 (Matern-5/2), 94-117 (Periodic);
  * name table gpax/kernels/kernels.py:227-241 */
 enum { B2GP_KERNEL_RBF = 0, B2GP_KERNEL_MATERN52 = 1, B2GP_KERNEL_PERIODIC = 2,
-       /* b2gp_gram only -- NNGP kernels, gpax/kernels/kernels.py:120-224 (erf / ReLU activation): `scale` carries var_w,
-        * `period` carries var_b, lengthscale[0] carries the depth; non-stationary, so the posterior entry points (which
-        * need k(x, x) in closed form) do not take them -- the shell routes them through its callable-kernel path */
+       /* NNGP kernels, gpax/kernels/kernels.py:120-224 (erf / ReLU activation): `scale` carries var_w, `period` carries
+        * var_b, lengthscale[0] carries the depth.  Taken by b2gp_gram, b2gp_gram_multitask, b2gp_posterior,
+        * b2gp_posterior_batch, b2gp_mll and b2gp_mll_v; theta[d+3] = (depth, unused [1, d), var_w, noise, var_b) and the
+        * likelihood's grad[d+3] = (0 [0, d), d/dlog var_w, d/dlog noise, d/dlog var_b).  On the posterior and likelihood
+        * entry points the depth is an integer in [0, 16] and 1 <= d <= 64.  Every other entry point refuses them. */
        B2GP_KERNEL_NNGP_ERF = 3, B2GP_KERNEL_NNGP_RELU = 4 };
 
 enum {
