@@ -31,6 +31,15 @@ class B200GPError(RuntimeError):
     pass
 
 
+def _mlp_nparams(D, widths):
+    """entries of the flat parameter layout of a network with input width D and layer widths `widths`"""
+    n, i = 0, int(D)
+    for w in widths:
+        n += i * int(w) + int(w)
+        i = int(w)
+    return n
+
+
 class Timing(C.Structure):
     _fields_ = [("total_ms", C.c_double), ("gram_ms", C.c_double), ("potrf_ms", C.c_double),
                 ("trsm_ms", C.c_double), ("epilogue_ms", C.c_double), ("h2d_ms", C.c_double),
@@ -92,6 +101,10 @@ SIGNATURES = {
                                _dp, _vp, _vp, _vp, _ip]),
     "b2gp_mtdkl_mll": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int,
                                  _vp, _vp, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _vp, _ip]),
+    "b2gp_bnn_loglik": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_double, C.c_uint,
+                                  _dp, _dp, _vp]),
+    "b2gp_bnn_predict": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
+                                   _vp, C.c_int64, _vp, _vp, C.c_uint]),
     "b2gp_sparse_elbo": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp,
                                    _vp, _ip]),
     "b2gp_dist_unique_id": (C.c_int, [_vp]),
@@ -573,6 +586,53 @@ class Context:
                                             _ptr(theta), _ptr(B), _ptr(noise), float(jitter), flags, C.byref(val), _ptr(gt),
                                             _ptr(gB), _ptr(gn), _ptr(gp), _ptr(gz), C.byref(info)))
         return val.value, gt, gB, gn, gp, gz, info.value
+
+    def bnn_loglik(self, X, y, widths, act, params, sigma, want_params=True):
+        """sum log N(y; MLP(X), sigma) and its gradients (b2gp_bnn_loglik).  X [N, D] and y [N, O]: both host arrays or both
+        DeviceArrays; widths [L] with widths[-1] = O; params [P] flat layout.  Returns (value, d/dsigma, grad_params [P] or
+        None)."""
+        X, Xp, flags = self._arg(X)
+        y, yp, yflags = self._arg(y)
+        if flags != yflags:
+            raise ValueError("X and y must both be host arrays or both DeviceArrays")
+        N, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        p = _f64(params).reshape(-1)
+        if p.size != _mlp_nparams(D, w):
+            raise ValueError(f"params has {p.size} entries, the network D={D}, widths={w.tolist()} has {_mlp_nparams(D, w)}")
+        if tuple(y.shape) != (N, int(w[-1])):
+            raise ValueError(f"y has shape {tuple(y.shape)}, the network needs ({N}, {int(w[-1])})")
+        val, gs = C.c_double(0.0), C.c_double(0.0)
+        gp = np.zeros(p.size) if want_params else None
+        self._check(self.lib.b2gp_bnn_loglik(self.h, Xp, N, D, yp, int(w[-1]), int(w.size), _ptr(w), int(act), _ptr(p),
+                                             float(sigma), flags, C.byref(val), C.byref(gs), _ptr(gp)))
+        return val.value, gs.value, gp
+
+    def bnn_predict(self, X, widths, act, params, sigma=None, eps=None):
+        """loc [S, P, O] = MLP(X) for S weight sets and, given eps [S, n, P, O] and sigma [S], y_sampled [S, P, O] =
+        loc + sigma * mean_k eps (b2gp_bnn_predict).  X [P, D]: a host array or a DeviceArray; params [S, P] or [P].
+        Returns (loc, y_sampled or None)."""
+        X, Xp, flags = self._arg(X)
+        Pn, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        p = _f64(params)
+        p = p.reshape(1, -1) if p.ndim == 1 else p
+        S, O = p.shape[0], int(w[-1])
+        if p.shape[1] != _mlp_nparams(D, w):
+            raise ValueError(f"params rows have {p.shape[1]} entries, the network D={D}, widths={w.tolist()} has "
+                             f"{_mlp_nparams(D, w)}")
+        loc = np.empty((S, Pn, O))
+        ys, n, sg = None, 0, None
+        if eps is not None:
+            eps = _f64(eps)
+            if eps.ndim != 4 or eps.shape[0] != S or eps.shape[2:] != (Pn, O):
+                raise ValueError(f"eps has shape {eps.shape}, expected ({S}, n, {Pn}, {O})")
+            n = eps.shape[1]
+            sg = _f64(np.broadcast_to(np.asarray(sigma, dtype=np.float64).reshape(-1), (S,)))
+            ys = np.empty((S, Pn, O))
+        self._check(self.lib.b2gp_bnn_predict(self.h, Xp, Pn, D, int(w.size), _ptr(w), int(act), _ptr(p), S, p.shape[1], O,
+                                              _ptr(sg), _ptr(eps), n, _ptr(loc), _ptr(ys), flags))
+        return loc, ys
 
     @staticmethod
     def _arg(a):

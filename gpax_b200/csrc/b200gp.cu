@@ -20,6 +20,7 @@
 #include "dist.cuh"
 #include "dkl.cuh"
 #include "nngp.cuh"
+#include "bnn.cuh"
 
 // ------------------------------------------------------------------------------------------ helpers
 static inline bool dev_ptrs(unsigned flags) { return (flags & B2GP_FLAG_DEVICE_PTRS) != 0; }
@@ -78,6 +79,7 @@ extern "C" int b2gp_ctx_create(int device, b2gp_ctx** out) {
     ctx->cc_major = prop.major;
     ctx->cc_minor = prop.minor;
     ctx->mem_bytes = prop.totalGlobalMem;
+    ctx->smem_optin = prop.sharedMemPerBlockOptin;
     for (int i = 0; i < B2GP_MAX_STREAMS; ++i) {
         if (cudaStreamCreateWithFlags(&ctx->slots[i].stream, cudaStreamNonBlocking) != cudaSuccess) return B2GP_ERR_CUDA;
         for (int e = 0; e < 8; ++e) cudaEventCreate(&ctx->slots[i].ev[e]);
@@ -162,6 +164,11 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
         ctx->tall_min_fp64 = (int)value;
         return B2GP_OK;
     }
+    if (strcmp(key, "bnn_fused") == 0) {   // tests and timing only: 0 puts b2gp_bnn_* on the layered route
+        ARG_CHECK(ctx, value == 0 || value == 1);
+        ctx->bnn_fused = (int)value;
+        return B2GP_OK;
+    }
     if (strcmp(key, "oz_debug") == 0) {   // timing experiments only: != 0 skips the C read-modify-write
         ARG_CHECK(ctx, value >= 0 && value <= 2);
         ctx->oz_debug = (int)value;
@@ -187,7 +194,7 @@ extern "C" int b2gp_get_option(b2gp_ctx* ctx, const char* key, int64_t* value) {
     } tab[] = {{"streams", ctx->n_streams},       {"ozaki", ctx->ozaki},         {"trsm_strip", ctx->trsm_strip},
                {"oz_cluster", ctx->oz_cluster},   {"enqueue_threads", ctx->enqueue_threads}, {"big_grid", ctx->big_grid},
                {"oz_min_tiles", ctx->oz_min_tiles}, {"panel", ctx->panel},       {"tall_min", ctx->tall_min},
-               {"tall_min_fp64", ctx->tall_min_fp64},
+               {"tall_min_fp64", ctx->tall_min_fp64}, {"bnn_fused", ctx->bnn_fused},
                {"oz_debug", ctx->oz_debug},       {"tma", ctx->use_tma}};
     for (const auto& e : tab)
         if (strcmp(key, e.key) == 0) {
@@ -1851,6 +1858,125 @@ extern "C" int b2gp_mtdkl_mll(b2gp_ctx* ctx, int kind, const double* X, const in
     if (grad_z && *info == 0) CUDA_TRY(ctx, cudaMemcpyAsync(grad_z, gz, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
     if (back && *info == 0) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, gz, grad_params));
     return tm.end(ctx, st);
+}
+
+// ------------------------------------------------------------------------------------------ Bayesian MLP (bnn.cuh)
+static int bnn_optin(b2gp_ctx* ctx) {
+    static PerDeviceOnce attr;
+    if (attr.need(ctx->device)) {
+        CUDA_TRY(ctx, cudaFuncSetAttribute(bnn_loglik_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)(ctx->smem_optin - 8 * BNN_THREADS)));
+        CUDA_TRY(ctx, cudaFuncSetAttribute(bnn_predict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin));
+        attr.done(ctx->device);
+    }
+    return B2GP_OK;
+}
+
+// BNN's likelihood sum_{i,o} log N(y_io; z_io, sigma): two launches on the fused route, the DKL forward / backward pass
+// around bnn_resid_kernel on the layered one.  Both leave sum r^2 in the slot after the parameter gradient.
+extern "C" int b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                               const int64_t* widths, int act, const double* params, double sigma, unsigned flags, double* value,
+                               double* grad_sigma, double* grad_params) {
+    if (!ctx) return B2GP_ERR_ARG;
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, X && y && params && value && grad_sigma && n_layers >= 1 && s.d == O && !f32_io(flags));
+    ARG_CHECK(ctx, sigma > 0.0 && std::isfinite(sigma));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    CallTimer tm(ctx);
+    RET_IF(tm.begin(st));
+    const bool dev = dev_ptrs(flags);
+    const double *dX, *dy, *dP;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev, &dX));
+    RET_IF(stage_in(ctx, st, ctx->d_in[1], y, (size_t)N * O * 8, dev, &dy));
+    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)s.nparams * 8, false, &dP));
+    const double inv_s2 = 1.0 / (sigma * sigma);
+    const size_t smem = ctx->bnn_fused ? bnn_fused_smem(D, n_layers, widths, true, ctx->smem_optin) : 0;
+    const double* sums;   // [grad params | sum r^2] on the device
+    if (smem) {
+        RET_IF(bnn_optin(ctx));
+        int per_sm = 0;
+        CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bnn_loglik_tile_kernel, BNN_THREADS, smem));
+        const int64_t nblk = std::min<int64_t>(ceil_div(N, BNN_ROWS), (int64_t)ctx->sm_count * std::max(per_sm, 1));
+        const int64_t ld = s.nparams + 1;
+        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(nblk + 1) * ld * 8));
+        double* partial = (double*)ctx->mlp[3].p;
+        double* out = partial + nblk * ld;
+        RET_IF(launch(ctx, st, (unsigned)nblk, BNN_THREADS, smem, bnn_loglik_tile_kernel, bnn_net(D, n_layers, widths), act, dX, dy,
+                      N, dP, inv_s2, partial));
+        RET_IF(launch(ctx, st, (unsigned)ceil_div(ld, 256), 256, 0, bnn_reduce_kernel, (const double*)partial, (int)nblk, (int)ld, out));
+        if (grad_params) CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, out, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
+        sums = out;
+    } else {
+        std::vector<double*> H;
+        RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP, H));
+        const MlpBack b = mlp_back_layout(s);
+        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(b.tot + 1) * 8));
+        double* base = (double*)ctx->mlp[3].p;
+        double* r2 = base + b.tot;
+        RET_IF(launch(ctx, st, 1, BNN_THREADS, 0, bnn_resid_kernel, (const double*)H[s.L], dy, N * O, inv_s2, base, r2));
+        if (grad_params) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, base, grad_params));
+        sums = r2;
+    }
+    double r2sum = 0.0;
+    CUDA_TRY(ctx, cudaMemcpyAsync(&r2sum, sums + (smem ? s.nparams : 0), 8, cudaMemcpyDeviceToHost, st));
+    RET_IF(tm.end(st, nullptr));
+    const double no = (double)N * (double)O;
+    *value = -0.5 * r2sum * inv_s2 - no * (log(sigma) + 0.5 * log(2.0 * 3.141592653589793));
+    *grad_sigma = r2sum * inv_s2 / sigma - no / sigma;
+    return B2GP_OK;
+}
+
+// loc[s] = MLP(X; weight set s) and y_sampled[s] = loc[s] + sigma[s] * mean_k eps[s, k] for S weight sets: one launch on
+// the fused route, the DKL forward pass and bnn_sample_kernel per draw on the layered one; one copy back either way.
+extern "C" int b2gp_bnn_predict(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int n_layers, const int64_t* widths, int act,
+                                const double* params, int64_t S, int64_t params_stride, int64_t O, const double* sigma,
+                                const double* eps, int64_t n, double* loc, double* y_sampled, unsigned flags) {
+    if (!ctx) return B2GP_ERR_ARG;
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, P, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, X && params && loc && n_layers >= 1 && s.d == O && S >= 1 && params_stride >= s.nparams);
+    ARG_CHECK(ctx, !eps || (sigma && y_sampled && n >= 1 && n <= (1 << 30)));
+    ARG_CHECK(ctx, !f32_io(flags));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    CallTimer tm(ctx);
+    RET_IF(tm.begin(st));
+    const int64_t PO = P * O;
+    const double *dX, *dP, *dsig = nullptr, *deps = nullptr;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)P * D * 8, dev_ptrs(flags), &dX));
+    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)((S - 1) * params_stride + s.nparams) * 8, false, &dP));
+    if (eps) {
+        RET_IF(stage_in(ctx, st, ctx->d_in[2], sigma, (size_t)S * 8, false, &dsig));
+        RET_IF(stage_in(ctx, st, ctx->d_in[3], eps, (size_t)S * n * PO * 8, false, &deps));
+    }
+    const int64_t nout = round_up(S * PO, 8);
+    RET_IF(ensure(ctx, ctx->d_out[0], (size_t)(eps ? 2 : 1) * nout * 8));
+    double* dloc = (double*)ctx->d_out[0].p;
+    double* dys = eps ? dloc + nout : nullptr;
+    const size_t smem = ctx->bnn_fused ? bnn_fused_smem(D, n_layers, widths, false, ctx->smem_optin) : 0;
+    if (smem) {
+        RET_IF(bnn_optin(ctx));
+        const BnnNet net = bnn_net(D, n_layers, widths);
+        for (int64_t s0 = 0; s0 < S; s0 += 65535) {   // grid.y holds at most 65535 draws
+            const dim3 grid((unsigned)ceil_div(P, BNN_ROWS), (unsigned)std::min<int64_t>(S - s0, 65535));
+            RET_IF(launch(ctx, st, grid, BNN_THREADS, smem, bnn_predict_kernel, net, act, dX, P, dP, params_stride, dsig, deps, (int)n,
+                          dloc, dys, s0));
+        }
+    } else {
+        std::vector<double*> H;
+        for (int64_t m = 0; m < S; ++m) {
+            RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP + m * params_stride, H));
+            RET_IF(launch(ctx, st, grid_for(PO), 256, 0, bnn_sample_kernel, (const double*)H[s.L], PO, m, dsig, deps, (int)n, dloc, dys));
+        }
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(loc, dloc, (size_t)S * PO * 8, cudaMemcpyDeviceToHost, st));
+    if (eps) CUDA_TRY(ctx, cudaMemcpyAsync(y_sampled, dys, (size_t)S * PO * 8, cudaMemcpyDeviceToHost, st));
+    RET_IF(tm.end(st, nullptr));
+    return B2GP_OK;
 }
 
 // value and gradient of the VFE bound of the sparse GP (see sparse_elbo.cuh): d/dlog(lengthscale[d], k_scale, noise, period)

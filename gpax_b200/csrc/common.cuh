@@ -129,6 +129,8 @@ struct b2gp_ctx {
     int tall_min = 2048;   // smallest N factored by potrf_tall on the int8 route
     int tall_min_fp64 = 8192;  // smallest N factored by potrf_tall on the fp64 route (ozaki = 0); DESIGN.md 4.2
     int oz_debug = 0;  // see OzArgs::debug (0 in production)
+    int bnn_fused = 1;     // 1: BNN entry points take the fused kernels where the network fits (bnn.cuh); 0: layered route
+    size_t smem_optin = 0; // opt-in dynamic shared memory per block of the device
     // 0: fp64 DMMA only; 6 / 7: large rank-k updates through the int8 wgmma path with that many base-256 digit planes
     // (46 / 54 bits per operand); -1: 6 or 7 per factorisation from a bound on cond(K), see oz_auto_planes().
     // Default 0: on H100 the int8 path is slower than DMMA (DESIGN.md section 5).

@@ -325,6 +325,30 @@ int  b2gp_mtdkl_mll(b2gp_ctx* ctx, int kind, const double* X, const int* task, i
                     unsigned flags, double* value, double* grad_theta, double* grad_B, double* grad_noise,
                     double* grad_params, double* grad_z, int* info);
 
+/* ---- fully Bayesian MLP (gpax/models/bnn.py over spm.py; gpax_b200/csrc/bnn.cuh) --------------------------------------
+ * The network of b2gp_mlp_forward: n_layers >= 1 dense layers with widths[l] outputs (widths[n_layers-1] = O), act on
+ * every layer but the last, params in the flat layout (per layer W_l [in, out] row-major, then b_l).
+ * b2gp_bnn_loglik: value = sum_{i,o} log N(y[i,o]; MLP(X)[i,o], sigma) -- the likelihood of sPM.model, spm.py:63-77 --
+ *   with d value / d sigma and, when grad_params is given, d value / d params in the flat layout.  sigma > 0, finite.  X[N,D], y[N,O] follow
+ *   `flags` (B2GP_FLAG_DEVICE_PTRS; B2GP_FLAG_F32 is refused); widths, params and the outputs are HOST pointers.
+ *   Deterministic: identical calls give identical bits.
+ * Route: fused (two launches: a tile kernel that keeps the weight set, a gradient accumulator and one 32-row tile's
+ *   activations in shared memory, and a fixed-order reduction) when 8 * (2 * nparams + 32 * sum_l (width_l | 1)) bytes,
+ *   with width_0 = D, plus 2 KB fit in the device's opt-in shared memory per block and n_layers <= 16; otherwise
+ *   layered (the b2gp_mlp_forward pass, a residual kernel, b2gp_dkl_mll's backward pass).  Option "bnn_fused" = 0 forces
+ *   the layered route.
+ * b2gp_bnn_predict: loc[s] = MLP(X; params + s * params_stride) for S weight sets, [S,P,O]; when eps [S,n,P,O]
+ *   is given, y_sampled[s] = loc[s] + sigma[s] * mean_k eps[s,k] (k in order; spm.py:150-154).  X follows `flags`,
+ *   everything else is a HOST pointer.  Fused (grid (row tiles, draws): one launch per 65535 draws) when
+ *   8 * (nparams + 32 * sum_l (width_l | 1)) bytes fit, as above; otherwise the forward pass and a sampling epilogue per
+ *   draw.                                                                                                                */
+int  b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                     const int64_t* widths, int act, const double* params, double sigma, unsigned flags, double* value,
+                     double* grad_sigma, double* grad_params);
+int  b2gp_bnn_predict(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int n_layers, const int64_t* widths, int act,
+                      const double* params, int64_t S, int64_t params_stride, int64_t O, const double* sigma,
+                      const double* eps, int64_t n, double* loc, double* y_sampled, unsigned flags);
+
 /* Samples of S multivariate normals: y[s,i,:] = mean[s,:] + chol(cov[s]) eps[s,i,:], i < n -- replaces
  * numpyro.distributions.MultivariateNormal(mean, cov).sample (gpax/models/gp.py:292, gpax/acquisition/base_acq.py:221)
  * where the caller changed cov after the posterior call (gpax/models/hskgp.py:201-204 adds the predicted noise variance).
