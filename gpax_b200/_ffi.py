@@ -23,6 +23,7 @@ KIND = {"RBF": KERNEL_RBF, "Matern": KERNEL_MATERN52, "Periodic": KERNEL_PERIODI
 FLAG_DEVICE_PTRS = 1 << 0
 FLAG_LOWER_ONLY = 1 << 1
 FLAG_F32 = 1 << 2
+FLAG_KPP_DIAG = 1 << 3
 OUT_MEAN, OUT_VAR, OUT_COV, OUT_SAMPLE = 1 << 4, 1 << 5, 1 << 6, 1 << 7
 OUT_DMEAN, OUT_DVAR = 1 << 8, 1 << 9
 
@@ -96,6 +97,9 @@ SIGNATURES = {
     "b2gp_sparse_posterior": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
                                         _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _ip]),
+    "b2gp_mll_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int64, C.c_uint, _dp, _vp, _vp, _ip]),
+    "b2gp_posterior_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
+                                      C.c_int64, C.c_uint, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mlp_forward": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_uint]),
     "b2gp_dkl_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint,
                                _dp, _vp, _vp, _vp, _ip]),
@@ -262,7 +266,7 @@ class Context:
 
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
-             "potrf_tall_fp64", "mll_nngp_grad")
+             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""
@@ -465,6 +469,71 @@ class Context:
                                         _ptr(theta), _ptr(nv), float(jitter), 0, C.byref(val), _ptr(grad), _ptr(alpha), _ptr(gnv),
                                         C.byref(info)))
         return val.value, grad, alpha, info.value, gnv
+
+    def mll_gram(self, K, yres, dKs=(), want_grad=True, want_alpha=False):
+        """log N(yres; 0, K) from a caller-supplied K [N, N] (factored as (K + K^T) / 2), the traces
+        grad[j] = 1/2 sum (alpha alpha^T - K^-1) * dKs[j] for the N x N matrices in `dKs`, and alpha = K^-1 yres
+        (b2gp_mll_gram).  K, yres and the dKs are all NumPy arrays, or all DeviceArrays (B2GP_FLAG_DEVICE_PTRS).
+        Returns (value, grad [len(dKs)] or None, alpha [N] or None, info)."""
+        dev = isinstance(K, DeviceArray)
+        if dev:
+            N = K.shape[0]
+            if K.shape != (N, N) or tuple(yres.shape) != (N,) or any(tuple(D.shape) != (N, N) for D in dKs):
+                raise ValueError("K and every dK must be [N, N] and yres [N]")
+            Kp, yp, ptrs = K.ptr, yres.ptr, [D.ptr.value for D in dKs]
+        else:
+            K, yres = _f64(K), _f64(yres)
+            N = K.shape[0]
+            dKs = [_f64(D) for D in dKs]
+            if K.shape != (N, N) or yres.shape != (N,) or any(D.shape != (N, N) for D in dKs):
+                raise ValueError("K and every dK must be [N, N] and yres [N]")
+            Kp, yp, ptrs = _ptr(K), _ptr(yres), [D.ctypes.data for D in dKs]
+        p = len(ptrs) if want_grad else 0
+        arr = (C.c_void_p * max(p, 1))(*ptrs[:p])
+        val = C.c_double(0.0)
+        grad = np.zeros(p) if want_grad else None
+        alpha = np.zeros(N) if want_alpha else None
+        info = C.c_int(0)
+        self._check(self.lib.b2gp_mll_gram(self.h, Kp, N, N, yp, C.cast(arr, _vp), N, p, FLAG_DEVICE_PTRS if dev else 0,
+                                           C.byref(val), _ptr(grad), _ptr(alpha), C.byref(info)))
+        return val.value, grad, alpha, info.value
+
+    def posterior_gram(self, Kxx, Kpx, Kpp, yres, want=("mean", "cov"), eps=None, kpp_diag=False, timing=False):
+        """The batched posterior from caller-supplied Gram blocks (b2gp_posterior_gram): Kxx [S, N, N] or [N, N] (shared),
+        Kpx [S, P, N] or [P, N], Kpp [S, P, P] or [P, P] -- or with kpp_diag its diagonal [S, P] or [P] (mean / var only) --
+        and yres [N] or [S, N].  Host fp64 arrays; outputs as posterior()."""
+        Kxx, Kpx, yres = _f64(Kxx), _f64(Kpx), _f64(yres)
+        N = Kxx.shape[-1]
+        P = Kpx.shape[-2]
+        Kpp = None if Kpp is None else _f64(Kpp)
+        pp = (P,) if kpp_diag else (P, P)
+        S = max([1] + [a.shape[0] for a, nd in ((Kxx, 3), (Kpx, 3), (Kpp, len(pp) + 1), (yres, 2)) if a is not None and a.ndim == nd])
+        for a, shp in ((Kxx, (N, N)), (Kpx, (P, N)), (Kpp, pp), (yres, (N,))):
+            if a is not None and a.shape not in (shp, (S,) + shp):
+                raise ValueError(f"Gram block of shape {a.shape}: expected {shp} or {(S,) + shp}")
+        stride = lambda a, n: 0 if a is None or a.ndim == len(n) else int(np.prod(n))   # noqa: E731
+        flags = FLAG_KPP_DIAG if kpp_diag else 0
+        out = {"mean": None, "var": None, "cov": None, "y_sampled": None}
+        for name, bit, shape in (("mean", OUT_MEAN, (S, P)), ("var", OUT_VAR, (S, P)), ("cov", OUT_COV, (S, P, P))):
+            if name in want:
+                flags |= bit
+                out[name] = np.empty(shape)
+        n_samp = 0
+        if eps is not None:
+            eps = _f64(eps).reshape(S, -1, P)
+            n_samp = eps.shape[1]
+            flags |= OUT_SAMPLE
+            out["y_sampled"] = np.empty((S, n_samp, P))
+        info = np.zeros(S, dtype=np.int32)
+        t = Timing()
+        self._check(self.lib.b2gp_posterior_gram(
+            self.h, _ptr(Kxx), stride(Kxx, (N, N)), N, _ptr(Kpx), stride(Kpx, (P, N)), _ptr(Kpp), stride(Kpp, pp), P, S, _ptr(yres),
+            stride(yres, (N,)), flags, _ptr(out["mean"]), _ptr(out["var"]), _ptr(out["cov"]), _ptr(eps), n_samp, _ptr(out["y_sampled"]),
+            info.ctypes.data_as(_vp), C.byref(t) if timing else None))
+        out["info"] = info
+        if timing:
+            out["timing"] = t.as_dict()
+        return out
 
     def posterior_multitask(self, kind, Xtr, task_tr, yres, Xnew, task_new, theta, B, noise, group=1, noiseless=False, jitter=1e-6,
                             want=("mean", "cov"), eps=None, timing=False, flags=0):

@@ -601,6 +601,35 @@ struct MtDesc {
     const double* noise;   // [S, T]
 };
 
+// ---- caller-supplied Gram matrices (b2gp_mll_gram, b2gp_posterior_gram)
+// The lower triangle of (K + K^T) / 2 into A (leading dimension lda).  A host K is first copied whole into `stage`.
+static int gram_copyin(b2gp_ctx* ctx, cudaStream_t st, DevBuf& stage, const double* K, int64_t ldk, int64_t N, bool dev, double* A,
+                       int64_t lda) {
+    const double* src = K;
+    int64_t lds = ldk;
+    if (!dev) {
+        lds = round_up(N, 8);
+        RET_IF(ensure(ctx, stage, (size_t)N * lds * 8));
+        CUDA_TRY(ctx, cudaMemcpy2DAsync(stage.p, (size_t)lds * 8, K, (size_t)ldk * 8, (size_t)N * 8, (size_t)N, cudaMemcpyHostToDevice, st));
+        src = (const double*)stage.p;
+    }
+    const unsigned t = (unsigned)ceil_div(N, (int64_t)GCOPY_TILE);
+    return launch(ctx, st, dim3(t, t), dim3(GCOPY_TILE, 8), 0, gram_copyin_kernel, src, lds, N, A, lda);
+}
+
+// b2gp_posterior_gram: the three Gram blocks of every draw come from the caller (host or device arrays, as `flags`):
+// k_XX [N, N] (symmetrised on the copy-in), k_pX [P, N], k_pp [P, P] or only its diagonal [P] (kpp_diag); strides between
+// draws in doubles, 0 = shared.
+struct GramPost {
+    const double* Kxx;
+    int64_t kxx_stride;
+    const double* Kpx;
+    int64_t kpx_stride;
+    const double* Kpp;
+    int64_t kpp_stride;
+    bool kpp_diag;
+};
+
 // The posterior with everything that may vary per draw: the training inputs (xtr_stride doubles between draws; 0 =
 // shared), the test inputs (xnew_stride), the targets (yres_stride) and an optional vector of per-point noise variances
 // added to the diagonal of k_XX (nv_stride between draws; 0 = shared).  b2gp_posterior is the all-shared special case.
@@ -611,7 +640,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                           const double* theta, const double* noise_vec, int64_t nv_stride, int noiseless, double jitter,
                           unsigned flags, double* mean, double* var, double* cov, const double* eps, int64_t n_samp,
                           double* y_sampled, int* info, b2gp_timing* timing, double* dmean_out = nullptr, double* dvar_out = nullptr,
-                          const MtDesc* mt = nullptr) {
+                          const MtDesc* mt = nullptr, const GramPost* gp = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
     const bool nngp = is_nngp(kind);   // NNGP: no multi-task form, no test-input gradient
@@ -619,7 +648,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     ARG_CHECK(ctx, xtr_stride == 0 || xtr_stride >= N * d);
     ARG_CHECK(ctx, xnew_stride == 0 || xnew_stride >= P * d);
     ARG_CHECK(ctx, nv_stride == 0 || nv_stride >= N);
-    ARG_CHECK(ctx, Xtr && yres && Xnew && theta && info);
+    ARG_CHECK(ctx, (gp || (Xtr && Xnew && theta)) && yres && info);
     ARG_CHECK(ctx, N >= 1 && P >= 1 && S >= 1 && d >= 1 && d <= GRAM_MAX_D);
     ARG_CHECK(ctx, yres_stride == 0 || yres_stride >= N);
     const bool want_mean = flags & B2GP_OUT_MEAN, want_var = flags & B2GP_OUT_VAR;
@@ -663,7 +692,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     // NNGP: d+3 zeros, the theta of the zero prior the variance epilogue starts from
     const double* dzero = nullptr;
     std::vector<double> hzero;
-    if (nngp) {
+    if (nngp || gp) {
         hzero.assign((size_t)d + 3, 0.0);
         RET_IF(stage_in(ctx, st0, ctx->d_in[5], hzero.data(), hzero.size() * 8, false, &dzero));
     }
@@ -742,7 +771,8 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
         if (need_cov) RET_IF(ensure(ctx, sl.cov, (size_t)P * ldC * 8));
         if (want_samp) RET_IF(ensure(ctx, sl.LinvC, (size_t)linv_bytes(P)));
-        if (!want_mean || ((mt || nngp) && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)((mt || nngp) ? 2 * P : P) * 8));
+        if (!want_mean || ((mt || nngp || gp) && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)((mt || nngp || gp) ? 2 * P : P) * 8));
+        if (gp && !dev) RET_IF(ensure(ctx, sl.Vt, (size_t)N * ldA * 8));   // a host k_XX is staged here before the copy-in
     }
     // inputs and the memset of dinfo were queued on st0: order the other streams behind them
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
@@ -751,7 +781,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
 
     // host copy of theta: the accuracy-aware digit-plane count of the int8 path is chosen per draw (oz_auto_planes)
     std::vector<double> htheta;
-    if (ctx->ozaki == -1 && !mt) {
+    if (ctx->ozaki == -1 && !mt && !gp) {
         htheta.resize((size_t)S * nth);
         if (dev) {
             CUDA_TRY(ctx, cudaMemcpyAsync(htheta.data(), dtheta, (size_t)S * nth * 8, cudaMemcpyDeviceToHost, st0));
@@ -761,6 +791,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         }
     }
     const double noise_mult_new = noiseless ? 0.0 : 1.0;  // gp.py:260-261
+    const cudaMemcpyKind cpkind = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;   // caller Gram blocks
     std::vector<StageEvents> sev;
     if (timing) sev.resize((size_t)S);
 
@@ -770,7 +801,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     // leaves it so, and it is re-validated -- together with the factor's `info` -- only after the call's work has
     // completed on the device (end of this function).
     bool reuse = false;
-    const bool cacheable = (S == 1 && !dev && !noise_vec && !mt);
+    const bool cacheable = (S == 1 && !dev && !noise_vec && !mt && !gp);
     if (cacheable) {
         auto& fc = ctx->fcache;
         const size_t xbytes = (size_t)N * d * (f32 ? 4 : 8);
@@ -790,7 +821,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         double* A = (double*)sl.A.p;
         double* Vt = A + N * ldA;
         double* Linv = (double*)sl.Linv.p;
-        const double* th = dtheta + s * nth;
+        const double* th = dtheta ? dtheta + s * nth : nullptr;
         const double* dXtr_s = dXtr + s * xtr_stride;
         const double* dXnew_s = dXnew + s * xnew_stride;
         // the P-side solve rides along with the factorisation (int8 or fp64 route of the tall-panel scheme)
@@ -810,7 +841,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         const int *dtr = dtask, *dtn = mt ? dtask + N : nullptr;
         auto rhs_rows = [&]() -> int {
             // k_pX = kernel(X_new, X_train, params, jitter=0.0)  (gp.py:268); same-shape inputs add 0 there
-            if (mt)
+            if (gp)
+                CUDA_TRY(ctx, cudaMemcpy2DAsync(Vt, (size_t)ldV * 8, gp->Kpx + s * gp->kpx_stride, (size_t)N * 8, (size_t)N * 8, (size_t)P, cpkind, st));
+            else if (mt)
                 RET_IF(launch_gram_lcm(ctx, st, LCM_RECT, kind, dXnew_s, dtn, P, dXtr_s, dtr, N, d, T, L, grp, th, Bs, ns, 0.0, 0.0, Vt, ldV));
             else
                 RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, 0.0, 0.0, 0, 0, Vt, ldV));
@@ -820,7 +853,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         };
         if (!reuse) {
             // k_XX = kernel(X_train, X_train, params, noise, jitter)  (gp.py:269) -- lower triangle only
-            if (mt)
+            if (gp)
+                RET_IF(gram_copyin(ctx, st, sl.Vt, gp->Kxx + s * gp->kxx_stride, N, N, dev, A, ldA));
+            else if (mt)
                 RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dXtr_s, dtr, N, dXtr_s, dtr, N, d, T, L, grp, th, Bs, ns, 1.0, jitter, A, ldA));
             else
                 RET_IF(launch_gram(ctx, st, kind, dXtr_s, N, dXtr_s, N, d, th, 1.0, jitter, 1, 1, A, ldA));
@@ -861,14 +896,18 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                                        jitter, prior, 1));
                 RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, add_vec_kernel, dvar + s * P, (const double*)prior, P));
             }
-        } else if (nngp) {   // as the multi-task branch, with the NNGP prior diagonal k(x_p, x_p) + noise_p + jitter
+        } else if (nngp || gp) {   // as the multi-task branch, with the prior diagonal k(x_p, x_p) + noise_p + jitter
             if (want_mean || want_var || want_samp)
                 RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot_kernel, Vt, ldV, N, P, (int)B2GP_KERNEL_PERIODIC, d, dzero, 0.0, 0.0,
                               inf, mean_s, want_var ? dvar + s * P : nullptr));
             if (want_var) {
                 double* prior = (double*)sl.misc.p + P;
-                RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, nngp_diag_kernel, dXnew_s, P, d, kind, th, noise_mult_new,
-                              jitter, prior));
+                if (gp)   // diag(k_pp): a strided copy of the full block's diagonal, or the caller's diagonal as it is
+                    CUDA_TRY(ctx, cudaMemcpy2DAsync(prior, 8, gp->Kpp + s * gp->kpp_stride, (size_t)(gp->kpp_diag ? 1 : P + 1) * 8, 8, (size_t)P,
+                                                    cpkind, st));
+                else
+                    RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, nngp_diag_kernel, dXnew_s, P, d, kind, th, noise_mult_new,
+                                  jitter, prior));
                 RET_IF(launch(ctx, st, (unsigned)ceil_div(P, (int64_t)256), 256, 0, add_vec_kernel, dvar + s * P, (const double*)prior, P));
             }
         } else if (want_mean || want_var || want_samp) {
@@ -883,7 +922,9 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             // cov = k_pp - V^T V  (gp.py:267, 272), lower tiles then mirrored -> exactly symmetric
             double* C = want_cov ? dcov + s * P * P : (double*)sl.cov.p;
             const int64_t ldc = want_cov ? P : ldC;
-            if (mt)
+            if (gp)
+                CUDA_TRY(ctx, cudaMemcpy2DAsync(C, (size_t)ldc * 8, gp->Kpp + s * gp->kpp_stride, (size_t)P * 8, (size_t)P * 8, (size_t)P, cpkind, st));
+            else if (mt)
                 RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dXnew_s, dtn, P, dXnew_s, dtn, P, d, T, L, grp, th, Bs, ns, noise_mult_new,
                                        jitter, C, ldc));
             else
@@ -1024,6 +1065,25 @@ extern "C" int b2gp_posterior_grad(b2gp_ctx* ctx, int kind, const double* Xtr, i
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
     return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
                           var, nullptr, nullptr, 0, nullptr, info, timing, dmean, dvar);
+}
+
+extern "C" int b2gp_posterior_gram(b2gp_ctx* ctx, const double* Kxx, int64_t kxx_stride, int64_t N, const double* Kpx, int64_t kpx_stride,
+                                   const double* Kpp, int64_t kpp_stride, int64_t P, int64_t S, const double* yres, int64_t yres_stride,
+                                   unsigned flags, double* mean, double* var, double* cov, const double* eps, int64_t n_samp,
+                                   double* y_sampled, int* info, b2gp_timing* timing) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_posterior_gram", "fp64 arrays only", __FILE__, __LINE__);
+    const bool diag = flags & B2GP_FLAG_KPP_DIAG;
+    ARG_CHECK(ctx, !(flags & (B2GP_OUT_DMEAN | B2GP_OUT_DVAR)));
+    ARG_CHECK(ctx, !diag || !(flags & (B2GP_OUT_COV | B2GP_OUT_SAMPLE)));
+    ARG_CHECK(ctx, Kxx && Kpx && N >= 1 && P >= 1);
+    ARG_CHECK(ctx, Kpp || !(flags & (B2GP_OUT_VAR | B2GP_OUT_COV | B2GP_OUT_SAMPLE)));
+    ARG_CHECK(ctx, kxx_stride == 0 || kxx_stride >= N * N);
+    ARG_CHECK(ctx, kpx_stride == 0 || kpx_stride >= P * N);
+    ARG_CHECK(ctx, kpp_stride == 0 || kpp_stride >= (diag ? P : P * P));
+    const GramPost gp{Kxx, kxx_stride, Kpx, kpx_stride, Kpp, kpp_stride, diag};
+    return posterior_impl(ctx, B2GP_KERNEL_RBF, nullptr, 0, N, yres, yres_stride, nullptr, 0, P, 1, S, nullptr, nullptr, 0, 0, 0.0, flags,
+                          mean, var, cov, eps, n_samp, y_sampled, info, timing, nullptr, nullptr, nullptr, &gp);
 }
 
 // the common checks of the two multi-task entries: limits, host fp64 arrays, task ids in [0, T) (so that no kernel can
@@ -1407,17 +1467,65 @@ __global__ void mll_diag_grad_kernel(const double* __restrict__ alpha, const dou
     if (i < n) g[i] = 0.5 * (alpha[i] * alpha[i] - Kinv[i * ldk + i]);
 }
 
+// b2gp_mll_gram: K and its derivatives dK_j come from the caller instead of the fused Gram build and gradient reduction.
+// K (leading dimension ldk) and every dK[j] (lddk) follow `flags`; dK is a host array of p pointers.
+struct GramMll {
+    const double* K;
+    int64_t ldk;
+    const double* const* dK;
+    int64_t lddk, p;
+};
+
+// gout[j] = 1/2 sum_{a,b} W_ab dK_j[a, b] (mll_gram_trace_kernel, then the fixed-order column sums of mll_lcm_finish_kernel).
+// Device dK: one launch over all p.  Host dK: streamed through the two N x ld buffers buf0 / buf1 -- the copy of dK_{j+1} on
+// a second stream overlaps the reduction of dK_j, and the copy into a buffer waits for the reduction that last read it.
+// `dptrs` is device scratch for max(p, 2) pointers.
+static int mll_gram_trace(b2gp_ctx* ctx, cudaStream_t st, const GramMll& gm, bool dev, int tiles, const double* alpha,
+                          const double* Kinv, int64_t ld, int64_t N, double* buf0, double* buf1, const double** dptrs, double* partial,
+                          double* gout) {
+    const int p = (int)gm.p;
+    const dim3 grid((unsigned)tiles, (unsigned)tiles);
+    count_path(ctx, (int)PATH_MLL_GRAM_TRACE);
+    if (dev) {
+        CUDA_TRY(ctx, cudaMemcpyAsync(dptrs, gm.dK, (size_t)p * sizeof(double*), cudaMemcpyHostToDevice, st));
+        RET_IF(launch(ctx, st, grid, MLL_THREADS, 0, mll_gram_trace_kernel, alpha, Kinv, ld, N, (const double* const*)dptrs, gm.lddk, p, 0,
+                      p, partial));
+    } else {
+        const double* bufs[2] = {buf0, buf1};
+        CUDA_TRY(ctx, cudaMemcpyAsync(dptrs, bufs, sizeof bufs, cudaMemcpyHostToDevice, st));
+        cudaStream_t cs = ctx->slots[1].stream;
+        cudaEvent_t free_ev = ctx->pool.get(), cp[2] = {ctx->pool.get(), ctx->pool.get()}, red[2] = {ctx->pool.get(), ctx->pool.get()};
+        ARG_CHECK(ctx, free_ev && cp[0] && cp[1] && red[0] && red[1]);
+        CUDA_TRY(ctx, cudaEventRecord(free_ev, st));   // everything before (L^{-T} in buf0, the factor in buf1) is done with
+        CUDA_TRY(ctx, cudaStreamWaitEvent(cs, free_ev, 0));
+        for (int j = 0; j < p; ++j) {
+            const int b = j & 1;
+            if (j >= 2) CUDA_TRY(ctx, cudaStreamWaitEvent(cs, red[b], 0));
+            CUDA_TRY(ctx, cudaMemcpy2DAsync((void*)bufs[b], (size_t)ld * 8, gm.dK[j], (size_t)gm.lddk * 8, (size_t)N * 8, (size_t)N,
+                                            cudaMemcpyHostToDevice, cs));
+            CUDA_TRY(ctx, cudaEventRecord(cp[b], cs));
+            CUDA_TRY(ctx, cudaStreamWaitEvent(st, cp[b], 0));
+            RET_IF(launch(ctx, st, grid, MLL_THREADS, 0, mll_gram_trace_kernel, alpha, Kinv, ld, N, (const double* const*)(dptrs + b), ld, 1, j,
+                          p, partial));
+            CUDA_TRY(ctx, cudaEventRecord(red[b], st));
+        }
+    }
+    return launch(ctx, st, (unsigned)p, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, (int64_t)tiles * tiles, p, gout);
+}
+
 static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, const double* theta,
                     const double* noise_vec, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
-                    double* grad_noise_vec, int* info, const MtDesc* mt = nullptr, double* grad_x_dev = nullptr) {
+                    double* grad_noise_vec, int* info, const MtDesc* mt = nullptr, double* grad_x_dev = nullptr,
+                    const GramMll* gm = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, !grad_noise_vec || grad);
+    ARG_CHECK(ctx, !gm || (!mt && !noise_vec && !grad_x_dev && kind == B2GP_KERNEL_RBF));
     ARG_CHECK(ctx, !grad_x_dev || (grad && !noise_vec && (!mt || kind != B2GP_KERNEL_PERIODIC)));
     ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
     // NNGP: single task, no input gradient; no per-feature accumulator, so the Gram build's d <= 64 is the limit
     const bool nngp = is_nngp(kind);
     ARG_CHECK(ctx, !nngp || (!mt && !grad_x_dev));
-    ARG_CHECK(ctx, X && yres && theta && value && info);
+    ARG_CHECK(ctx, (gm || (X && theta)) && yres && value && info);
     ARG_CHECK(ctx, N >= 1 && d >= 1 && d <= (nngp ? GRAM_MAX_D : MLL_MAX_D));
     if (nngp) RET_IF(nngp_check_depth(ctx, "b2gp_mll", theta[0]));
     const int depth = nngp ? (int)theta[0] : 0;
@@ -1432,13 +1540,13 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     // mll_lcm_grad_kernel are nout wide, L blocks of tiles^2
     const int T = mt ? mt->T : 0, L = mt ? mt->L : 0;
     const int nth = mt ? L * (d + 2) : d + 3;
-    const int ngrad = mt ? L * (d + 2) + L * T * T + T : nth, nout = d + 2 + T * T + T;
+    const int ngrad = gm ? (int)gm->p : mt ? L * (d + 2) + L * T * T + T : nth, nout = d + 2 + T * T + T;
     const double *dX, *dy, *dth, *dnv = nullptr, *dmt = nullptr;
     const int* dtask = nullptr;
     std::vector<double> hmt;
     RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, dev, &dX));
     RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)N * 8, dev, &dy));
-    RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
+    RET_IF(stage_in(ctx, st, ctx->d_in[3], gm ? nullptr : theta, (size_t)nth * 8, false, &dth));
     if (noise_vec) RET_IF(stage_in(ctx, st, ctx->d_in[6], noise_vec, (size_t)N * 8, dev, &dnv));
     if (mt) {
         hmt.resize((size_t)L * T * T + T);
@@ -1458,6 +1566,8 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + L * tiles * tiles * nout + L * nout) * 8));
     else if (nngp)   // partials [tiles^2, 3] | self-chains [N, depth, 3]
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * 3 + N * depth * 3) * 8));
+    else if (gm)   // partials [tiles^2, p] | grad [p] | the device array of dK pointers [max(p, 2)]
+        RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + (tiles * tiles + 2) * gm->p + 2) * 8));
     else
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * nth) * 8));
     int* dinfo = (int*)ctx->d_info.p;
@@ -1469,7 +1579,10 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     double* sc = alpha + ld;             // [0] sum log L_ii, [1] |w|^2, [8..8+nth) grad
     double* partial = sc + 64;
     double* gmt = partial + (size_t)L * tiles * tiles * nout;   // multi-task: per-latent column sums of the partials
-    if (mt)
+    double* gdev = nullptr;              // caller-Gram mode: the gradient [p]
+    if (gm)   // K staged through sl.cov, which takes L^{-T} only after the factorisation
+        RET_IF(gram_copyin(ctx, st, sl.cov, gm->K, gm->ldk, N, dev, A, ld));
+    else if (mt)
         RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dX, dtask, N, dX, dtask, N, d, T, L, mt->group, dth, dmt, dmt + (size_t)L * T * T, 1.0,
                                jitter, A, ld));
     else
@@ -1495,7 +1608,11 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
             // K^{-1} = L^{-T} L^{-1} accumulated onto zeros: beta = 1 is what the int8 tensor-core path takes (7 planes here)
             CUDA_TRY(ctx, cudaMemsetAsync(Kinv, 0, (size_t)N * ld * 8, st));
             RET_IF(gemm_nt(ctx, st, N, N, N, 1.0, Bt, ld, Bt, ld, 1.0, Kinv, ld, true));
-            if (mt) {
+            if (gm) {   // L^{-T} (sl.cov) and the factor (A) are free again: the staging buffers of host dK
+                gdev = partial + tiles * tiles * gm->p;
+                RET_IF(mll_gram_trace(ctx, st, *gm, dev, (int)tiles, alpha, Kinv, ld, N, Bt, A, (const double**)(gdev + gm->p), partial,
+                                      gdev));
+            } else if (mt) {
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles, (unsigned)L), MLL_THREADS, 0, mll_lcm_grad_kernel, dX, dtask, N,
                               d, kind, T, L, mt->group, dth, (const double*)dmt, (const double*)(dmt + (size_t)L * T * T), jitter,
                               (const double*)alpha, (const double*)Kinv, ld, partial));
@@ -1538,6 +1655,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, alpha, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
     std::vector<double> colsum(mt ? (size_t)L * nout : 0);
     if (grad && mt) CUDA_TRY(ctx, cudaMemcpyAsync(colsum.data(), gmt, colsum.size() * 8, cudaMemcpyDeviceToHost, st));
+    if (gdev) CUDA_TRY(ctx, cudaMemcpyAsync(grad, gdev, (size_t)gm->p * 8, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
     if (grad && mt) {   // grad_theta [L, d+2] | grad_B [L, T, T] (symmetrised) | grad_noise [T]  (mtgp.cuh)
         const int nth1 = d + 2;
@@ -1554,7 +1672,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     if (grad && nngp) {   // [0, d) depth slots: 0; d: log var_w; d+1: log noise; d+2: log var_b
         for (int k = 0; k < d; ++k) grad[k] = 0.0;
         for (int k = 0; k < 3; ++k) grad[d + k] = hsc[8 + k];
-    } else if (grad && !mt) {
+    } else if (grad && !mt && !gm) {
         for (int k = 0; k < nth; ++k) grad[k] = hsc[8 + k];
     }
     if (*info != 0) {
@@ -1577,6 +1695,21 @@ extern "C" int b2gp_mll_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, c
                           const double* noise_vec, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
                           double* grad_noise_vec, int* info) {
     return mll_impl(ctx, kind, X, N, yres, d, theta, noise_vec, jitter, flags, value, grad, alpha_out, grad_noise_vec, info);
+}
+
+extern "C" int b2gp_mll_gram(b2gp_ctx* ctx, const double* K, int64_t N, int64_t ldk, const double* yres, const double* const* dK,
+                             int64_t lddk, int64_t p, unsigned flags, double* value, double* grad, double* alpha_out, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_mll_gram", "fp64 arrays only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, K && N >= 1 && ldk >= N && p >= 0);
+    const bool want_grad = grad && p > 0;
+    if (want_grad) {
+        ARG_CHECK(ctx, dK && lddk >= N);
+        for (int64_t j = 0; j < p; ++j) ARG_CHECK(ctx, dK[j]);
+    }
+    const GramMll gm{K, ldk, dK, lddk, want_grad ? p : 0};
+    return mll_impl(ctx, B2GP_KERNEL_RBF, nullptr, N, yres, 1, nullptr, nullptr, 0.0, flags, value, want_grad ? grad : nullptr, alpha_out,
+                    nullptr, info, nullptr, nullptr, &gm);
 }
 
 // MultiTaskGP / CoregGP.model's likelihood (mtgp.py:147-167, corgp.py:66-98) with the LCM kernel and its gradient

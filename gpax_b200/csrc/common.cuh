@@ -110,6 +110,7 @@ enum PathCounter {
     PATH_POTRF_TALL,    // factorisations that took potrf_tall on the int8 route (top-level entries, not its recursion)
     PATH_POTRF_TALL_FP64,  // factorisations that took potrf_tall on the fp64 DMMA route (ozaki = 0), top-level entries
     PATH_MLL_NNGP_GRAD,    // likelihood gradients that took the NNGP route (mll_nngp_grad_kernel, nngp.cuh), one per call
+    PATH_MLL_GRAM_TRACE,   // likelihood gradients reduced against caller-supplied dK (mll_gram_trace_kernel), one per call
     PATH_COUNT
 };
 

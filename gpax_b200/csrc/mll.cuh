@@ -118,3 +118,82 @@ __global__ void mll_finish_kernel(const double* partial, int64_t nblocks, int no
     for (int64_t b = 0; b < nblocks; ++b) s += partial[b * nout + k];
     grad[k] = 0.5 * s;
 }
+
+// ---- caller-supplied Gram matrices (b2gp_mll_gram, b2gp_posterior_gram)
+// A[i, j] = (K[i, j] + K[j, i]) / 2 for j <= i: the symmetric part the reference's Cholesky factors
+// (MultivariateNormal(covariance_matrix=k)), written as the lower triangle the factorisation reads.  32 x 32 tiles, the
+// transposed tile staged through shared memory so that both reads are coalesced.  An exactly symmetric K is copied
+// bit for bit.
+constexpr int GCOPY_TILE = 32;
+__global__ void gram_copyin_kernel(const double* __restrict__ K, int64_t ldk, int64_t n, double* __restrict__ A, int64_t lda) {
+    __shared__ double t[GCOPY_TILE][GCOPY_TILE + 1];
+    if (blockIdx.x > blockIdx.y) return;
+    const int64_t r0 = (int64_t)blockIdx.y * GCOPY_TILE, c0 = (int64_t)blockIdx.x * GCOPY_TILE;
+    for (int y = threadIdx.y; y < GCOPY_TILE; y += blockDim.y) {
+        const int64_t i = c0 + y, j = r0 + threadIdx.x;
+        if (i < n && j < n) t[y][threadIdx.x] = K[i * ldk + j];   // K[c0 + y, r0 + x]
+    }
+    __syncthreads();
+    for (int y = threadIdx.y; y < GCOPY_TILE; y += blockDim.y) {
+        const int64_t i = r0 + y, j = c0 + threadIdx.x;
+        if (i < n && j <= i) A[i * lda + j] = 0.5 * (K[i * ldk + j] + t[threadIdx.x][y]);
+    }
+}
+
+// partial[block * pstride + k0 + k], k < p: sum over the block's 64 x 64 tile of the FULL matrix of W_ij dK_k[i, j], with
+// W = alpha alpha^T - K^{-1} formed on the fly from alpha and the lower triangle of K^{-1} (no symmetry assumed of dK_k).
+// The block's K^{-1} entries are staged through shared memory (an upper tile reads the transposed lower one), each
+// thread keeps its 16 W values in registers, and every dK_k is read once against them: W is formed once per tile
+// however many derivative matrices there are.  dK is a device array of p device pointers, leading dimension lddk.
+// Fixed-order warp and block sums: identical calls give identical bits.
+constexpr int TRACE_CHUNK = 32;   // derivative matrices per block-level reduction round
+__global__ void __launch_bounds__(MLL_THREADS)
+mll_gram_trace_kernel(const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk, int64_t N,
+                      const double* const* __restrict__ dK, int64_t lddk, int p, int k0, int pstride, double* __restrict__ partial) {
+    constexpr int PER = MLL_TILE * MLL_TILE / MLL_THREADS;
+    __shared__ double kin[MLL_TILE][MLL_TILE + 1];
+    __shared__ double red[MLL_THREADS / 32][TRACE_CHUNK];
+    const int64_t r0 = (int64_t)blockIdx.y * MLL_TILE, c0 = (int64_t)blockIdx.x * MLL_TILE;
+    const int64_t R0 = r0 > c0 ? r0 : c0, C0 = r0 > c0 ? c0 : r0;   // the lower-triangle block holding this tile's K^{-1}
+    for (int e = threadIdx.x; e < MLL_TILE * MLL_TILE; e += MLL_THREADS) {
+        const int64_t x = e / MLL_TILE, y = e % MLL_TILE, i = R0 + x, j = C0 + y;
+        kin[x][y] = (i < N && j <= i) ? Kinv[i * ldk + j] : 0.0;
+    }
+    __syncthreads();
+    double W[PER];
+    int64_t off[PER];
+    const int b = threadIdx.x % MLL_TILE;
+#pragma unroll
+    for (int r = 0; r < PER; ++r) {
+        const int a = threadIdx.x / MLL_TILE + r * (MLL_THREADS / MLL_TILE);
+        const int64_t i = r0 + a, j = c0 + b;
+        off[r] = -1;
+        W[r] = 0.0;
+        if (i < N && j < N) {
+            const double kv = i >= j ? kin[i - R0][j - C0] : kin[j - R0][i - C0];
+            W[r] = alpha[i] * alpha[j] - kv;
+            off[r] = i * lddk + j;
+        }
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int kc = 0; kc < p; kc += TRACE_CHUNK) {
+        const int nk = p - kc < TRACE_CHUNK ? p - kc : TRACE_CHUNK;
+        for (int kk = 0; kk < nk; ++kk) {
+            const double* __restrict__ D = dK[kc + kk];
+            double v = 0.0;
+#pragma unroll
+            for (int r = 0; r < PER; ++r)
+                if (off[r] >= 0) v += W[r] * D[off[r]];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+            if (lane == 0) red[warp][kk] = v;
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < nk) {
+            double v = 0.0;
+            for (int w = 0; w < MLL_THREADS / 32; ++w) v += red[w][threadIdx.x];
+            partial[((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * pstride + k0 + kc + threadIdx.x] = v;
+        }
+        __syncthreads();
+    }
+}

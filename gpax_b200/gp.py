@@ -44,6 +44,17 @@ def _theta_rows(params: Dict[str, np.ndarray], d: int, batched: bool) -> np.ndar
     return th
 
 
+GRAM_CHUNK_BYTES = 1 << 30      # host Gram bytes of one b2gp_posterior_gram call (user kernel callables)
+
+
+def gram_chunks(S, N, P, full_kpp=True, budget=GRAM_CHUNK_BYTES):
+    """[(start, stop)] over S draws such that each chunk's k_XX [N, N], k_pX [P, N] and k_pp ([P, P], or its diagonal
+    [P]) stay under `budget` bytes; a draw larger than the budget is a chunk of its own"""
+    per_draw = 8 * (N * N + P * N + (P * P if full_kpp else P))
+    step = max(1, int(budget) // per_draw)
+    return [(a, min(a + step, S)) for a in range(0, S, step)]
+
+
 def _eps_dtype():
     return np.float64 if x64_enabled() else np.float32
 
@@ -163,14 +174,15 @@ class ExactGP:
         Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
         d = X.shape[1]
         jitter = float(kwargs.get("jitter", 1e-6))
+        if self._fused is None:
+            return self._posterior_gram(X, y, Xn, params, batched, noiseless, want, eps, jitter)
         theta = self._theta(params, d, batched)
         S = theta.shape[0]
         yres = self._residuals(X, y, params, batched, S)
-        if self._fused is None:
-            raise NotImplementedError(
-                "user-supplied kernel callables are evaluated through get_mvn_posterior_callable(); "
-                "predict() with draws requires 'RBF', 'Matern' or 'Periodic'")
         out = self.ctx.posterior(self._fused, X, yres, Xn, theta, noiseless, jitter, want, eps)
+        return self._add_prior_mean(out, Xn, params, batched, S)
+
+    def _add_prior_mean(self, out, Xn, params, batched, S):
         pm = self._prior_mean(Xn, params, batched, S)
         if pm is not None:
             if out["mean"] is not None:
@@ -178,6 +190,31 @@ class ExactGP:
             if out["y_sampled"] is not None:
                 out["y_sampled"] = out["y_sampled"] + (pm[:, None, :] if pm.ndim == 2 else pm)
         return out
+
+    def _posterior_gram(self, X, y, Xn, params, batched, noiseless, want, eps, jitter):
+        """User kernel callable: per draw the three Gram blocks of gp.py:267-269 from the callable (host), then one
+        b2gp_posterior_gram call per chunk of draws (GRAM_CHUNK_BYTES of host Grams) for the factorisation, solves, mean,
+        variance, covariance and samples on the GPU"""
+        S = len(next(np.asarray(v) for v in params.values() if v is not None)) if batched else 1
+        yres = np.broadcast_to(self._residuals(X, y, params, batched, S), (S, X.shape[0]))
+        N, P = X.shape[0], Xn.shape[0]
+        full_kpp = "cov" in want or eps is not None
+        chunks = []
+        for a, b in gram_chunks(S, N, P, full_kpp):
+            Kxx, Kpx, Kpp = np.empty((b - a, N, N)), np.empty((b - a, P, N)), np.empty((b - a, P, P) if full_kpp else (b - a, P))
+            for s in range(a, b):
+                ps = {k: (None if v is None else np.asarray(v)[s]) for k, v in params.items()} if batched else params
+                noise = ps["noise"]
+                noise_p = noise * (1 - int(bool(noiseless)))                                       # gp.py:260-261
+                k_pp = np.asarray(self.kernel(Xn, Xn, ps, noise_p, jitter=jitter), dtype=np.float64)   # gp.py:267
+                Kpp[s - a] = k_pp if full_kpp else np.diagonal(k_pp)
+                Kpx[s - a] = self.kernel(Xn, X, ps, jitter=0.0)                                      # gp.py:268
+                Kxx[s - a] = self.kernel(X, X, ps, noise, jitter=jitter)                             # gp.py:269
+            chunks.append(self.ctx.posterior_gram(Kxx, Kpx, Kpp, yres[a:b], want, None if eps is None else eps[a:b],
+                                                  kpp_diag=not full_kpp))
+        out = {k: (None if chunks[0][k] is None else np.concatenate([c[k] for c in chunks]))
+               for k in ("mean", "var", "cov", "y_sampled", "info")}
+        return self._add_prior_mean(out, Xn, params, batched, S)
 
     def _posterior_grad(self, X_new, params, batched, noiseless, **kwargs):
         """Per-draw posterior mean [S, P], variance [S, P] and their gradients w.r.t. the test inputs dmean, dvar

@@ -144,8 +144,7 @@ def gp_model_program(m, d, kind):
         with P.plate("ard", d):
             length = P.sample("k_length", lp)
         kp = {"k_length": length, "k_scale": P.sample("k_scale", P.LogNormal(0.0, 1.0))}
-        if kind == "Periodic":
-            kp["period"] = P.sample("period", P.LogNormal(0.0, 1.0))
+        kp["period"] = P.sample("period", P.LogNormal(0.0, 1.0)) if kind == "Periodic" else None
     if m.noise_prior is not None:
         noise = m.noise_prior()
     else:                                                              # gp.py:222-227
@@ -178,9 +177,10 @@ class ProgramLogJoint:
     too."""
 
     FD_STEP = 1e-5
+    CALLABLE_KERNEL = False      # GramLogJoint: the kernel is the model's callable, not a fused GPU kernel
 
     def __init__(self, model, jitter=1e-6, lik=None):
-        if model._fused is None:
+        if model._fused is None and not self.CALLABLE_KERNEL:
             raise NotImplementedError("fit() needs kernel 'RBF', 'Matern' or 'Periodic'")
         self.m, self.jitter = model, float(jitter)
         X, y = model._train_arrays()
@@ -203,13 +203,18 @@ class ProgramLogJoint:
     def _model_program(self):
         return gp_model_program(self.m, self.d, self.kind)
 
-    def _run(self, u):
-        """u -> (theta[d+3], mean vector or None, sites with values)"""
+    def _program_at(self, u):
+        """u -> the model program's (kernel-parameter dict, noise, mean-function parameters) and its sites with values"""
         vals, o = {}, 0
         for s in self.sites:
             vals[s.name] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
             o += s.size
         (kp, noise, mp), sites, _ = P.run_program(self._model_program, vals)
+        return kp, noise, mp, sites
+
+    def _run(self, u):
+        """u -> (theta[d+3], mean vector or None, sites with values)"""
+        kp, noise, mp, sites = self._program_at(u)
         th = np.ones(self.d + 3)
         if _is_nngp(self.kind):
             th[:] = self.m._theta(dict(kp, noise=noise), self.d, False)[0]
@@ -312,6 +317,77 @@ class ProgramLogJoint:
                 out[s.name][r] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
                 o += s.size
         return out
+
+
+class GramLogJoint(ProgramLogJoint):
+    """The log joint of an ExactGP / viGP whose kernel is a user callable k(X, Z, params, noise, jitter) (gp.py:137-164
+    with any kernel gpax's get_kernel passes through).  Sites are those of ProgramLogJoint: the kernel_prior program's,
+    or the defaults of gp.py:229-247 over the model's kernel_dim with "period": None in the dict the callable receives.
+
+    One evaluation at u runs the program, calls the kernel once for K = k(X, X, params, noise, jitter) and, for every
+    coordinate u_k that moves the kernel dict or the noise, twice more for the central difference
+    dK_k = (K(u + h e_k) - K(u - h e_k)) / 2h.  One b2gp_mll_gram call then returns the value, the traces
+    d value / du_k = 1/2 sum (alpha alpha^T - K^-1) * dK_k and alpha = K^-1 (y - m): the N^3 factorisation is never
+    differenced, each direction costs two N^2 kernel evaluations on the host.  Coordinates of mean_fn_prior sites get
+    alpha . dm/du_k and no kernel evaluation; the prior terms are ProgramLogJoint's."""
+
+    CALLABLE_KERNEL = True
+
+    def __init__(self, model, jitter=1e-6):
+        super().__init__(model, jitter)
+        mean_sites = set()
+        if self.has_mean_params:     # mean_fn_prior runs after, and apart from, the kernel and noise statements
+            _, ms, _ = P.run_program(model.mean_fn_prior)
+            mean_sites = set(ms)
+        self.moves_kernel = np.concatenate([np.full(s.size, s.name not in mean_sites) for s in self.sites]) \
+            if self.sites else np.zeros(0, dtype=bool)
+        self.kernel_evals = 0
+
+    def _model_program(self):
+        return gp_model_program(self.m, self.m.kernel_dim, None)
+
+    def _gram(self, kp, noise):
+        self.kernel_evals += 1
+        return np.asarray(self.m.kernel(self.X, self.X, kp, noise, jitter=self.jitter), dtype=np.float64)
+
+    def __call__(self, u, jacobian):
+        u = np.asarray(u, dtype=np.float64)
+        kp, noise, mp, sites = self._program_at(u)
+        self.n_evals += 1
+        K = self._gram(kp, noise)
+        if not np.all(np.isfinite(K)):
+            return -np.inf, np.zeros(self.dim)
+        mean = self._mean(mp)
+        yres = self.y0 if mean is None else self.y0 - mean
+        h = self.FD_STEP
+        dKs, kcoords, dmean = [], [], {}
+        for k in range(self.dim):
+            if not (self.moves_kernel[k] or self.has_mean_params):
+                continue
+            e = np.zeros(self.dim)
+            e[k] = h
+            kpp, npl, mpp, _ = self._program_at(u + e)
+            kpm, nmi, mpm, _ = self._program_at(u - e)
+            if self.moves_kernel[k]:
+                dKs.append((self._gram(kpp, npl) - self._gram(kpm, nmi)) / (2 * h))
+                kcoords.append(k)
+            if self.has_mean_params:
+                dmean[k] = (self._mean(mpp) - self._mean(mpm)) / (2 * h)
+        val, g, alpha, info = self.m.ctx.mll_gram(K, yres, dKs, want_grad=True, want_alpha=self.has_mean_params)
+        if info != 0 or not np.isfinite(val):
+            return -np.inf, np.zeros(self.dim)
+        lp, grad = self._log_prior(u, sites, jacobian, want_grad=not self.hierarchical)
+        grad[kcoords] += g
+        for k, dm in dmean.items():
+            grad[k] += float(np.dot(alpha, dm))
+        if self.hierarchical:
+            for k in range(self.dim):
+                e = np.zeros(self.dim)
+                e[k] = h
+                lpp, _ = self._log_prior(u + e, self._program_at(u + e)[3], jacobian, want_grad=False)
+                lpm, _ = self._log_prior(u - e, self._program_at(u - e)[3], jacobian, want_grad=False)
+                grad[k] += (lpp - lpm) / (2 * h)
+        return val + lp, grad
 
 
 def mtgp_model_program(m, d, T, R, L):
@@ -422,6 +498,10 @@ class MTLogJoint(ProgramLogJoint):
 
 
 def make_log_joint(model, jitter=1e-6):
+    from .gp import ExactGP
+    from .vigp import viGP
+    if model._fused is None and type(model) in (ExactGP, viGP):
+        return GramLogJoint(model, jitter)
     if model.kernel_prior is not None or model.noise_prior is not None or \
             (model.mean_fn is not None and model.mean_fn_prior is not None):
         return ProgramLogJoint(model, jitter)

@@ -94,3 +94,78 @@ def initialize_inducing_points(X, ratio=0.1, method="uniform", key=None):
         from sklearn.cluster import KMeans
         return np.asarray(KMeans(n_clusters=m, random_state=0, n_init=10).fit(X).cluster_centers_)
     raise ValueError("Method must be 'uniform', 'random', or 'kmeans'")
+
+
+# ---- user mean and kernel functions written with named parameters (gpax/utils/fn.py)
+def _params_fn(func, leading, params_names, name=None):
+    """A copy of `func` whose arguments are `leading` + `params` and whose body reads every name in `params_names` as
+    params["name"].  The body is rewritten on its syntax tree and compiled in `func`'s own globals, so the modules the
+    user's function refers to (np, math, ...) resolve as they did."""
+    import ast
+    import inspect
+    import textwrap
+
+    tree = ast.parse(textwrap.dedent(inspect.getsource(func)))
+    fdef = tree.body[0]
+    names = set(params_names)
+
+    class ToParams(ast.NodeTransformer):
+        def visit_Name(self, node):
+            if node.id in names:
+                return ast.copy_location(ast.Subscript(value=ast.Name(id="params", ctx=ast.Load()), slice=ast.Constant(node.id),
+                                                       ctx=node.ctx), node)
+            return node
+
+    fdef = ToParams().visit(fdef)
+    fdef.decorator_list = []
+    fdef.name = name or fdef.name
+    fdef.args = ast.arguments(posonlyargs=[], args=[ast.arg(arg=a) for a in list(leading) + ["params"]], vararg=None, kwonlyargs=[],
+                              kw_defaults=[], kwarg=None, defaults=[])
+    ns = dict(func.__globals__)
+    exec(compile(ast.fix_missing_locations(tree), inspect.getsourcefile(func) or "<set_fn>", "exec"), ns)
+    return ns[fdef.name]
+
+
+def set_fn(func):
+    """gpax/utils/fn.py set_fn: f(x, a, b, ...) -> f(x, params) reading a, b, ... from the dict `params`, the form
+    ExactGP's mean_fn takes with a mean_fn_prior."""
+    import inspect
+    args = list(inspect.signature(func).parameters)
+    return _params_fn(func, args[:1], args[1:])
+
+
+def set_kernel_fn(func, independent_vars=("X", "Z"), jit_decorator=True, docstring=None):
+    """gpax/utils/fn.py set_kernel_fn: k(X, Z, p1, p2, ...) -> k(X, Z, params, noise=0, jitter=1e-6, **kwargs) reading its
+    parameters (the arguments without a default, other than `independent_vars`) from `params`, and adding
+    (noise + jitter) I when X.shape == Z.shape -- the kernel-callable form ExactGP / viGP take.  `jit_decorator` is
+    accepted for the reference's signature and ignored: there is no tracer on this side."""
+    import functools
+    import inspect
+    sig = inspect.signature(func)
+    names = [k for k, v in sig.parameters.items() if v.default is inspect.Parameter.empty and k not in independent_vars]
+    core = _params_fn(func, list(independent_vars), names, name=func.__name__)
+
+    @functools.wraps(func)
+    def kernel_fn(X, Z, params, noise=0, jitter=1e-6, **kwargs):
+        k = np.asarray(core(X, Z, params))
+        if np.shape(X) == np.shape(Z):
+            k = k + (noise + jitter) * np.eye(np.shape(X)[0])
+        return k
+    kernel_fn.__doc__ = docstring if docstring else func.__doc__
+    del kernel_fn.__wrapped__
+    return kernel_fn
+
+
+def _set_noise_kernel_fn(func):
+    """gpax/utils/fn.py _set_noise_kernel_fn: the kernel of a noise model, reading its "k..." parameters under
+    "k_noise..." names (k_noise_length for k_length, ...).  The keys are mapped before the call rather than the
+    source rewritten, so this works on any kernel callable, the fused RBFKernel / MaternKernel / PeriodicKernel included
+    (their parameters are read inside the Gram build, not in Python source)."""
+    import functools
+
+    @functools.wraps(func)
+    def noise_kernel_fn(X, Z, params, *args, **kwargs):
+        mapped = {k: v for k, v in params.items() if not k.startswith("k")}
+        mapped.update({"k" + k[len("k_noise"):]: v for k, v in params.items() if k.startswith("k_noise")})
+        return func(X, Z, mapped, *args, **kwargs)
+    return noise_kernel_fn

@@ -59,6 +59,7 @@ enum {
                                         noise_vec, eps in; K, mean, var, cov, y_sampled out) are float, the reference's default
                                         precision (gpax/utils/utils.py:19-21); theta stays double.  Widened / narrowed on the
                                         device, everything in between is fp64                                  */
+    B2GP_FLAG_KPP_DIAG    = 1u << 3, /* b2gp_posterior_gram: Kpp holds only the diagonal of each k_pp, [S, P]; OUT_MEAN / OUT_VAR only */
     B2GP_OUT_MEAN         = 1u << 4, /* b2gp_posterior: produce mean[S,P]                                    */
     B2GP_OUT_VAR          = 1u << 5, /* ... var[S,P] = diag(cov)     (viGP.predict, vigp.py:184-185)         */
     B2GP_OUT_COV          = 1u << 6, /* ... cov[S,P,P]               (get_mvn_posterior, gp.py:272)          */
@@ -234,6 +235,23 @@ int  b2gp_posterior_multitask(b2gp_ctx* ctx, int kind, const double* Xtr, const 
                               double jitter, unsigned flags, double* mean, double* var, double* cov, const double* eps,
                               int64_t n_samp, double* y_sampled, int* info, b2gp_timing* timing);
 
+/* The posterior of b2gp_posterior_batch with the Gram blocks supplied by the caller: the route of a user kernel callable
+ * k(X, Z, params, noise, jitter) (gpax/kernels/kernels.py:227-241; gp.py:267-269).  Per draw s:
+ *   Kxx[s * kxx_stride]  [N, N]  k_XX = kernel(X, X, params_s, noise_s, jitter); the library factors its symmetric part
+ *                                (K + K^T) / 2, as the reference's Cholesky does
+ *   Kpx[s * kpx_stride]  [P, N]  k_pX = kernel(X_new, X, params_s, jitter=0.0)
+ *   Kpp[s * kpp_stride]  [P, P]  k_pp = kernel(X_new, X_new, params_s, noise_p, jitter) -- its lower triangle is read, and
+ *                                var is taken as diag(k_pp) - |v_p|^2.  With B2GP_FLAG_KPP_DIAG: only diag(k_pp), [P]
+ *                                per draw, and the outputs are limited to mean / var.  May be NULL for mean-only calls.
+ * Strides are in doubles between draws, 0 = shared.  yres, flags (B2GP_OUT_* and B2GP_FLAG_DEVICE_PTRS, which covers the
+ * Gram blocks too), outputs, eps and info as b2gp_posterior_batch.  B2GP_FLAG_F32 gives B2GP_ERR_UNSUPPORTED.  The call
+ * neither uses nor fills the factor cache; under "ozaki" = -1 it takes 7 digit planes (the cond(K) bound needs k_scale). */
+int  b2gp_posterior_gram(b2gp_ctx* ctx, const double* Kxx, int64_t kxx_stride, int64_t N,
+                         const double* Kpx, int64_t kpx_stride, const double* Kpp, int64_t kpp_stride, int64_t P, int64_t S,
+                         const double* yres, int64_t yres_stride, unsigned flags,
+                         double* mean, double* var, double* cov, const double* eps, int64_t n_samp, double* y_sampled,
+                         int* info, b2gp_timing* timing);
+
 /* Nystrom / VFE sparse posterior for one theta -- replaces viSparseGP.get_mvn_posterior
  * (gpax/models/sparse_gp.py:173-223).  Xu[M,d] inducing points; theta[d+3] as above;
  * outputs mean[P] and var[P] (B2GP_OUT_VAR) and/or cov[P,P] (B2GP_OUT_COV).                        */
@@ -260,6 +278,19 @@ int  b2gp_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double*
 int  b2gp_mll_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d,
                 const double* theta, const double* noise_vec, double jitter, unsigned flags,
                 double* value, double* grad, double* alpha_out, double* grad_noise_vec, int* info);
+
+/* The likelihood and its gradient from caller-supplied matrices (a user kernel callable's fit):
+ *   value   = log N(yres; 0, K)  with K[N, N] (leading dimension ldk) factored as its symmetric part (K + K^T) / 2
+ *   grad[j] = 1/2 sum_{a,b} (alpha alpha^T - K^{-1})_{ab} dK_j[a, b],  j < p,  alpha = K^{-1} yres
+ * dK is a HOST array of p pointers to N x N matrices (leading dimension lddk); no symmetry is assumed of them.  K, yres and
+ * every dK_j are host arrays, or device arrays under B2GP_FLAG_DEVICE_PTRS; host dK_j are streamed through two device
+ * buffers, so p is limited by host memory only.  grad[p] and alpha_out[N] are optional HOST outputs (p = 0 or grad = NULL:
+ * no gradient).  The factorisation and solves are those of b2gp_mll (every "ozaki" / tall-panel route); the trace runs in
+ * a fixed order, so identical calls give identical bits.  NaN value and gradient where info != 0.  B2GP_FLAG_F32 gives
+ * B2GP_ERR_UNSUPPORTED.                                                                                                  */
+int  b2gp_mll_gram(b2gp_ctx* ctx, const double* K, int64_t N, int64_t ldk, const double* yres,
+                   const double* const* dK, int64_t lddk, int64_t p, unsigned flags,
+                   double* value, double* grad, double* alpha_out, int* info);
 
 /* The likelihood of MultiTaskGP.model / CoregGP.model (gpax/models/mtgp.py:147-167, corgp.py:66-98): log N(yres; 0, K)
  * with K the LCM covariance of b2gp_posterior_multitask (X[N,d], task[N], group, T, L, theta[L,d+2], B[L,T,T], noise[T]
