@@ -97,6 +97,8 @@ SIGNATURES = {
     "b2gp_sparse_posterior": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
                                         _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _ip]),
+    "b2gp_mll_batch": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, C.c_int64, _vp, C.c_double, C.c_uint, _vp, _vp, _vp,
+                                 _vp, _vp]),
     "b2gp_mll_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int64, C.c_uint, _dp, _vp, _vp, _ip]),
     "b2gp_posterior_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
                                       C.c_int64, C.c_uint, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
@@ -266,7 +268,7 @@ class Context:
 
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
-             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace")
+             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""
@@ -469,6 +471,28 @@ class Context:
                                         _ptr(theta), _ptr(nv), float(jitter), 0, C.byref(val), _ptr(grad), _ptr(alpha), _ptr(gnv),
                                         C.byref(info)))
         return val.value, grad, alpha, info.value, gnv
+
+    def mll_batch(self, kind, X, yres, theta, jitter=1e-6, want_grad=True, want_alpha=False, want_grad_x=False):
+        """B independent likelihoods (b2gp_mll_batch): member b is ctx.mll(kind, X[b], yres[b], theta[b]) and, with
+        want_grad_x, d value / d X[b] as ctx.dkl_mll(n_layers=0).  X [B, N, d], yres [B, N], theta [B, d+3] (host arrays).
+        Returns (value [B], grad [B, d+3] or None, alpha [B, N] or None, grad_x [B, N, d] or None, info [B])."""
+        X, yres, theta = _f64(X), _f64(yres), _f64(theta)
+        if X.ndim != 3:
+            raise ValueError(f"X must be [B, N, d], got shape {X.shape}")
+        B, N, d = X.shape
+        if yres.shape != (B, N) or theta.shape != (B, d + 3):
+            raise ValueError(f"yres must be [{B}, {N}] and theta [{B}, {d + 3}], got {yres.shape} and {theta.shape}")
+        if want_grad_x and not want_grad:
+            raise ValueError("want_grad_x needs want_grad")
+        val = np.zeros(B)
+        grad = np.zeros((B, d + 3)) if want_grad else None
+        alpha = np.zeros((B, N)) if want_alpha else None
+        gx = np.zeros((B, N, d)) if want_grad_x else None
+        info = np.zeros(B, dtype=np.int32)
+        self._check(self.lib.b2gp_mll_batch(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(X), N, _ptr(yres), d, B,
+                                            _ptr(theta), float(jitter), 0, _ptr(val), _ptr(grad), _ptr(alpha), _ptr(gx),
+                                            _ptr(info)))
+        return val, grad, alpha, gx, info
 
     def mll_gram(self, K, yres, dKs=(), want_grad=True, want_alpha=False):
         """log N(yres; 0, K) from a caller-supplied K [N, N] (factored as (K + K^T) / 2), the traces

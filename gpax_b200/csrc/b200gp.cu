@@ -21,6 +21,7 @@
 #include "dkl.cuh"
 #include "nngp.cuh"
 #include "bnn.cuh"
+#include "mll_batch.cuh"
 
 // ------------------------------------------------------------------------------------------ helpers
 static inline bool dev_ptrs(unsigned flags) { return (flags & B2GP_FLAG_DEVICE_PTRS) != 0; }
@@ -1924,6 +1925,77 @@ extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N,
     if (grad_z && *info == 0) CUDA_TRY(ctx, cudaMemcpyAsync(grad_z, gz, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
     if (back && *info == 0) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, gz, grad_params));
     return tm.end(ctx, st);
+}
+
+// vExactGP / UIGP: B independent likelihoods (mll_batch.cuh).  N <= B2GP_MLL_BATCH_SMALL_MAX_N: one launch of
+// mll_batch_small_kernel, one CTA per member.  Larger N: mll_impl per member -- the b2gp_mll route and, with grad_x, the b2gp_dkl_mll(n_layers = 0)
+// one (mll_dz_kernel), so each member's outputs are those calls' bits.
+extern "C" int b2gp_mll_batch(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, int64_t B,
+                              const double* theta, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
+                              double* grad_x, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (is_nngp(kind) || f32_io(flags) || dev_ptrs(flags))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_mll_batch", "RBF / Matern / Periodic, host fp64 arrays only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_PERIODIC);
+    ARG_CHECK(ctx, X && yres && theta && value && info && N >= 1 && B >= 1 && d >= 1 && d <= MLL_MAX_D);
+    ARG_CHECK(ctx, !grad_x || grad);
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    const int nth = d + 3;
+    if (N > B2GP_MLL_BATCH_SMALL_MAX_N) {
+        cudaStream_t st = ctx->slots[0].stream;
+        StepTimer tm;
+        RET_IF(tm.begin(ctx, st));
+        if (grad_x) RET_IF(ensure(ctx, ctx->mlp[3], (size_t)N * d * 8));
+        double* gx = (double*)ctx->mlp[3].p;
+        for (int64_t b = 0; b < B; ++b) {
+            RET_IF(mll_impl(ctx, kind, X + b * N * d, N, yres + b * N, d, theta + b * nth, nullptr, jitter, 0, value + b,
+                            grad ? grad + b * nth : nullptr, alpha_out ? alpha_out + b * N : nullptr, nullptr, info + b, nullptr,
+                            grad_x ? gx : nullptr));
+            if (grad_x && info[b] == 0) {
+                CUDA_TRY(ctx, cudaMemcpyAsync(grad_x + b * N * d, gx, (size_t)N * d * 8, cudaMemcpyDeviceToHost, st));
+                CUDA_TRY(ctx, cudaStreamSynchronize(st));
+            }
+        }
+        RET_IF(tm.end(ctx, st));
+    } else {
+        ctx->fcache.valid = false;
+        Slot& sl = ctx->slots[0];
+        cudaStream_t st = sl.stream;
+        CallTimer tm(ctx);
+        RET_IF(tm.begin(st));
+        count_path(ctx, (int)PATH_MLL_BATCH_SMALL);
+        const double *dX, *dy, *dth;
+        RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)(B * N * d) * 8, false, &dX));
+        RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)(B * N) * 8, false, &dy));
+        RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)(B * nth) * 8, false, &dth));
+        // outputs value [B] | grad [B, d+3] | alpha [B, N] | grad_x [B, N, d], then info [B]
+        const int64_t o_g = B, o_a = o_g + B * nth, o_x = o_a + B * N, o_end = o_x + B * N * d;
+        RET_IF(ensure(ctx, ctx->d_out[0], (size_t)o_end * 8 + (size_t)B * sizeof(int)));
+        double* dout = (double*)ctx->d_out[0].p;
+        int* dinfo = (int*)(dout + o_end);
+        static PerDeviceOnce attr;
+        if (attr.need(ctx->device)) {
+            CUDA_TRY(ctx, cudaFuncSetAttribute(mll_batch_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MLLB_SMEM));
+            attr.done(ctx->device);
+        }
+        RET_IF(launch(ctx, st, (unsigned)B, PD_THREADS, MLLB_SMEM, mll_batch_small_kernel, kind, dX, (int)N, dy, d, dth, jitter, dout,
+                      grad ? dout + o_g : nullptr, alpha_out ? dout + o_a : nullptr, grad_x ? dout + o_x : nullptr, dinfo));
+        CUDA_TRY(ctx, cudaMemcpyAsync(value, dout, (size_t)B * 8, cudaMemcpyDeviceToHost, st));
+        if (grad) CUDA_TRY(ctx, cudaMemcpyAsync(grad, dout + o_g, (size_t)(B * nth) * 8, cudaMemcpyDeviceToHost, st));
+        if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, dout + o_a, (size_t)(B * N) * 8, cudaMemcpyDeviceToHost, st));
+        if (grad_x) CUDA_TRY(ctx, cudaMemcpyAsync(grad_x, dout + o_x, (size_t)(B * N * d) * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        RET_IF(tm.end(st, nullptr));
+    }
+    for (int64_t b = 0; b < B; ++b) {   // a member without a factorisation: NaN outputs, whatever the route left there
+        if (info[b] == 0) continue;
+        value[b] = NAN;
+        for (int k = 0; grad && k < nth; ++k) grad[b * nth + k] = NAN;
+        for (int64_t i = 0; alpha_out && i < N; ++i) alpha_out[b * N + i] = NAN;
+        for (int64_t i = 0; grad_x && i < N * d; ++i) grad_x[b * N * d + i] = NAN;
+    }
+    ctx->last.flops = (double)B * N * N * N * (grad ? 1.0 / 3 + 1.0 + 1.0 : 1.0 / 3);
+    return B2GP_OK;
 }
 
 // viMTDKL's likelihood: the forward pass on the N points, z expanded to the N * group GP rows (point-major, one device

@@ -111,6 +111,7 @@ enum PathCounter {
     PATH_POTRF_TALL_FP64,  // factorisations that took potrf_tall on the fp64 DMMA route (ozaki = 0), top-level entries
     PATH_MLL_NNGP_GRAD,    // likelihood gradients that took the NNGP route (mll_nngp_grad_kernel, nngp.cuh), one per call
     PATH_MLL_GRAM_TRACE,   // likelihood gradients reduced against caller-supplied dK (mll_gram_trace_kernel), one per call
+    PATH_MLL_BATCH_SMALL,  // b2gp_mll_batch calls that took the one-launch small route (mll_batch_small_kernel), one per call
     PATH_COUNT
 };
 

@@ -4,13 +4,15 @@ variants.py -- the exact-GP model variants of SURVEY.md section 8f-3 on the same
   MeasuredNoiseGP   gpax/models/mngp.py    measured per-point noise in the likelihood (k + diag(noise), :92-97), noise
                                            extrapolated to new points at predict time (:159-247)
   VarNoiseGP        gpax/models/hskgp.py   heteroskedastic GP: a second (noise) GP over log-variances (:105-206)
-  vExactGP          gpax/models/vgp.py     vector-valued targets: an outer task axis over X, y and the parameters (:125-172)
-  UIGP              gpax/models/uigp.py    uncertain inputs: the training inputs X_prime are a per-draw parameter (:131-150)
+  vExactGP          gpax/models/vgp.py     vector-valued targets: an outer task axis over X, y and the parameters (:55-196)
+  UIGP              gpax/models/uigp.py    uncertain inputs: the training inputs X_prime are a sampled site (:78-150)
 
 Every posterior is one b2gp_posterior_batch call (per-member inputs, per-point noise vectors); likelihoods with a
-noise vector are b2gp_mll_v; samples from covariances modified on the way are b2gp_mvn_sample.  Nothing numerical runs
+noise vector are b2gp_mll_v; the task-batched likelihood of vExactGP and UIGP's likelihood with its input gradient are
+b2gp_mll_batch; samples from covariances modified on the way are b2gp_mvn_sample.  Nothing numerical runs
 on the host except elementwise glue the reference also does in Python (exp of a predicted log-variance, broadcasting).
 """
+import math
 import warnings
 from typing import Callable, Dict, Optional, Tuple
 
@@ -374,6 +376,28 @@ class vExactGP(ExactGP):
                 out["y_sampled"] = out["y_sampled"] + pm[:, :, None, :]
         return out
 
+    def fit(self, rng_key, X, y, num_warmup: int = 2000, num_samples: int = 2000, num_chains: int = 1,
+            chain_method: str = "sequential", progress_bar: bool = True, print_summary: bool = True, device=None,
+            rng_key_predict=None, **kwargs: float) -> None:
+        """vgp.py:55-121 under NUTS: one GP per task, every site with a task axis; each log-joint evaluation is one
+        b2gp_mll_batch call over the B tasks."""
+        from .inference import run_nuts
+        X, y = self._set_data(X, y)
+        self.X_train, self.y_train = X, y
+        lj = _VExactLogJoint(self, kwargs.get("jitter", 1e-6))
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        if print_summary:
+            self._print_summary()
+
+    def predict_in_batches(self, rng_key, X_new, batch_size: int = 100, samples=None, n: int = 1,
+                           filter_nans: bool = False, predict_fn=None, noiseless: bool = False, device=None,
+                           **kwargs: float) -> Tuple[np.ndarray, np.ndarray]:
+        """vgp.py:175-196: X_new [B, P, d] split along the point axis; means [B, P] and samples [S, n, B, P] joined on it."""
+        X_new = self._set_data(X_new)
+        y_pred, y_sampled = self._predict_in_batches(rng_key, X_new, batch_size, 1, samples, n, filter_nans, predict_fn,
+                                                     noiseless, device, **kwargs)
+        return np.concatenate(y_pred, -1), np.concatenate(y_sampled, -1)
+
     def get_mvn_posterior(self, X_new, params: Dict[str, np.ndarray], noiseless: bool = False,
                           **kwargs: float) -> Tuple[np.ndarray, np.ndarray]:
         """vgp.py:147-172: (mean [B, P], cov [B, P, P]) for a single sample of the parameters (each with a task axis)."""
@@ -395,6 +419,84 @@ class vExactGP(ExactGP):
         if filter_nans:
             y_sampled = y_sampled[[i for i in range(S) if not np.isnan(y_sampled[i]).any()]]
         return out["mean"].mean(0), y_sampled
+
+
+class _VExactLogJoint:
+    """log joint of vExactGP.model (vgp.py:55-121) over u = [log k_length (B*d), u k_scale (B), u noise (B)[, log period
+    (B)]].  The B per-task likelihoods and their gradients are one b2gp_mll_batch call.  The priors are wired as
+    vgp.py:101-121 writes them: k_length is always LogNormal(0, 1), `lengthscale_prior_dist` is the prior of k_scale, and
+    `noise_prior_dist` that of noise (vgp.py:92-99)."""
+
+    def __init__(self, model, jitter):
+        if model._fused is None:
+            raise NotImplementedError("vExactGP.fit: callable kernels are not supported; use 'RBF', 'Matern' or 'Periodic'")
+        if model.kernel_prior is not None or model.noise_prior is not None:
+            raise NotImplementedError("vExactGP.fit: kernel_prior / noise_prior programs are not interpreted")
+        if model.mean_fn_prior is not None:
+            raise NotImplementedError("vExactGP.fit: mean_fn_prior (a probabilistic mean function) is not supported")
+        self.m, self.jitter, self.kind = model, float(jitter), model._fused
+        X = np.asarray(model.X_train, dtype=np.float64)
+        self.X = X if X.ndim == 3 else X[..., None]
+        self.B, self.N, self.d = self.X.shape
+        y = np.asarray(model.y_train, dtype=np.float64).reshape(self.B, self.N)
+        if model.mean_fn is not None:
+            y = y - np.asarray(model.mean_fn(self.X), dtype=np.float64).squeeze().reshape(self.B, self.N)
+        self.y = y
+        B, d = self.B, self.d
+        # (site, prior, number of coordinates, theta column(s))
+        self.sites = [("k_length", P.LogNormal(0.0, 1.0), B * d, slice(0, d)),
+                      ("k_scale", model.lengthscale_prior_dist or P.LogNormal(0.0, 1.0), B, d),
+                      ("noise", model.noise_prior_dist or P.LogNormal(0.0, 1.0), B, d + 1)]
+        if self.kind == "Periodic":
+            self.sites.append(("period", P.LogNormal(0.0, 1.0), B, d + 2))
+        for _, pr, _, _ in self.sites:
+            if not isinstance(pr, P.Prior):
+                raise TypeError("priors must be gpax_b200.priors objects (numpyro distributions cannot be used here)")
+        self.off = np.cumsum([0] + [n for _, _, n, _ in self.sites])
+        self.dim = int(self.off[-1])
+        self.n_evals = 0
+
+    def _blocks(self, u):
+        for (name, pr, n, col), a in zip(self.sites, self.off[:-1]):
+            yield name, pr, col, slice(int(a), int(a) + n)
+
+    def theta_of(self, u):
+        th = np.ones((self.B, self.d + 3))
+        for _, pr, col, sl in self._blocks(u):
+            th[:, col] = np.asarray(pr.transform(u[sl]), dtype=np.float64).reshape(th[:, col].shape)
+        return th
+
+    def init_u(self):
+        return np.concatenate([np.full(n, float(pr.inverse(pr.median()))) for _, pr, n, _ in self.sites])
+
+    def __call__(self, u, jacobian):
+        th = self.theta_of(u)
+        val, g, _, _, info = self.m.ctx.mll_batch(self.kind, self.X, self.y, th, self.jitter, True)
+        self.n_evals += 1
+        val = float(val.sum())
+        if (info != 0).any() or not np.isfinite(val):
+            return -np.inf, np.zeros(self.dim)
+        grad = np.zeros(self.dim)
+        for _, pr, col, sl in self._blocks(u):
+            uk = u[sl]
+            t, gk = th[:, col].reshape(-1), g[:, col].reshape(-1)            # g is d/dlog(theta)
+            dt = np.asarray(pr.dtheta_du(uk), dtype=np.float64)
+            val += float(np.sum(pr.log_prob(t)))
+            grad[sl] = gk / t * dt + np.asarray(pr.dlog_prob(t)) * dt
+            if jacobian:
+                val += float(np.sum(pr.log_abs_jac(uk)))
+                grad[sl] += pr.dlog_abs_jac(uk)
+        return val, grad
+
+    def to_dict(self, U):
+        """k_length [S, B, d], k_scale / noise (/ period) [S, B]: the reference's sample shapes"""
+        U = np.atleast_2d(U)
+        th = np.stack([self.theta_of(u) for u in U])
+        d = self.d
+        out = {"k_length": th[:, :, :d], "k_scale": th[:, :, d], "noise": th[:, :, d + 1]}
+        if self.kind == "Periodic":
+            out["period"] = th[:, :, d + 2]
+        return out
 
 
 # ---------------------------------------------------------------------------------------------- UIGP
@@ -447,6 +549,25 @@ class UIGP(ExactGP):
         out = self._uigp_batched(self._set_data(X_new), params, False, noiseless, ("mean", "cov"), **kwargs)
         return out["mean"][0], out["cov"][0]
 
+    def fit(self, rng_key, X, y, num_warmup: int = 2000, num_samples: int = 2000, num_chains: int = 1,
+            chain_method: str = "sequential", progress_bar: bool = True, print_summary: bool = True, device=None,
+            rng_key_predict=None, **kwargs: float) -> None:
+        """uigp.py:78-129 under NUTS: sigma_x, the latent inputs X_prime and the kernel parameters; the likelihood and its
+        gradient w.r.t. X_prime are one b2gp_mll_batch call per evaluation."""
+        from .inference import run_nuts
+        X, y = self._set_data(X, y)
+        self.X_train, self.y_train = X, y
+        lj = _UIGPLogJoint(self, kwargs.get("jitter", 1e-6))
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        if print_summary:
+            self._print_summary()
+
+    def _print_summary(self):
+        """uigp.py:192-194: every site but X_prime"""
+        for k, v in self.get_samples(1).items():
+            if "X_prime" not in k:
+                print(f"{k:>12s}  mean {np.mean(v, axis=(0, 1))}  std {np.std(v, axis=(0, 1))}")
+
     def predict(self, rng_key, X_new, samples: Optional[Dict[str, np.ndarray]] = None, n: int = 1, filter_nans: bool = False,
                 noiseless: bool = False, device=None, **kwargs: float) -> Tuple[np.ndarray, np.ndarray]:
         """gp.py:351-399 over uigp.py:159-174: per draw the test inputs are jittered by the learned sigma_x and averaged
@@ -466,3 +587,97 @@ class UIGP(ExactGP):
         if filter_nans:
             y_sampled = y_sampled[[i for i in range(S) if not np.isnan(y_sampled[i]).any()]]
         return out["mean"].mean(0), y_sampled
+
+
+class _UIGPLogJoint:
+    """log joint of UIGP.model (uigp.py:78-129) over u = [u sigma_x (d), X_prime (N*d), u k_length (d), u k_scale, u noise
+    [, u period]].  X_prime is real-valued and centred: X_prime ~ Normal(X, sigma_x) per feature, sampled as NumPyro does.
+    The likelihood log N(y; 0, K(X_prime) + (noise + jitter) I) with its gradients w.r.t. log theta and X_prime is one
+    b2gp_mll_batch call with B = 1; the Normal term's gradients w.r.t. X_prime and sigma_x are closed-form."""
+
+    def __init__(self, model, jitter):
+        if model._fused is None:
+            raise NotImplementedError("UIGP.fit: callable kernels are not supported; use 'RBF', 'Matern' or 'Periodic'")
+        if model.kernel_prior is not None or model.noise_prior is not None:
+            raise NotImplementedError("UIGP.fit: kernel_prior / noise_prior programs are not interpreted")
+        if model.mean_fn is not None or model.mean_fn_prior is not None:
+            raise NotImplementedError("UIGP.fit: mean functions are not supported (their derivative w.r.t. X_prime is not "
+                                      "available)")
+        self.m, self.jitter, self.kind = model, float(jitter), model._fused
+        self.X, self.y = model._train_arrays()
+        self.N, self.d = self.X.shape
+        d = self.d
+        self.sx_prior = model.sigma_x_prior_dist or P.HalfNormal(0.1)                     # uigp.py:113-116
+        kp = [model.lengthscale_prior_dist or P.LogNormal(0.0, 1.0)] * d + [P.LogNormal(0.0, 1.0)]   # gp.py:235-244
+        kidx = list(range(d + 1))
+        if self.kind == "Periodic":
+            kp.append(P.LogNormal(0.0, 1.0))
+            kidx.append(d + 2)
+        kp.append(model.noise_prior_dist or P.LogNormal(0.0, 1.0))                         # gp.py:222-227
+        kidx.append(d + 1)
+        self.kpriors, self.kidx = kp, kidx
+        for pr in [self.sx_prior] + kp:
+            if not isinstance(pr, P.Prior):
+                raise TypeError("priors must be gpax_b200.priors objects (numpyro distributions cannot be used here)")
+        self.nx = self.N * d
+        self.k0 = d + self.nx                    # first kernel coordinate
+        self.dim = self.k0 + len(kp)
+        self.n_evals = 0
+
+    def _split(self, u):
+        d = self.d
+        sx = np.asarray(self.sx_prior.transform(u[:d]), dtype=np.float64)
+        Xp = u[d:self.k0].reshape(self.N, d)
+        th = np.ones(d + 3)
+        for k, (pr, i) in enumerate(zip(self.kpriors, self.kidx)):
+            th[i] = pr.transform(u[self.k0 + k])
+        return sx, Xp, th
+
+    def init_u(self):
+        """init_to_median: X_prime at X, every other site at its prior median"""
+        pr = self.sx_prior
+        return np.concatenate([np.full(self.d, float(pr.inverse(pr.median()))), self.X.reshape(-1),
+                               [float(p.inverse(p.median())) for p in self.kpriors]])
+
+    def __call__(self, u, jacobian):
+        d = self.d
+        sx, Xp, th = self._split(u)
+        val, g, _, gx, info = self.m.ctx.mll_batch(self.kind, Xp[None], self.y[None], th[None], self.jitter, True, False, True)
+        self.n_evals += 1
+        val = float(val[0])
+        if info[0] != 0 or not np.isfinite(val) or not np.all(np.isfinite(sx)) or not np.all(sx > 0):
+            return -np.inf, np.zeros(self.dim)
+        grad = np.zeros(self.dim)
+        # X_prime ~ Normal(X, sigma_x): value, d/dX_prime, d/dsigma_x
+        r = (Xp - self.X) / sx
+        val += float(np.sum(-0.5 * r * r - np.log(sx) - 0.5 * math.log(2 * math.pi)))
+        grad[d:self.k0] = (gx[0] - r / sx).reshape(-1)
+        dsx = np.sum(r * r, axis=0) / sx - self.N / sx
+        pr, us = self.sx_prior, u[:d]
+        dt = np.asarray(pr.dtheta_du(us), dtype=np.float64)
+        val += float(np.sum(pr.log_prob(sx)))
+        grad[:d] = dsx * dt + np.asarray(pr.dlog_prob(sx)) * dt
+        if jacobian:
+            val += float(np.sum(pr.log_abs_jac(us)))
+            grad[:d] += pr.dlog_abs_jac(us)
+        for k, (pr, i) in enumerate(zip(self.kpriors, self.kidx)):
+            uk, t = u[self.k0 + k], th[i]
+            dt = float(pr.dtheta_du(uk))
+            val += float(pr.log_prob(t))
+            grad[self.k0 + k] = g[0, i] / t * dt + float(pr.dlog_prob(t)) * dt       # g is d/dlog(theta)
+            if jacobian:
+                val += float(pr.log_abs_jac(uk))
+                grad[self.k0 + k] += float(pr.dlog_abs_jac(uk))
+        return val, grad
+
+    def to_dict(self, U):
+        """sigma_x [S, d], X_prime [S, N, d], k_length [S, d], k_scale / noise (/ period) [S]"""
+        U = np.atleast_2d(U)
+        parts = [self._split(u) for u in U]
+        th = np.stack([p[2] for p in parts])
+        d = self.d
+        out = {"sigma_x": np.stack([p[0] for p in parts]), "X_prime": np.stack([p[1] for p in parts]),
+               "k_length": th[:, :d], "k_scale": th[:, d], "noise": th[:, d + 1]}
+        if self.kind == "Periodic":
+            out["period"] = th[:, d + 2]
+        return out

@@ -339,6 +339,25 @@ int  b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D
                   const double* theta, double jitter, unsigned flags,
                   double* value, double* grad_theta, double* grad_params, double* grad_z, int* info);
 
+/* B independent exact-GP likelihoods (the per-task likelihoods of vExactGP.model, gpax/models/vgp.py:55-89, and the one
+ * of UIGP.model with its input gradient, uigp.py:78-107).  X[B,N,d], yres[B,N], theta[B,d+3]: member b's arrays, layouts
+ * as b2gp_mll.  HOST outputs: value[B]; grad[B,d+3] (optional) d value / dlog theta; alpha_out[B,N] (optional) K^{-1} yres;
+ * grad_x[B,N,d] (optional, needs grad) d value / dX; info[B].  Member b returns what b2gp_mll and
+ * b2gp_dkl_mll(n_layers = 0) return on member b.  A member with info[b] != 0 has NaN outputs; the others are unaffected.
+ *   N <= B2GP_MLL_BATCH_SMALL_MAX_N: one launch for the whole batch, one CTA per member that factors, inverts and reduces
+ *            in shared memory (gpax_b200/csrc/mll_batch.cuh); counted by the route counter mll_batch_small.
+ *   larger N: b2gp_mll / b2gp_dkl_mll(n_layers = 0) per member, so each member's outputs are those calls' bits.
+ * Kinds RBF, Matern-5/2, Periodic; d <= 16 (else B2GP_ERR_ARG, as is grad_x without grad).  NNGP kinds, B2GP_FLAG_F32
+ * and B2GP_FLAG_DEVICE_PTRS give B2GP_ERR_UNSUPPORTED.  Identical calls give identical bits.                          */
+/* The largest N that b2gp_mll_batch's one-launch route takes (at most 128, one potrf leaf): the largest N at which it was
+ * measured to win at B = 1 against one b2gp_mll and one b2gp_dkl_mll(n_layers = 0) call for every kind and d in {1, 3}
+ * (1.09-1.67x at N = 96 on an H100 80GB HBM3 at 700 W; at N = 112 RBF d = 1 loses, 0.93x; DESIGN.md 4.13).          */
+#define B2GP_MLL_BATCH_SMALL_MAX_N 96
+
+int  b2gp_mll_batch(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, int64_t B,
+                    const double* theta, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
+                    double* grad_x, int* info);
+
 /* The multi-task counterpart (the likelihood of viMTDKL.model, gpax/models/vi_mtdkl.py): log N(yres; 0, K) with K the
  * LCM covariance of b2gp_mll_multitask on the embedding z = MLP(X), expanded to the GP rows:
  *   X[N, D]                 the network's inputs, N points, without the task column
