@@ -1,5 +1,6 @@
 """Worker of tests/test_gpu_dist_lib.py: one rank of the in-library multi-GPU posterior (env: RANK, WORLD_SIZE, LOCAL_RANK,
-MASTER_ADDR, MASTER_PORT; argv: pr pc N P nb kernel outfile)."""
+MASTER_ADDR, MASTER_PORT; argv: pr pc N P nb kernel outfile [sparse]).  With the optional last argument "sparse" the rank
+also runs the N-sharded sparse posterior (b2gp_dist_sparse_posterior) on its shard of SPARSE_SHAPE."""
 import os
 import sys
 
@@ -19,6 +20,14 @@ def problem(N, P, kernel):
     return X, y, Xn, theta
 
 
+SPARSE_SHAPE = (3000, 200, 150, "Matern")     # N, M, P, kernel of the sharded sparse case
+
+
+def shard(N, rank, world):
+    """rank's share [lo, hi) of N training points; uneven when world does not divide N"""
+    return rank * N // world, (rank + 1) * N // world
+
+
 def main():
     pr, pc, N, P, nb = (int(a) for a in sys.argv[1:6])
     kernel, out = sys.argv[6], sys.argv[7]
@@ -31,8 +40,17 @@ def main():
     res2 = dc.posterior(kernel, X, y, Xn, theta, nb=nb)          # a second call reuses the cached lists / buffers
     assert np.array_equal(res["mean"], res2["mean"]) and np.array_equal(res["var"], res2["var"])
     np.savez(out + f".rank{dc.rank}.npz", mean=res["mean"], var=res["var"], info=res["info"], potrf_ms=res["timing"]["potrf_ms"],
-             ozaki=dc.ctx.get_option("ozaki"))
+             ozaki=dc.ctx.get_option("ozaki"), **(sparse(dc) if sys.argv[8:] == ["sparse"] else {}))
     dc.close()
+
+
+def sparse(dc):
+    from dist_single_worker import sparse_problem
+    N, M, P, kernel = SPARSE_SHAPE
+    X, y, Xu, Xn, theta = sparse_problem(N, M, P, 2, kernel)
+    lo, hi = shard(N, dc.rank, dc.world)
+    res = dc.sparse_posterior(kernel, Xu, X[lo:hi], y[lo:hi], Xn, theta, jitter=1e-5)
+    return {"sparse_mean": res["mean"], "sparse_var": res["var"], "sparse_info": res["info"]}
 
 
 if __name__ == "__main__":

@@ -129,6 +129,30 @@ def test_sharded_sparse_two_ranks():
         np.testing.assert_allclose(var, np.diag(ref_cov), rtol=1e-7, atol=1e-7 * np.abs(ref_cov).max())
 
 
+def test_stand_in_potrf_inv_reports_the_first_bad_pivot_and_exports_the_block_inverses():
+    """the stand-in's potrf_inv reports what b2gp_potrf_inv reports (BlockCyclicGP._panel turns it into k * nb + i)"""
+    import sys
+    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+    from dist_helpers import NumpyOps
+    ops = NumpyOps()
+    rng = np.random.default_rng(4)
+    n = 300
+    G = rng.standard_normal((n, n))
+    A = G @ G.T / n + np.eye(n)
+    L = np.linalg.cholesky(A)
+    a, linv = ops.from_numpy(A), ops.zeros((3 * 128 * 128,))
+    assert ops.potrf_inv(a, linv) == 0
+    np.testing.assert_allclose(np.tril(a.numpy()), L, rtol=1e-12, atol=1e-12)
+    blocks = linv.numpy().reshape(3, 128, 128)
+    for b, (lo, hi) in enumerate([(0, 128), (128, 256), (256, 300)]):
+        np.testing.assert_allclose(blocks[b, :hi - lo, :hi - lo] @ L[lo:hi, lo:hi], np.eye(hi - lo), atol=1e-12)
+    assert not blocks[2, 44:].any() and not blocks[2, :, 44:].any()
+    for j in (0, 127, 200):
+        bad = A.copy()
+        bad[j, j] -= L[j, j] ** 2 + 1.0            # pivot j becomes sqrt(-1); pivots before it are untouched
+        assert ops.potrf_inv(ops.from_numpy(bad), linv) == j + 1
+
+
 def test_single_rank_degenerates_to_local(monkeypatch):
     """world_size 1 (no process group): no collective is issued"""
     import sys
