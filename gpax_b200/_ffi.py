@@ -105,6 +105,9 @@ SIGNATURES = {
     "b2gp_mlp_forward": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_uint]),
     "b2gp_dkl_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint,
                                _dp, _vp, _vp, _vp, _ip]),
+    "b2gp_dkl_posterior_grad": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int, _vp,
+                                          C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp,
+                                          _vp, _vp]),
     "b2gp_mtdkl_mll": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, C.c_int,
                                  _vp, _vp, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _vp, _ip]),
     "b2gp_bnn_loglik": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_double, C.c_uint,
@@ -652,6 +655,41 @@ class Context:
                                           int(act), _ptr(p) if p.size else None, _ptr(theta), float(jitter), flags, C.byref(val),
                                           _ptr(gt), _ptr(gp), _ptr(gz), C.byref(info)))
         return val.value, gt, gp, gz, info.value
+
+    def dkl_posterior_grad(self, kind, X, yres, Xnew, widths, act, params, theta, noiseless=False, jitter=1e-6,
+                           want=("mean", "var", "dmean", "dvar")):
+        """The posterior on z = MLP(X) and its gradients w.r.t. the raw test inputs (b2gp_dkl_posterior_grad).  X [N, D],
+        Xnew [P, D], yres [N] or [S, N]; widths [L] and act as mlp_forward; params [S, P] or [P] in the flat layout;
+        theta [S, d+3] or [d+3].  Host fp64 arrays.  Returns a dict with mean / var [S, P], dmean / dvar [S, P, D] (None
+        where not in `want`) and info [S]."""
+        X, Xnew = _f64(X), _f64(Xnew)
+        N, D = X.shape
+        P = Xnew.shape[0]
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        d = int(w[-1]) if w.size else D
+        p = _f64(params)
+        p = p.reshape(1, -1) if p.ndim == 1 else p
+        theta = _f64(theta).reshape(-1, d + 3)
+        S = theta.shape[0]
+        if w.size and p.shape[0] != S:
+            raise ValueError(f"{p.shape[0]} weight sets for {S} theta rows")
+        if w.size and p.shape[1] != _mlp_nparams(D, w):
+            raise ValueError(f"params rows have {p.shape[1]} entries, the network D={D}, widths={w.tolist()} has "
+                             f"{_mlp_nparams(D, w)}")
+        yres = _f64(yres)
+        stride = 0 if yres.ndim == 1 else yres.shape[1]
+        bits = {"mean": (OUT_MEAN, (S, P)), "var": (OUT_VAR, (S, P)), "dmean": (OUT_DMEAN, (S, P, D)), "dvar": (OUT_DVAR, (S, P, D))}
+        flags, out = 0, {}
+        for name, (bit, shape) in bits.items():
+            out[name] = np.empty(shape) if name in want else None
+            flags |= bit if name in want else 0
+        info = np.zeros(S, dtype=np.int32)
+        self._check(self.lib.b2gp_dkl_posterior_grad(
+            self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(X), N, D, _ptr(yres), stride, _ptr(Xnew), P, int(w.size),
+            _ptr(w), int(act), _ptr(p) if p.size else None, S, p.shape[1], _ptr(theta), int(bool(noiseless)), float(jitter), flags,
+            _ptr(out["mean"]), _ptr(out["var"]), _ptr(out["dmean"]), _ptr(out["dvar"]), info.ctypes.data_as(_vp)))
+        out["info"] = info
+        return out
 
     def mtdkl_mll(self, kind, X, task, yres, widths, act, params, theta, B, noise, group=1, jitter=1e-6, want_params=True,
                   want_z=False):

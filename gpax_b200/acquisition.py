@@ -341,21 +341,27 @@ _DEFAULT_PARAM = {"EI": 0.0, "UCB": 0.25, "POI": 0.01, "UE": 0.0}
 def _analytic_kind(acq_fn, model, kwargs):
     """'EI' / 'UCB' / 'POI' / 'UE' when acq_fn is one of them and the gradient can be had in closed form, else None.
 
-    Only a plain ExactGP or viGP qualifies: their predict() is the exact-GP posterior that b2gp_posterior_grad
-    differentiates.  Every subclass (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, or a user's own) predicts
-    something else, so it takes the finite-difference branch even though it inherits _posterior_grad."""
+    A plain ExactGP or viGP qualifies: their predict() is the exact-GP posterior that b2gp_posterior_grad
+    differentiates.  So do a plain viDKL or DKL with single-channel targets: their predict() is that posterior on the
+    network's embedding, which b2gp_dkl_posterior_grad differentiates w.r.t. the raw inputs.  Every other subclass
+    (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, viMTDKL, iBNN, or a user's own) predicts something else, so
+    it takes the finite-difference branch even though it inherits _posterior_grad; so does a multi-channel viDKL."""
+    from .dkl import DKL, viDKL
     from .gp import ExactGP
     from .vigp import viGP
     kind = {EI: "EI", UCB: "UCB", POI: "POI", UE: "UE"}.get(acq_fn)
-    if kind is None or kwargs.get("penalty") or type(model) not in (ExactGP, viGP):
+    if kind is None or kwargs.get("penalty") or type(model) not in (ExactGP, viGP, viDKL, DKL):
         return None
     if model.mean_fn is not None or model._fused is None:
+        return None
+    if type(model) in (viDKL, DKL) and getattr(model, "y_train", None) is not None and np.ndim(model.y_train) != 1:
         return None
     return kind
 
 
 def _analytic_objective(kind, rng_key, model, d, kwargs):
-    """x [d] -> (acq(x), d acq / dx) through one b2gp_posterior_grad call per evaluation"""
+    """x [d] -> (acq(x), d acq / dx) through one model._posterior_grad call per evaluation (b2gp_posterior_grad, or
+    b2gp_dkl_posterior_grad for viDKL / DKL)"""
     from .gp import _eps_dtype
     kw = dict(kwargs)
     n = int(kw.pop("n", 1))
@@ -387,11 +393,14 @@ def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, 
     maxiter 500 as jaxopt's default) minimises -acq(x) from the best of them, x shaped (1, d) for each evaluation.
 
     The reference differentiates the acquisition w.r.t. x with JAX.  Here EI, UCB, POI and UE without a penalty, on a
-    model with a built-in kernel and no mean function, get the same gradient in closed form from the posterior's own
-    derivatives w.r.t. the test input (b2gp_posterior_grad: one posterior call per evaluation, value and gradient
-    together).  Every other acquisition (KG, Thompson, the q-batch functions, penalties, user callables, mean
-    functions) is handed to L-BFGS-B without a gradient: SciPy then takes finite differences, d + 1 posterior calls per
-    gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
+    plain ExactGP / viGP with a built-in kernel and no mean function, get the same gradient in closed form from the
+    posterior's own derivatives w.r.t. the test input (b2gp_posterior_grad: one posterior call per evaluation, value and
+    gradient together).  On a viDKL or DKL with single-channel targets the posterior's gradient w.r.t. the embedding is
+    pulled back through the network to the raw input (b2gp_dkl_posterior_grad, one call per evaluation); viDKL's single
+    weight set keeps the factor of the training embedding cached across the evaluations.  Every other acquisition (KG,
+    Thompson, the q-batch functions, penalties, user callables), model (mean functions, viMTDKL, multi-channel viDKL,
+    iBNN, other subclasses) is handed to L-BFGS-B without a gradient: SciPy then takes finite differences, d + 1
+    posterior calls per gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
     guess, [d], or a 0-d array in one dimension."""
     from scipy.optimize import minimize
     from .utils import x64_enabled

@@ -1927,6 +1927,123 @@ extern "C" int b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N,
     return tm.end(ctx, st);
 }
 
+// viDKL / DKL's posterior and its gradient w.r.t. the raw test inputs: embed X and Xnew per weight set (mlp_forward_dev,
+// keeping the test points' hidden activations), posterior_impl on the embeddings with the derivative rows, then
+// mlp_input_vjp_kernel pulls d mean / dz and d var / dz back through the network.  The embeddings go through host
+// arrays into posterior_impl, exactly as b2gp_posterior receives b2gp_mlp_forward's output: the S = 1 factor cache keys
+// on those bytes and on nothing else.  Everything besides posterior_impl works in ctx->mlp[0..3] on slot 0's stream
+// (the forward GEMMs have beta = 0, so never the int8 route and its slot scratch) and leaves slot 0's matrix and Ukeep --
+// the cached factor -- alone; unlike b2gp_mlp_forward this entry point therefore keeps the cache valid.
+extern "C" int b2gp_dkl_posterior_grad(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D, const double* yres,
+                                       int64_t yres_stride, const double* Xnew, int64_t P, int n_layers, const int64_t* widths, int act,
+                                       const double* params, int64_t S, int64_t params_stride, const double* theta, int noiseless,
+                                       double jitter, unsigned flags, double* mean, double* var, double* dmean, double* dvar, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (flags & (B2GP_FLAG_F32 | B2GP_FLAG_DEVICE_PTRS | B2GP_OUT_COV | B2GP_OUT_SAMPLE))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_dkl_posterior_grad", "host fp64 arrays, outputs mean / var / dmean / dvar only",
+                       __FILE__, __LINE__);
+    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+    MlpShape sx, sp;
+    RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, sx));
+    ARG_CHECK(ctx, P >= 1 && S >= 1);
+    RET_IF(mlp_shape(ctx, P, D, n_layers, widths, act, sp));
+    ARG_CHECK(ctx, X && Xnew && yres && theta && info && (n_layers == 0 || (params && params_stride >= sx.nparams)));
+    ARG_CHECK(ctx, sx.d <= GRAM_MAX_D && D <= (int64_t)VJP_TILE * 65535);
+    const unsigned outs = flags & (B2GP_OUT_MEAN | B2GP_OUT_VAR | B2GP_OUT_DMEAN | B2GP_OUT_DVAR);
+    if (n_layers == 0)
+        return b2gp_posterior_grad(ctx, kind, X, N, yres, yres_stride, Xnew, P, (int)D, S, theta, noiseless, jitter, outs, mean, var, dmean,
+                                   dvar, info, nullptr);
+    const bool want_dm = outs & B2GP_OUT_DMEAN, want_dv = outs & B2GP_OUT_DVAR;
+    ARG_CHECK(ctx, (!want_dm || dmean) && (!want_dv || dvar));
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const int64_t launches0 = ctx->launches;
+    cudaStream_t st = ctx->slots[0].stream;
+    const int L = n_layers;
+    const int64_t dz = sx.d;
+
+    // ---- 1. inputs: [X | Xnew] in mlp[0], the S weight sets in mlp[1]
+    const int64_t xoff = round_up(N * D, 8);
+    RET_IF(ensure(ctx, ctx->mlp[0], (size_t)(xoff + P * D) * 8));
+    double* dX = (double*)ctx->mlp[0].p;
+    CUDA_TRY(ctx, cudaMemcpyAsync(dX, X, (size_t)N * D * 8, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(dX + xoff, Xnew, (size_t)P * D * 8, cudaMemcpyHostToDevice, st));
+    const double* dP = nullptr;
+    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)((S - 1) * params_stride + sx.nparams) * 8, false, &dP));
+
+    // mlp[3]: the test points' hidden activations H_1 .. H_{L-1} per weight set (the layout mlp_forward_dev gives them) |
+    // the cotangents [R][S, P, dz] | dX [S, R, P, D] | the kernel's G buffers when they do not fit in shared memory
+    const int R = (want_dm ? 1 : 0) + (want_dv ? 1 : 0);
+    int64_t hstride = 0, wmax = 0;
+    for (int l = 0; l + 1 < L; ++l) hstride += round_up(P * sp.out[l], 8);
+    for (int l = 0; l < L; ++l) wmax = std::max(wmax, sp.out[l]);
+    const size_t smem = (size_t)2 * VJP_MAX_R * wmax * 8;
+    const bool use_smem = smem <= VJP_SMEM_MAX;
+    const dim3 grid((unsigned)(S * P), (unsigned)ceil_div(D, (int64_t)VJP_TILE));
+    const int64_t o_cot = round_up(S * hstride, 8), o_dx = o_cot + round_up((int64_t)VJP_MAX_R * S * P * dz, 8);
+    const int64_t o_g = o_dx + round_up((int64_t)S * R * P * D, 8);
+    const int64_t tot = o_g + (use_smem || R == 0 ? 0 : (int64_t)grid.x * grid.y * 2 * VJP_MAX_R * wmax);
+    RET_IF(ensure(ctx, ctx->mlp[3], (size_t)tot * 8));
+    double* work = (double*)ctx->mlp[3].p;
+
+    // ---- embeddings: the training set's and the test points' per weight set, on the host for posterior_impl
+    std::vector<double> Ztr((size_t)S * N * dz), Zn((size_t)S * P * dz);
+    std::vector<double*> H;
+    for (int64_t m = 0; m < S; ++m) {
+        const double* Pm = dP + m * params_stride;
+        RET_IF(mlp_forward_dev(ctx, st, sp, act, dX + xoff, Pm, H));
+        if (hstride > 0 && R > 0)
+            CUDA_TRY(ctx, cudaMemcpyAsync(work + m * hstride, H[1], (size_t)hstride * 8, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(ctx, cudaMemcpyAsync(Zn.data() + m * P * dz, H[L], (size_t)P * dz * 8, cudaMemcpyDeviceToHost, st));
+        RET_IF(mlp_forward_dev(ctx, st, sx, act, dX, Pm, H));
+        CUDA_TRY(ctx, cudaMemcpyAsync(Ztr.data() + m * N * dz, H[L], (size_t)N * dz * 8, cudaMemcpyDeviceToHost, st));
+    }
+    CUDA_TRY(ctx, cudaStreamSynchronize(st));
+
+    // ---- 2. the posterior and its gradient w.r.t. the embedding
+    std::vector<double> dmz(want_dm ? (size_t)S * P * dz : 0), dvz(want_dv ? (size_t)S * P * dz : 0);
+    const int64_t xs = S > 1 ? N * dz : 0, xns = S > 1 ? P * dz : 0;
+    RET_IF(posterior_impl(ctx, kind, Ztr.data(), xs, N, yres, yres_stride, Zn.data(), xns, P, (int)dz, S, theta, nullptr, 0, noiseless,
+                          jitter, outs, mean, var, nullptr, nullptr, 0, nullptr, info, nullptr, want_dm ? dmz.data() : nullptr,
+                          want_dv ? dvz.data() : nullptr));
+
+    // ---- 3. the pull-back to the raw inputs
+    if (R > 0) {
+        double* cot = work + o_cot;
+        double* dXout = work + o_dx;
+        const double* c0 = want_dm ? dmz.data() : dvz.data();
+        CUDA_TRY(ctx, cudaMemcpyAsync(cot, c0, (size_t)S * P * dz * 8, cudaMemcpyHostToDevice, st));
+        if (R > 1) CUDA_TRY(ctx, cudaMemcpyAsync(cot + S * P * dz, dvz.data(), (size_t)S * P * dz * 8, cudaMemcpyHostToDevice, st));
+        VjpNet net{};
+        net.L = L;
+        net.R = R;
+        net.width[0] = D;
+        for (int l = 0; l < L; ++l) {
+            net.width[l + 1] = sp.out[l];
+            net.woff[l] = sp.woff[l];
+        }
+        RET_IF(launch(ctx, st, grid, VJP_THREADS, use_smem ? smem : 0, mlp_input_vjp_kernel, net, dP, params_stride,
+                      (const double*)work, hstride, P, act, (const double*)cot, (const double*)(R > 1 ? cot + S * P * dz : nullptr),
+                      dXout, use_smem ? (double*)nullptr : work + o_g, wmax));
+        // dX [S, R, P, D]: row r of every weight set to its output
+        const size_t row = (size_t)P * D * 8;
+        if (want_dm) CUDA_TRY(ctx, cudaMemcpy2DAsync(dmean, row, dXout, R * row, row, (size_t)S, cudaMemcpyDeviceToHost, st));
+        if (want_dv)
+            CUDA_TRY(ctx, cudaMemcpy2DAsync(dvar, row, dXout + (R - 1) * P * D, R * row, row, (size_t)S, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    }
+    for (int64_t m = 0; m < S; ++m) {
+        if (info[m] == 0) continue;
+        if (outs & B2GP_OUT_MEAN) std::fill(mean + m * P, mean + (m + 1) * P, (double)NAN);
+        if (outs & B2GP_OUT_VAR) std::fill(var + m * P, var + (m + 1) * P, (double)NAN);
+        if (want_dm) std::fill(dmean + m * P * D, dmean + (m + 1) * P * D, (double)NAN);
+        if (want_dv) std::fill(dvar + m * P * D, dvar + (m + 1) * P * D, (double)NAN);
+    }
+    ctx->last.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    ctx->last.launches = ctx->launches - launches0;
+    return B2GP_OK;
+}
+
 // vExactGP / UIGP: B independent likelihoods (mll_batch.cuh).  N <= B2GP_MLL_BATCH_SMALL_MAX_N: one launch of
 // mll_batch_small_kernel, one CTA per member.  Larger N: mll_impl per member -- the b2gp_mll route and, with grad_x, the b2gp_dkl_mll(n_layers = 0)
 // one (mll_dz_kernel), so each member's outputs are those calls' bits.

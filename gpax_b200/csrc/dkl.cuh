@@ -15,6 +15,9 @@
 // columns in tiles: for tiles left of the diagonal the rows of K^{-1} are read, right of it the columns (as rows j,
 // consecutive i) -- both coalesced; every entry of the lower triangle is read twice, N^2 doubles in all.  Each row's sum
 // is accumulated in a fixed order and reduced across the row's threads by a fixed shuffle tree: deterministic, no atomics.
+//
+// mlp_input_vjp_kernel (bottom of the file): the network's vector-Jacobian product w.r.t. its inputs, which turns the
+// posterior's gradient w.r.t. z into the gradient w.r.t. the raw test inputs (b2gp_dkl_posterior_grad, optimize_acq).
 #pragma once
 #include "common.cuh"
 #include "grad.cuh"
@@ -303,4 +306,104 @@ static int launch_transpose(b2gp_ctx* ctx, cudaStream_t st, const double* A, int
     if (rows <= 0 || cols <= 0) return B2GP_OK;
     dim3 grid((unsigned)ceil_div(cols, 32), (unsigned)ceil_div(rows, 32));
     return launch(ctx, st, grid, dim3(32, 8), 0, mlp_transpose_kernel, A, lda, rows, cols, B, ldb);
+}
+
+// ---- mlp_input_vjp_kernel: the network's input vector-Jacobian product for the posterior's gradient w.r.t. raw inputs
+// (b2gp_dkl_posterior_grad).  Per weight set s, test point p and cotangent row r (d mean / dz, d var / dz):
+//     G = cot[r][s, p, :]                                   (the last layer has no activation)
+//     G <- (G W_l^T) * act'(H_l[p])   for l = L-1 .. 1       act' from the stored post-activation: ReLU h > 0, tanh 1 - h^2
+//     dX[s, r, p, :] = G W_0^T
+// mlp_backward_dev's recursion continued one layer further down, for one row instead of N.  One launch covers every
+// (s, p, r): a CTA owns one (s, p) and all R rows, so each weight it reads serves R products.  Entry i of G W_l^T is
+// row i of W_l [in, out] (row-major, coalesced) dotted with G: one warp per row, lanes striding the row in a fixed
+// order, a fixed xor tree across the warp -- identical calls give identical bits.  The G vectors ping-pong between two
+// [R][wmax] buffers: shared memory, or (hidden widths too wide for it) a per-CTA slice of global scratch through the same
+// code.  The bottom layer is tiled over the input dimension D: grid.y CTAs per (s, p) take VJP_TILE input rows each and
+// each recomputes the (small) layers above it, so wide inputs spread over the machine and no buffer grows with D.
+constexpr int VJP_THREADS = 256;
+constexpr int VJP_WARPS = VJP_THREADS / 32;
+constexpr int VJP_TILE = 64;           // input rows of the bottom layer per CTA
+constexpr int VJP_MAX_R = 2;
+constexpr int VJP_MAX_LAYERS = 64;     // mlp_shape's bound
+constexpr size_t VJP_SMEM_MAX = 48 * 1024;   // the G buffers go to global scratch above this (no opt-in needed below it)
+
+struct VjpNet {
+    int L, R;
+    int64_t width[VJP_MAX_LAYERS + 1];   // width[0] = D, width[l + 1] = out_l
+    int64_t woff[VJP_MAX_LAYERS];        // W_l's offset in a weight set's flat parameters
+};
+
+__global__ void __launch_bounds__(VJP_THREADS)
+mlp_input_vjp_kernel(VjpNet net, const double* __restrict__ params, int64_t pstride, const double* __restrict__ Hk, int64_t hstride,
+                     int64_t P, int act, const double* __restrict__ cot0, const double* __restrict__ cot1, double* __restrict__ dX,
+                     double* gscratch, int64_t wmax) {
+    extern __shared__ __align__(16) double vjp_sm[];
+    const int64_t sp = blockIdx.x;                       // s * P + p
+    const int64_t s = sp / P, p = sp % P;
+    const int L = net.L, R = net.R;
+    const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+    double* buf = gscratch ? gscratch + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * 2 * VJP_MAX_R * wmax : vjp_sm;
+    double* G = buf;                                     // G[r * wmax + j]
+    double* Gn = buf + VJP_MAX_R * wmax;
+    const double* Ps = params + s * pstride;
+    const int64_t dz = net.width[L];
+    for (int64_t j = threadIdx.x; j < dz; j += VJP_THREADS) {
+        G[j] = cot0[sp * dz + j];
+        if (R > 1) G[wmax + j] = cot1[sp * dz + j];
+    }
+    // H_l (l >= 1) of this weight set: [P, width[l]] blocks one after the other, each padded to 8 doubles
+    int64_t hoff = 0;
+    for (int l = 1; l + 1 < L; ++l) hoff += (P * net.width[l] + 7) / 8 * 8;
+    for (int l = L - 1; l >= 1; --l) {
+        __syncthreads();
+        const int64_t in = net.width[l], out = net.width[l + 1];
+        const double* W = Ps + net.woff[l];
+        const double* H = Hk + s * hstride + hoff + p * in;
+        for (int64_t i = warp; i < in; i += VJP_WARPS) {
+            double a0 = 0.0, a1 = 0.0;
+            for (int64_t j = lane; j < out; j += 32) {
+                const double w = W[i * out + j];
+                a0 = fma(w, G[j], a0);
+                if (R > 1) a1 = fma(w, G[wmax + j], a1);
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+                a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+            }
+            if (lane == 0) {
+                const double h = H[i];
+                const double m = act == B2GP_ACT_RELU ? (h > 0.0 ? 1.0 : 0.0) : 1.0 - h * h;
+                Gn[i] = a0 * m;
+                if (R > 1) Gn[wmax + i] = a1 * m;
+            }
+        }
+        double* t = G;
+        G = Gn;
+        Gn = t;
+        if (l > 1) hoff -= (P * net.width[l - 1] + 7) / 8 * 8;
+    }
+    __syncthreads();
+    // bottom layer: this CTA's VJP_TILE rows of W_0 [D, width[1]]
+    const int64_t D = net.width[0], out = net.width[1];
+    const double* W = Ps + net.woff[0];
+    const int64_t i1 = D < ((int64_t)blockIdx.y + 1) * VJP_TILE ? D : ((int64_t)blockIdx.y + 1) * VJP_TILE;
+    for (int64_t i = (int64_t)blockIdx.y * VJP_TILE + warp; i < i1; i += VJP_WARPS) {
+        double a0 = 0.0, a1 = 0.0;
+        for (int64_t j = lane; j < out; j += 32) {
+            const double w = W[i * out + j];
+            a0 = fma(w, G[j], a0);
+            if (R > 1) a1 = fma(w, G[wmax + j], a1);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+            a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+        }
+        if (lane == 0) {
+            double* o = dX + ((s * R) * P + p) * D + i;   // dX [S, R, P, D]
+            o[0] = a0;
+            if (R > 1) o[P * D] = a1;
+        }
+    }
 }

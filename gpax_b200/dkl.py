@@ -3,8 +3,9 @@ dkl.py -- deep kernel learning with the reference's surface: `viDKL` (gpax/model
 `DKL` (gpax/models/dkl.py:69-150).  The GP runs on the embedding z = MLP(X).  Every numerical step is on the GPU:
 b2gp_mlp_forward embeds inputs for any number of weight sets, b2gp_dkl_mll evaluates the likelihood log N(y; 0, K(z)) and
 its gradient w.r.t. the kernel hyper-parameters and, through the network's backward pass, every weight and bias, and
-b2gp_posterior predicts on the embeddings.  The optimiser (viDKL: Adam with b1 = 0.5, inference.adam) and the sampler (DKL:
-NUTS, inference.run_nuts) are the host-side loops the other models use.
+b2gp_posterior predicts on the embeddings; b2gp_dkl_posterior_grad gives the posterior's gradient w.r.t. the raw test
+inputs, which acquisition.optimize_acq uses for single-channel viDKL and DKL.  The optimiser (viDKL: Adam with b1 = 0.5,
+inference.adam) and the sampler (DKL: NUTS, inference.run_nuts) are the host-side loops the other models use.
 
 The feature extractor is the reference's default MLP only: viDKL's ReLU MLP 64 -> 64 -> z_dim (vidkl.py:400-412) and DKL's
 tanh MLP over `hidden_dim` (dkl.py:167-177).  Custom haiku modules or callables, `latent_prior` and custom `nn_prior`
@@ -117,6 +118,22 @@ class _MLPModel(ExactGP):
         y = np.asarray(self.y_train, dtype=np.float64)
         return self._posterior(X_new, np.atleast_2d(flat), th, y if y.ndim == 2 else y.reshape(-1), noiseless, want, eps,
                                float(kwargs.get("jitter", 1e-6)))
+
+    def _posterior_grad(self, X_new, params, batched, noiseless, **kwargs):
+        """Per-draw posterior mean [S, P], variance [S, P] and their gradients dmean, dvar [S, P, D] w.r.t. the RAW test
+        inputs (b2gp_dkl_posterior_grad: the posterior gradient on the embedding pulled back through the network), for
+        one (batched=False: viDKL's (nn_params, kernel_params)) or S (batched=True: DKL's draws) parameter sets.  Single-
+        channel targets only; acquisition.optimize_acq calls it for viDKL and DKL."""
+        y = np.asarray(self.y_train, dtype=np.float64)
+        if y.ndim != 1:
+            raise NotImplementedError("posterior gradients of a multi-channel model are not supported")
+        flat, kp = self._split_params(params)
+        th = _theta_rows(kp, self.kernel_dim, batched)
+        X = np.asarray(self._set_data(self.X_train), dtype=np.float64)
+        Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
+        out = self.ctx.dkl_posterior_grad(self._fused, X, y, Xn, self.widths, self.act, np.atleast_2d(flat), th, noiseless,
+                                          float(kwargs.get("jitter", 1e-6)))
+        return out["mean"], out["var"], out["dmean"], out["dvar"]
 
 
 # ------------------------------------------------------------------------------------------------------------ viDKL

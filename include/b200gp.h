@@ -339,6 +339,26 @@ int  b2gp_dkl_mll(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D
                   const double* theta, double jitter, unsigned flags,
                   double* value, double* grad_theta, double* grad_params, double* grad_z, int* info);
 
+/* The posterior of viDKL / DKL and its gradient w.r.t. the RAW test inputs -- what jax.grad of the acquisition w.r.t. x
+ * takes through the network in gpax/acquisition/optimize.py:70-88 (vidkl.py:206-236, dkl.py:113-132 under the grad).
+ * For S weight sets (params + s * params_stride) and theta[S, d+3]:
+ *   1. X[N,D] and Xnew[P,D] are embedded per weight set as b2gp_mlp_forward does (same kernels, same bits);
+ *   2. b2gp_posterior_grad runs on the embeddings (per-draw embeddings when S > 1), dmean_z / dvar_z [S,P,d];
+ *   3. one launch pulls them back through the network: dX = J_MLP(x)^T d/dz (mlp_input_vjp_kernel, dkl.cuh).
+ * Outputs (HOST): mean / var [S,P] and dmean / dvar [S,P,D], any subset by B2GP_OUT_MEAN / VAR / DMEAN / DVAR; info[S].
+ * yres / yres_stride, noiseless and jitter as b2gp_posterior.  mean and var are those of b2gp_posterior on the
+ * b2gp_mlp_forward embeddings, on the same route.  n_layers = 0 is b2gp_posterior_grad on X (D = d).  Kinds RBF,
+ * Matern-5/2, Periodic; host fp64 arrays only: B2GP_FLAG_F32, B2GP_FLAG_DEVICE_PTRS, B2GP_OUT_COV and B2GP_OUT_SAMPLE
+ * give B2GP_ERR_UNSUPPORTED.  S = 1 calls share the factor cache of b2gp_posterior (the key includes the training
+ * embedding's bits): nothing this call runs besides the posterior touches the cached factor, so a repeated call with
+ * the same weights, theta and training set solves against the cached factor.  NaN outputs where info[s] != 0; the other
+ * draws are unaffected.  The pull-back runs in a fixed order: identical calls give identical bits.  b2gp_last_timing
+ * reports the whole call (total_ms its wall time).                                                                     */
+int  b2gp_dkl_posterior_grad(b2gp_ctx* ctx, int kind, const double* X, int64_t N, int64_t D, const double* yres,
+                             int64_t yres_stride, const double* Xnew, int64_t P, int n_layers, const int64_t* widths, int act,
+                             const double* params, int64_t S, int64_t params_stride, const double* theta, int noiseless,
+                             double jitter, unsigned flags, double* mean, double* var, double* dmean, double* dvar, int* info);
+
 /* B independent exact-GP likelihoods (the per-task likelihoods of vExactGP.model, gpax/models/vgp.py:55-89, and the one
  * of UIGP.model with its input gradient, uigp.py:78-107).  X[B,N,d], yres[B,N], theta[B,d+3]: member b's arrays, layouts
  * as b2gp_mll.  HOST outputs: value[B]; grad[B,d+3] (optional) d value / dlog theta; alpha_out[B,N] (optional) K^{-1} yres;
