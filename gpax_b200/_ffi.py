@@ -271,7 +271,7 @@ class Context:
 
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
-             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small")
+             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small", "potrf_tall_batch")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""

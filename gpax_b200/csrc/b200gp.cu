@@ -165,6 +165,11 @@ extern "C" int b2gp_set_option(b2gp_ctx* ctx, const char* key, int64_t value) {
         ctx->tall_min_fp64 = (int)value;
         return B2GP_OK;
     }
+    if (strcmp(key, "draw_batch") == 0) {   // tests and timing only: 0 = the route's group size, 1 = per-draw, B >= 2
+        ARG_CHECK(ctx, value >= 0 && value <= B2GP_MAX_STREAMS);
+        ctx->draw_batch = (int)value;
+        return B2GP_OK;
+    }
     if (strcmp(key, "bnn_fused") == 0) {   // tests and timing only: 0 puts b2gp_bnn_* on the layered route
         ARG_CHECK(ctx, value == 0 || value == 1);
         ctx->bnn_fused = (int)value;
@@ -195,7 +200,7 @@ extern "C" int b2gp_get_option(b2gp_ctx* ctx, const char* key, int64_t* value) {
     } tab[] = {{"streams", ctx->n_streams},       {"ozaki", ctx->ozaki},         {"trsm_strip", ctx->trsm_strip},
                {"oz_cluster", ctx->oz_cluster},   {"enqueue_threads", ctx->enqueue_threads}, {"big_grid", ctx->big_grid},
                {"oz_min_tiles", ctx->oz_min_tiles}, {"panel", ctx->panel},       {"tall_min", ctx->tall_min},
-               {"tall_min_fp64", ctx->tall_min_fp64}, {"bnn_fused", ctx->bnn_fused},
+               {"tall_min_fp64", ctx->tall_min_fp64}, {"bnn_fused", ctx->bnn_fused}, {"draw_batch", ctx->draw_batch},
                {"oz_debug", ctx->oz_debug},       {"tma", ctx->use_tma}};
     for (const auto& e : tab)
         if (strcmp(key, e.key) == 0) {
@@ -752,24 +757,46 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, (size_t)2 * S * sizeof(int), st0));
 
     // ---- per-slot workspaces
-    // the right-hand-side rows [k_pX; y^T] live directly under k_XX in the slot's matrix (potrf_tall solves them with the
-    // factorisation's own panel GEMMs)
+    // Draw region q of ctx->post = [Linv | A | panel scratch], regE doubles apart: the right-hand-side rows [k_pX; y^T]
+    // live directly under k_XX in A (potrf_tall solves them with the factorisation's own panel GEMMs), and consecutive
+    // regions form the batch of a group of draws.  Linv and k_XX do not move with P, so region 0 keeps the cached factor.
     const int64_t ldA = round_up(N, 8), ldV = ldA, ldC = round_up(P, 8);
     const bool need_cov = want_cov || want_samp;
-    for (int q = 0; q < nslots; ++q) {
-        Slot& sl = ctx->slots[q];
-        const size_t needA = (size_t)(N + R) * ldA * 8;
-        if (q == 0 && ctx->fcache.valid && ctx->fcache.N == N && sl.A.p && sl.A.cap < needA) {
-            // slot 0's matrix holds the cached factor and this call brings more test points than the one that made it:
+    const bool tall = use_tall(ctx, N) || use_tall_fp64(ctx, N);
+    const int64_t linvE = linv_bytes(N) / 8, aE = (N + R) * ldA;
+    const int64_t regE = round_up(linvE + aE + (tall ? panel_scratch_elems(ctx, N < ctx->panel ? N : ctx->panel) : 0), 32);
+    // Draws in lock-step groups of B (DESIGN.md 4.2): on the fp64 tall-panel route one batched potrf_tall factors a whole
+    // group, every launch covering all its draws, and `ngs` groups are in flight on as many slot streams.  B = 1 is one
+    // draw per group, every slot its own stream.  Group g runs on slot g % ngs, in regions (g % ngs) B .. + B - 1.  The
+    // route's own choice keeps two groups in flight (one group leaves its diagonal chain exposed, DESIGN.md 5): B = 4
+    // where the slots allow two groups of 4, fewer draws per group below that, and one draw per group (the per-draw
+    // route) where even two groups of 2 do not fit.  S >= 2 rules out the factor cache (S = 1 calls only).
+    int B = 1;
+    if (use_tall_fp64(ctx, N) && S >= 2) {
+        if (ctx->draw_batch == 0) {
+            B = nslots / 2 < B2GP_DRAW_BATCH_DEFAULT ? nslots / 2 : B2GP_DRAW_BATCH_DEFAULT;
+            if (B < 2) B = 1;
+        } else {
+            B = ctx->draw_batch < nslots ? ctx->draw_batch : nslots;
+        }
+    }
+    const int ngs = nslots / B;
+    const int64_t ngroups = ceil_div(S, (int64_t)B);
+    {
+        const size_t need = (size_t)ngs * B * regE * 8;   // the regions in use: ngs groups of B
+        if (ctx->fcache.valid && ctx->fcache.N == N && ctx->post.p && ctx->post.cap < need) {
+            // region 0 holds the cached factor and this call brings more test points than the one that made it:
             // grow the buffer AROUND the factor (a plain ensure() would free it and the reuse below would read garbage)
             DevBuf grown;
-            RET_IF(ensure(ctx, grown, needA));
-            CUDA_TRY(ctx, cudaMemcpyAsync(grown.p, sl.A.p, (size_t)N * ldA * 8, cudaMemcpyDeviceToDevice, st0));
+            RET_IF(ensure(ctx, grown, need));
+            CUDA_TRY(ctx, cudaMemcpyAsync(grown.p, ctx->post.p, (size_t)(linvE + N * ldA) * 8, cudaMemcpyDeviceToDevice, st0));
             CUDA_TRY(ctx, cudaStreamSynchronize(st0));
-            sl.A = std::move(grown);
+            ctx->post = std::move(grown);
         }
-        RET_IF(ensure(ctx, sl.A, needA));
-        RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
+        RET_IF(ensure(ctx, ctx->post, need));
+    }
+    for (int q = 0; q < ngs; ++q) {
+        Slot& sl = ctx->slots[q];
         if (need_cov) RET_IF(ensure(ctx, sl.cov, (size_t)P * ldC * 8));
         if (want_samp) RET_IF(ensure(ctx, sl.LinvC, (size_t)linv_bytes(P)));
         if (!want_mean || ((mt || nngp || gp) && want_var)) RET_IF(ensure(ctx, sl.misc, (size_t)((mt || nngp || gp) ? 2 * P : P) * 8));
@@ -777,7 +804,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     }
     // inputs and the memset of dinfo were queued on st0: order the other streams behind them
     CUDA_TRY(ctx, cudaEventRecord(ctx->inputs_ready, st0));
-    for (int q = 0; q < nslots; ++q)
+    for (int q = 0; q < ngs; ++q)
         if (slot_stream(q) != st0) CUDA_TRY(ctx, cudaStreamWaitEvent(slot_stream(q), ctx->inputs_ready, 0));
 
     // host copy of theta: the accuracy-aware digit-plane count of the int8 path is chosen per draw (oz_auto_planes)
@@ -815,13 +842,14 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     const bool keepU = cacheable && !reuse && use_tall(ctx, N);
     if (keepU) RET_IF(ensure(ctx, ctx->Ukeep, (size_t)ceil_div(N, (int64_t)ctx->panel) * ctx->panel * ctx->panel * 8));
 
-    // One draw's whole pipeline, queued on its slot's stream.  Returns a B2GP_* code.
-    auto enqueue_draw = [&](int64_t s) -> int {
-        Slot& sl = ctx->slots[s % nslots];
-        cudaStream_t st = slot_stream((int)(s % nslots));
-        double* A = (double*)sl.A.p;
+    // One draw's work before (front) or after (!front) the factorisation of its group, queued on the group's stream, in
+    // draw region `reg`.  Returns a B2GP_* code.
+    auto enqueue_draw = [&](int64_t s, int gq, int64_t reg, bool front) -> int {
+        Slot& sl = ctx->slots[gq];
+        cudaStream_t st = sl.stream;
+        double* Linv = (double*)ctx->post.p + reg * regE;
+        double* A = Linv + linvE;
         double* Vt = A + N * ldA;
-        double* Linv = (double*)sl.Linv.p;
         const double* th = dtheta ? dtheta + s * nth : nullptr;
         const double* dXtr_s = dXtr + s * xtr_stride;
         const double* dXnew_s = dXnew + s * xnew_stride;
@@ -829,13 +857,6 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         const bool fused_solve = !reuse && (use_tall(ctx, N) || use_tall_fp64(ctx, N));
         int* inf = dinfo + s;
         int* inf2 = dinfo + S + s;
-        if (timing) {
-            for (int e = 0; e < 6; ++e) sev[s].e[e] = ctx->pool.get();
-            CUDA_TRY(ctx, cudaEventRecord(sev[s].e[0], st));
-        }
-        // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7.
-        // The bound takes k(x, x) = k_scale, which an NNGP kernel does not satisfy: 7 there.
-        sl.oz_planes = (htheta.empty() || noise_vec || mt || nngp) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
         const int T = mt ? mt->T : 0, L = mt ? mt->L : 0, grp = mt ? mt->group : 0;
         const double* Bs = mt ? dmt + s * L * T * T : nullptr;
         const double* ns = mt ? dmt + (size_t)S * L * T * T + s * T : nullptr;
@@ -852,7 +873,18 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             if (G) RET_IF(launch_gram_dx(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, Vt + (P + 1) * ldV, ldV));
             return B2GP_OK;
         };
-        if (!reuse) {
+        if (front) {
+            if (timing) {
+                for (int e = 0; e < 6; ++e) sev[s].e[e] = ctx->pool.get();
+                CUDA_TRY(ctx, cudaEventRecord(sev[s].e[0], st));
+            }
+            // factorisation and P-side solve: 6 or 7 digit planes from the trace bound on cond(K); covariance / sampling: 7.
+            // The bound takes k(x, x) = k_scale, which an NNGP kernel does not satisfy: 7 there.
+            sl.oz_planes = (htheta.empty() || noise_vec || mt || nngp) ? 7 : oz_auto_planes((double)N, htheta[s * nth + d], htheta[s * nth + d + 1], jitter);
+            if (reuse) {
+                if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
+                return B2GP_OK;
+            }
             // k_XX = kernel(X_train, X_train, params, noise, jitter)  (gp.py:269) -- lower triangle only
             if (gp)
                 RET_IF(gram_copyin(ctx, st, sl.Vt, gp->Kxx + s * gp->kxx_stride, N, N, dev, A, ldA));
@@ -863,15 +895,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             if (dnv) RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ldA, N, dnv + s * nv_stride));
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
-            // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
-            if (fused_solve) count_tall_entry(ctx, use_tall(ctx, N));
-            if (fused_solve)
-                RET_IF(potrf_tall(ctx, st, sl, A, ldA, N, R, Linv, inf, 0, keepU ? (double*)ctx->Ukeep.p : nullptr));
-            else
-                RET_IF(potrf_rec(ctx, st, A, ldA, N, Linv, inf, 0));
-        } else {
-            if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
-            CUDA_TRY(ctx, cudaMemcpyAsync(inf, &ctx->fcache.info, sizeof(int), cudaMemcpyHostToDevice, st));
+            return B2GP_OK;
         }
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[2], st));
         if (!fused_solve) RET_IF(rhs_rows());
@@ -949,28 +973,56 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
         if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[5], st));
         return B2GP_OK;
     };
+    // One group: its draws' Gram blocks, the factorisation of all of them (with the P-side solve on the tall-panel route),
+    // then their epilogues.
+    auto enqueue_group = [&](int64_t g) -> int {
+        const int gq = (int)(g % ngs);
+        cudaStream_t st = slot_stream(gq);
+        const int64_t s0 = g * B, reg0 = (int64_t)gq * B;
+        const int nb = (int)(S - s0 < B ? S - s0 : B);
+        double* Linv = (double*)ctx->post.p + reg0 * regE;
+        double* A = Linv + linvE;
+        for (int j = 0; j < nb; ++j) RET_IF(enqueue_draw(s0 + j, gq, reg0 + j, true));
+        if (!reuse) {
+            // factor instead of jnp.linalg.inv (gp.py:271); with the tall-panel scheme also [V^T; w^T] = [k_pX; y^T] L^{-T}
+            if (tall) {
+                for (int j = 0; j < nb; ++j) count_tall_entry(ctx, use_tall(ctx, N));
+                if (nb > 1) count_path(ctx, (int)PATH_POTRF_TALL_BATCH);
+                Batch bt;
+                bt.n = nb;
+                bt.stride = regE;
+                RET_IF(potrf_tall(ctx, st, A + aE, A, ldA, N, R, Linv, dinfo + s0, 0, keepU ? (double*)ctx->Ukeep.p : nullptr, bt));
+            } else {
+                RET_IF(potrf_rec(ctx, st, A, ldA, N, Linv, dinfo + s0, 0));
+            }
+        } else {
+            CUDA_TRY(ctx, cudaMemcpyAsync(dinfo + s0, &ctx->fcache.info, sizeof(int), cudaMemcpyHostToDevice, st));
+        }
+        for (int j = 0; j < nb; ++j) RET_IF(enqueue_draw(s0 + j, gq, reg0 + j, false));
+        return B2GP_OK;
+    };
     // A draw is ~1.4k launches at N=16384 and the driver lets the host run only ~1k launches ahead of the device, so a
     // single queueing thread feeds the slots one after the other and their streams barely overlap.  One host thread
-    // per slot keeps every stream's queue full (the slots share nothing but read-only inputs).
-    if (ctx->enqueue_threads && nslots > 1 && S > nslots && !timing) {
-        std::vector<int> rcs((size_t)nslots, B2GP_OK);
+    // per group slot keeps every stream's queue full (the slots share nothing but read-only inputs).
+    if (ctx->enqueue_threads && ngs > 1 && ngroups > ngs && !timing) {
+        std::vector<int> rcs((size_t)ngs, B2GP_OK);
         std::vector<std::thread> workers;
-        for (int q = 0; q < nslots; ++q)
+        for (int q = 0; q < ngs; ++q)
             workers.emplace_back([&, q] {
                 if (cudaSetDevice(ctx->device) != cudaSuccess) {
                     rcs[q] = B2GP_ERR_CUDA;
                     return;
                 }
-                for (int64_t s = q; s < S && rcs[q] == B2GP_OK; s += nslots) rcs[q] = enqueue_draw(s);
+                for (int64_t g = q; g < ngroups && rcs[q] == B2GP_OK; g += ngs) rcs[q] = enqueue_group(g);
             });
         for (auto& w : workers) w.join();
-        for (int q = 0; q < nslots; ++q) RET_IF(rcs[q]);
+        for (int q = 0; q < ngs; ++q) RET_IF(rcs[q]);
     } else {
-        for (int64_t s = 0; s < S; ++s) RET_IF(enqueue_draw(s));
+        for (int64_t g = 0; g < ngroups; ++g) RET_IF(enqueue_group(g));
     }
     tm.mark_enqueued();
     // ---- join the slots on stream 0
-    for (int q = 0; q < nslots; ++q) {
+    for (int q = 0; q < ngs; ++q) {
         if (slot_stream(q) == st0) continue;
         CUDA_TRY(ctx, cudaEventRecord(ctx->slot_done[q], slot_stream(q)));
         CUDA_TRY(ctx, cudaStreamWaitEvent(st0, ctx->slot_done[q], 0));
@@ -1011,10 +1063,13 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ev_c, ev_d));
     t.d2h_ms = ms;
     if (timing) {
+        // A group's draws queue their Gram blocks one after the other, then the group's factorisation, then their
+        // epilogues: the factorisation is the span from the last draw's Gram end (e1) to the first draw's epilogue start
+        // (e2), counted once, with the group's last draw.  B = 1: each draw's own e1 -> e2.
         for (int64_t s = 0; s < S; ++s) {
             float a = 0, b = 0, c = 0, e = 0, f = 0;
             cudaEventElapsedTime(&a, sev[s].e[0], sev[s].e[1]);
-            cudaEventElapsedTime(&b, sev[s].e[1], sev[s].e[2]);
+            if ((s + 1) % B == 0 || s + 1 == S) cudaEventElapsedTime(&b, sev[s].e[1], sev[s / B * B].e[2]);
             cudaEventElapsedTime(&c, sev[s].e[2], sev[s].e[3]);
             cudaEventElapsedTime(&e, sev[s].e[3], sev[s].e[4]);
             cudaEventElapsedTime(&f, sev[s].e[4], sev[s].e[5]);
@@ -1287,16 +1342,16 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
         noise_h = theta[d + 1];
     }
     const int64_t ldM = round_up(M, 8), ldC = round_up(P, 8);
-    RET_IF(ensure(ctx, sl.A, (size_t)2 * M * ldM * 8));
-    RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)2 * M * ldM * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));
     RET_IF(ensure(ctx, ctx->d_out[0], (size_t)(2 * P + M + 16) * 8));
     if (want_cov && (!dev || f32)) RET_IF(ensure(ctx, ctx->d_out[2], (size_t)P * ldC * 8));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
-    double* Luu = (double*)sl.A.p;
+    double* Luu = slA;
     double* Kmat = Luu + M * ldM;
-    double* LinvU = (double*)sl.Linv.p;
+    double* LinvU = slLinv;
     double* LinvK = LinvU + linv_bytes(M) / 8;
     double* mv = (double*)ctx->d_out[0].p;
     double* vv = mv + P;
@@ -1342,13 +1397,13 @@ extern "C" int b2gp_sparse_partial(b2gp_ctx* ctx, int kind, const double* Xu, in
     const double* dth;
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)(d + 3) * 8, false, &dth));
     const int64_t ldM = round_up(M, 8);
-    RET_IF(ensure(ctx, sl.A, (size_t)2 * M * ldM * 8));
-    RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)2 * M * ldM * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
-    RET_IF(sparse_partial_dev(ctx, sl, kind, Xu, M, Xtr, N, yres, d, dth, jitter, theta[d + 1], (double*)sl.A.p, ldM,
-                              (double*)sl.Linv.p, Kpart, ldk, cpart, dinfo));
+    RET_IF(sparse_partial_dev(ctx, sl, kind, Xu, M, Xtr, N, yres, d, dth, jitter, theta[d + 1], slA, ldM,
+                              slLinv, Kpart, ldk, cpart, dinfo));
     CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, st));
     return tm.end(st, nullptr);
 }
@@ -1372,13 +1427,13 @@ extern "C" int b2gp_sparse_finish(b2gp_ctx* ctx, int kind, const double* Xu, int
     const double* dth;
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)(d + 3) * 8, false, &dth));
     const int64_t ldM = round_up(M, 8);
-    RET_IF(ensure(ctx, sl.A, (size_t)2 * M * ldM * 8));
-    RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)2 * M * ldM * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
-    double* Luu = (double*)sl.A.p;
-    double* LinvU = (double*)sl.Linv.p;
+    double* Luu = slA;
+    double* LinvU = slLinv;
     double* LinvK = LinvU + linv_bytes(M) / 8;
     // Luu is rebuilt here (M^3/3 flops) so that _finish does not depend on ctx state left by _partial
     RET_IF(launch_gram(ctx, st, kind, Xu, M, Xu, M, d, dth, 0.0, jitter, 1, 1, Luu, ldM));
@@ -1560,8 +1615,8 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     }
     const int64_t ld = round_up(N, 8);
     const int64_t tiles = ceil_div(N, MLL_TILE);
-    RET_IF(ensure(ctx, sl.A, (size_t)(N + 1) * ld * 8));
-    RET_IF(ensure(ctx, sl.Linv, (size_t)linv_bytes(N)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)(N + 1) * ld * 8, (size_t)linv_bytes(N), &slA, &slLinv));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     if (mt)
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + L * tiles * tiles * nout + L * nout) * 8));
@@ -1573,8 +1628,8 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
         RET_IF(ensure(ctx, sl.misc, (size_t)(3 * ld + 64 + tiles * tiles * nth) * 8));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 8, st));
-    double* A = (double*)sl.A.p;
-    double* Linv = (double*)sl.Linv.p;
+    double* A = slA;
+    double* Linv = slLinv;
     double* w = A + N * ld;              // y rides under K as a right-hand-side row: L^{-1} y after the factorisation
     double* alpha = (double*)sl.misc.p + ld;   // K^{-1} y
     double* sc = alpha + ld;             // [0] sum log L_ii, [1] |w|^2, [8..8+nth) grad
@@ -1599,7 +1654,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     if (grad || alpha_out) {
         RET_IF(ensure(ctx, sl.cov, (size_t)N * ld * 8));
         double* Bt = (double*)sl.cov.p;  // (L^{-1})^T
-        RET_IF(launch(ctx, st, grid_for(N * N), 256, 0, set_identity_kernel, Bt, ld, N));
+        RET_IF(launch(ctx, st, grid_for(N * N), 256, 0, set_identity_kernel, Bt, ld, N, (int64_t)0));
         RET_IF(trsm_rec(ctx, st, Bt, ld, N, A, ld, N, Linv));
         // alpha = L^{-T} w : alpha_i = <Bt[i,:], w>
         RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Bt, ld, N, w, 1.0, alpha, nullptr));
@@ -2325,8 +2380,8 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
     RET_IF(stage_in(ctx, st, ctx->d_in[5], Xu, (size_t)M * d * 8, dev, &dXu));
     const int64_t ldM = round_up(M, 8), ldN = round_up(N, 8);
-    RET_IF(ensure(ctx, sl.A, (size_t)2 * M * ldM * 8));
-    RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)2 * M * ldM * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     for (int i = 0; i < 6; ++i) RET_IF(ensure(ctx, ctx->eb[i], (size_t)M * ldM * 8));
     RET_IF(ensure(ctx, ctx->eb[6], (size_t)N * ldM * 8));
@@ -2335,9 +2390,9 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(ensure(ctx, ctx->eb[9], (size_t)(4 * ldM + 3 * ldN + 64 + M * (nth + d)) * 8));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
-    double* Luu = (double*)sl.A.p;
+    double* Luu = slA;
     double* Cm = Luu + M * ldM;
-    double* LinvU = (double*)sl.Linv.p;
+    double* LinvU = slLinv;
     double* LinvC = LinvU + linv_bytes(M) / 8;
     double *BtU = (double*)ctx->eb[0].p, *BtC = (double*)ctx->eb[1].p, *Cinv = (double*)ctx->eb[2].p;
     double *T1 = (double*)ctx->eb[3].p, *T2 = (double*)ctx->eb[4].p, *T3 = (double*)ctx->eb[5].p;
@@ -2364,7 +2419,7 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, nullptr, 1.0, nullptr, tmpM));
     RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 3));
     // C^{-1} = BtC BtC^T with BtC = (LC^{-1})^T, beta = C^{-1} b
-    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtC, ldM, M));
+    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtC, ldM, M, (int64_t)0));
     RET_IF(trsm_rec(ctx, st, BtC, ldM, M, Cm, ldM, M, LinvC));
     RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, BtC, ldM, M, u, 1.0, beta, tmpM));
     RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 4));
@@ -2389,7 +2444,7 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(gemm_nt(ctx, st, N, M, M, 1.0, Wt, ldM, Cinv, ldM, 0.0, E, ldM, false));
     RET_IF(launch(ctx, st, grid_for(N * M), 256, 0, elbo_gw_kernel, E, ldM, Wt, ldM, alpha, beta, N, M, coef, noise));
     // dELBO/dKuf^T = (dELBO/dW^T) Luu^{-1}
-    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtU, ldM, M));
+    RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtU, ldM, M, (int64_t)0));
     RET_IF(trsm_rec(ctx, st, BtU, ldM, M, Luu, ldM, M, LinvU));
     RET_IF(gemm_nt(ctx, st, N, M, M, 1.0, E, ldM, BtU, ldM, 0.0, GKuft, ldM, false));
     RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), dim3(32, 8), 0, transpose_kernel, GKuf, ldN, GKuft, ldM,
@@ -2611,7 +2666,7 @@ extern "C" int b2gp_debug_leaf(b2gp_ctx* ctx, int n, double* A_dev, int64_t lda,
         CUDA_TRY(ctx, cudaFuncSetAttribute(potrf_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PD_SMEM));
         attr.done(ctx->device);
     }
-    RET_IF(launch(ctx, st, 1, PD_THREADS, PD_SMEM, potrf_diag_kernel, A_dev, lda, n, linv_dev, dinfo, 0, dprof));
+    RET_IF(launch(ctx, st, 1, PD_THREADS, PD_SMEM, potrf_diag_kernel, A_dev, lda, n, linv_dev, dinfo, 0, dprof, (int64_t)0));
     CUDA_TRY(ctx, cudaMemcpyAsync(prof_host, dprof, 64 * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     return B2GP_OK;
@@ -3019,7 +3074,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
                 RET_IF(gemm_nt(ctx, s, nb, nb, nb, -1.0, E, local ? ld : nb, E, local ? ld : nb, 1.0, D, ld, true));
             }
             RET_IF(potrf_rec(ctx, s, D, ld, nb, (double*)ds->linv.p, dinfo, k * nb));
-            RET_IF(launch(ctx, s, grid_for(nb * nb), 256, 0, set_identity_kernel, U, nb, nb));
+            RET_IF(launch(ctx, s, grid_for(nb * nb), 256, 0, set_identity_kernel, U, nb, nb, (int64_t)0));
             RET_IF(trsm_rec(ctx, s, U, nb, nb, D, ld, nb, (const double*)ds->linv.p));      // U = L_kk^{-T}
             span(PH_POTRF, p0, mark(s));
         }
@@ -3251,16 +3306,16 @@ extern "C" int b2gp_dist_sparse_posterior(b2gp_ctx* ctx, int kind, const double*
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
     RET_IF(stage_in(ctx, st, ctx->d_in[5], Xu, (size_t)M * d * 8, false, &dXu));
     const int64_t ldM = round_up(M, 8);
-    RET_IF(ensure(ctx, sl.A, (size_t)(2 * M * ldM + ldM) * 8));      // Luu | K (+ the M-vector right behind it: one all-reduce)
-    RET_IF(ensure(ctx, sl.Linv, (size_t)2 * linv_bytes(M)));
+    double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
+    RET_IF(slot0_buffers(ctx, (size_t)(2 * M * ldM + ldM) * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));   // Luu | K (+ the M-vector right behind it: one all-reduce)
     RET_IF(ensure(ctx, ctx->d_out[0], (size_t)(2 * P + 16) * 8));
     RET_IF(ensure(ctx, ctx->d_info, 64));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
-    double* Luu = (double*)sl.A.p;
+    double* Luu = slA;
     double* Kmat = Luu + M * ldM;
     double* cvec = Kmat + M * ldM;
-    double* LinvU = (double*)sl.Linv.p;
+    double* LinvU = slLinv;
     double* LinvK = LinvU + linv_bytes(M) / 8;
     double* mv = (double*)ctx->d_out[0].p;
     double* vv = mv + P;

@@ -16,6 +16,7 @@
 
 #define B2GP_MAX_STREAMS 16
 #define B2GP_LEAF 128  // diagonal-block size of the factorisation (one CTA, shared memory)
+#define B2GP_DRAW_BATCH_DEFAULT 4  // draws per lock-step group of a multi-draw posterior on the fp64 tall route (DESIGN.md 4.2)
 
 // SM count of the largest device a context has been created on (grid_for's cap)
 inline std::atomic<int> g_grid_sms{1};
@@ -83,9 +84,9 @@ struct OzWork {
 // One "slot" = the workspace of one posterior draw in flight.
 struct Slot {
     cudaStream_t stream = nullptr;
-    DevBuf A;      // N x ldA      k_XX, then its factor L (lower)
-    DevBuf Vt;     // (P+1) x ldV  rows 0..P-1 = k_pX (gp.py:268), row P = y_res; then V^T, w^T
-    DevBuf Linv;   // nblk x 128 x 128 inverted diagonal blocks of L
+    // k_XX / its factor L and the inverted diagonal blocks of L live in b2gp_ctx::post (posterior draw regions;
+    // slot0_buffers for the single-slot entry points)
+    DevBuf Vt;     // N-row scratch: host Gram staging (b2gp_posterior_gram), W^T (sparse paths), K^{-1} (likelihoods)
     DevBuf cov;    // P x ldC      posterior covariance / its factor
     DevBuf LinvC;  // inverted diagonal blocks of chol(cov)
     DevBuf misc;   // small scratch
@@ -112,6 +113,7 @@ enum PathCounter {
     PATH_MLL_NNGP_GRAD,    // likelihood gradients that took the NNGP route (mll_nngp_grad_kernel, nngp.cuh), one per call
     PATH_MLL_GRAM_TRACE,   // likelihood gradients reduced against caller-supplied dK (mll_gram_trace_kernel), one per call
     PATH_MLL_BATCH_SMALL,  // b2gp_mll_batch calls that took the one-launch small route (mll_batch_small_kernel), one per call
+    PATH_POTRF_TALL_BATCH, // lock-step groups of posterior draws factored by one batched potrf_tall (fp64 route), one per group
     PATH_COUNT
 };
 
@@ -132,6 +134,9 @@ struct b2gp_ctx {
     int tall_min_fp64 = 8192;  // smallest N factored by potrf_tall on the fp64 route (ozaki = 0); DESIGN.md 4.2
     int oz_debug = 0;  // see OzArgs::debug (0 in production)
     int bnn_fused = 1;     // 1: BNN entry points take the fused kernels where the network fits (bnn.cuh); 0: layered route
+    // draws of a multi-draw posterior factored in lock-step by one batched potrf_tall (fp64 tall route): 0 picks the
+    // group size from the route (DESIGN.md 4.2), 1 factors every draw on its own, B >= 2 groups of B
+    int draw_batch = 0;
     size_t smem_optin = 0; // opt-in dynamic shared memory per block of the device
     // 0: fp64 DMMA only; 6 / 7: large rank-k updates through the int8 wgmma path with that many base-256 digit planes
     // (46 / 54 bits per operand); -1: 6 or 7 per factorisation from a bound on cond(K), see oz_auto_planes().
@@ -168,6 +173,10 @@ struct b2gp_ctx {
         int64_t U_nb = 0;      // > 0: `Ukeep` holds the explicit inverses of the factor's U_nb-wide diagonal blocks (potrf_tall)
     } fcache;
     DevBuf Ukeep;
+    // posterior workspaces of the slots, one allocation: draw region q = [Linv | A (k_XX, then the rows under it) | panel
+    // scratch] at q * stride doubles, so that a group of consecutive regions is one batch (posterior_impl); its front is
+    // also slot 0's matrix for the other entry points (slot0_buffers)
+    DevBuf post;
     int64_t cache_hits = 0;
     std::unique_ptr<DistState> dist;   // created by b2gp_dist_init, released by b2gp_dist_finalize or with the context
     b2gp_timing last{};                // what b2gp_last_timing reports
@@ -250,6 +259,18 @@ static inline int ensure(b2gp_ctx* ctx, DevBuf& b, size_t bytes) {
     return B2GP_OK;
 }
 
+// Slot 0's factor matrix (a_bytes) and inverted diagonal blocks (linv_bytes) for the entry points that work on slot 0
+// alone (likelihoods, sparse and distributed paths): the front of ctx->post, where the posterior keeps its draw
+// regions, so that a fit and a prediction on one context share one allocation.  This overwrites a cached posterior
+// factor: the callers drop the factor cache first.
+static inline int slot0_buffers(b2gp_ctx* ctx, size_t a_bytes, size_t linv_bytes, double** A, double** Linv) {
+    const size_t lb = (linv_bytes + 255) & ~(size_t)255;
+    RET_IF(ensure(ctx, ctx->post, lb + a_bytes));
+    *Linv = (double*)ctx->post.p;
+    *A = (double*)((char*)ctx->post.p + lb);
+    return B2GP_OK;
+}
+
 // cudaFuncSetAttribute is per device: a process may hold contexts on several devices (Context(device=1) next to
 // the default one), so the "already opted in to large dynamic shared memory" memo is a bit per device.
 struct PerDeviceOnce {
@@ -280,6 +301,14 @@ static inline int oz_auto_planes(double n, double k_scale, double noise, double 
     if (!(floor_ > 0.0) || !(k_scale > 0.0)) return 7;
     return (n * k_scale + floor_) / floor_ <= 1e6 ? 6 : 7;
 }
+
+// The draws of a batched launch: `n` draws whose operands (matrix, inverted diagonal blocks, panel scratch) all sit
+// `stride` doubles apart; a kernel takes its draw from grid y or z (or its persistent tile index) and offsets every
+// pointer by draw * stride.  n = 1 is one draw (stride unused).
+struct Batch {
+    int n = 1;
+    int64_t stride = 0;
+};
 
 // CTAs a persistent (one CTA per SM) kernel should launch
 static inline int persist_sms(b2gp_ctx* ctx) { return (ctx->big_grid > 0 && ctx->big_grid < ctx->sm_count) ? ctx->big_grid : ctx->sm_count; }

@@ -19,6 +19,14 @@
 #pragma once
 #include "common.cuh"
 
+// the draw offset of a kernel whose draw is blockIdx.y (Batch), re-read at every use rather than held in registers:
+// several configurations run at their register cap
+__device__ __forceinline__ int64_t ctaid_y_offset(int64_t bstride) {
+    unsigned y;
+    asm volatile("mov.u32 %0, %%ctaid.y;" : "=r"(y));
+    return (int64_t)y * bstride;
+}
+
 struct GemmArgs {
     int m, n, k;
     const double* A;
@@ -32,6 +40,8 @@ struct GemmArgs {
     int tiles_m, tiles_n;
     int tile_base = 0;  // first 128x128 tile index covered by this launch (tail launches, see gemm_tma.cuh)
     int sub = 0;        // 1: blockIdx.x enumerates the four 64x64 quarters of 128x128 tiles tile_base, tile_base+1, ...
+    int64_t bstride = 0;  // doubles between the draws' A, B and C (Batch); a draw is blockIdx.y, or tile / tpd for persistent and sub launches
+    int tpd = 0;          // tiles per draw of the persistent kernel and of the sub launches (tiles numbered over the whole batch)
 };
 
 constexpr int GEMM_BK = 16;
@@ -174,8 +184,14 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
     extern __shared__ __align__(16) double smem[];
 
     int ti, tj;
+    int64_t soff = 0;   // the draw offset of a sub launch (tiles numbered over the batch); others take it from blockIdx.y
     {
-        const int x = p.sub ? p.tile_base + (int)(blockIdx.x >> 2) : p.tile_base + (int)blockIdx.x;
+        int x = p.sub ? p.tile_base + (int)(blockIdx.x >> 2) : p.tile_base + (int)blockIdx.x;
+        if (!KTRI && p.sub) {
+            const int draw = x / p.tpd;
+            x -= draw * p.tpd;
+            soff = (int64_t)draw * p.bstride;
+        }
         const int tn = p.sub ? (p.tiles_n + 1) / 2 : p.tiles_n;   // tile columns in units of the indexed (128-wide) tiles
         if (p.lower_only) {
             int t = (int)((sqrt(8.0 * (double)x + 1.0) - 1.0) * 0.5);
@@ -197,7 +213,7 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
     const int warp = tid >> 5, lane = tid & 31;
     const int wm = warp / WARPS_N, wn = warp % WARPS_N;
     const int g = lane >> 2, t4 = lane & 3;
-    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && ((p.bstride & 1) == 0);
 
     for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
     if (KTRI) {
@@ -220,8 +236,8 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
         if (s < KT) {
             double* As = smem + s * STAGE_ELEMS;
             double* Bs = As + BM * GEMM_LDS;
-            load_slice<BM, NT, ALIGNED>(As, p.A, p.lda, p.m, p.k, row0, s * GEMM_BK, tid);
-            load_slice<BN, NT, ALIGNED>(Bs, p.B, p.ldb, p.n, p.k, col0, s * GEMM_BK, tid);
+            load_slice<BM, NT, ALIGNED>(As, p.A + soff + ctaid_y_offset(p.bstride), p.lda, p.m, p.k, row0, s * GEMM_BK, tid);
+            load_slice<BN, NT, ALIGNED>(Bs, p.B + soff + ctaid_y_offset(p.bstride), p.ldb, p.n, p.k, col0, s * GEMM_BK, tid);
         }
         cp_async_commit();
     }
@@ -234,8 +250,8 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
             if (nk < KT) {
                 double* As = smem + (nk % STAGES) * STAGE_ELEMS;
                 double* Bs = As + BM * GEMM_LDS;
-                load_slice<BM, NT, ALIGNED>(As, p.A, p.lda, p.m, p.k, row0, nk * GEMM_BK, tid);
-                load_slice<BN, NT, ALIGNED>(Bs, p.B, p.ldb, p.n, p.k, col0, nk * GEMM_BK, tid);
+                load_slice<BM, NT, ALIGNED>(As, p.A + soff + ctaid_y_offset(p.bstride), p.lda, p.m, p.k, row0, nk * GEMM_BK, tid);
+                load_slice<BN, NT, ALIGNED>(Bs, p.B + soff + ctaid_y_offset(p.bstride), p.ldb, p.n, p.k, col0, nk * GEMM_BK, tid);
             }
             cp_async_commit();
         }
@@ -256,7 +272,7 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
             const int c = col0 + wn * WTN + j * 8 + t4 * 2;
             if (c >= p.n) continue;
             if (p.lower_only && c > r) continue;
-            double* dst = p.C + (int64_t)r * p.ldc + c;
+            double* dst = p.C + soff + ctaid_y_offset(p.bstride) + (int64_t)r * p.ldc + c;
             const bool two = (c + 1 < p.n) && !(p.lower_only && c + 1 > r);
             double v0 = p.alpha * acc[i][j][0], v1 = p.alpha * acc[i][j][1];
             if (two && vec_ok) {
@@ -280,10 +296,10 @@ __global__ void __launch_bounds__(WARPS_M* WARPS_N * 32, MINB) gemm_nt_kernel(co
 }
 
 template <int BM, int BN, int WARPS_M, int WARPS_N, int STAGES, int MINB, bool KTRI = false>
-static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
+static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb = 1) {
     constexpr int smem_bytes = STAGES * (BM + BN) * GEMM_LDS * (int)sizeof(double);
     const bool aligned = ((a.lda & 1) == 0) && ((a.ldb & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.A) & 15) == 0) &&
-                         ((reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
+                         ((reinterpret_cast<uintptr_t>(a.B) & 15) == 0) && ((a.bstride & 1) == 0);
     a.tiles_m = (a.m + BM - 1) / BM;
     a.tiles_n = (a.n + BN - 1) / BN;
     int64_t grid = KTRI ? (int64_t)a.tiles_m : a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
@@ -295,21 +311,24 @@ static int launch_gemm_cfg(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
         attr_set[aligned ? 1 : 0].done(ctx->device);
     }
-    return launch(ctx, PATH_GEMM_NT, st, (unsigned)grid, WARPS_M * WARPS_N * 32, smem_bytes, kern, a);
+    return launch(ctx, PATH_GEMM_NT, st, dim3((unsigned)grid, (unsigned)nb), WARPS_M * WARPS_N * 32, smem_bytes, kern, a);
 }
 
-static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);        // gemm_tma.cuh
-static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a);  // gemm_tma.cuh
+static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb);        // gemm_tma.cuh
+static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb);  // gemm_tma.cuh
 static int ozaki_dispatch(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
                           const double* B, int64_t ldb, double* C, int64_t ldc, bool lower_only, bool overwrite, bool transB,
                           bool ktri);  // ozaki.cuh
 
 // C = beta*C + alpha*A*B^T.  lower_only requires a square C (m == n) whose diagonal is the matrix
 // diagonal.  `inplace_rows` marks the B <- B*Linv^T use where C aliases A: that is only safe with a
-// single column tile (n <= 128), which the 128-wide configuration guarantees.
+// single column tile (n <= 128), which the 128-wide configuration guarantees.  `bt`: the same product on bt.n draws, the
+// tile counts of the choices below taken over the whole batch (every configuration gives the same bits).
 static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                   int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, bool lower_only) {
+                   int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, bool lower_only,
+                   const Batch& bt = {}) {
     if (m <= 0 || n <= 0) return B2GP_OK;
+    const int nb = bt.n;
     GemmArgs a;
     a.m = (int)m;
     a.n = (int)n;
@@ -323,11 +342,13 @@ static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t
     a.alpha = alpha;
     a.beta = beta;
     a.lower_only = lower_only ? 1 : 0;
+    a.bstride = bt.stride;
     if (lower_only && m < n) return set_err(ctx, B2GP_ERR_ARG, "gemm_nt", "lower_only needs m >= n", __FILE__, __LINE__);
     // Large rank-k updates C += alpha A B^T (the trailing updates of the factorisation and of the blocked solves) go
     // to the int8 wgmma path when it is enabled (ozaki.cuh).  It needs beta == 1, k within the int32 accumulation bound, enough 128x64 tiles to
     // fill the machine twice, and operands distinct from C (the in-place solve keeps the DMMA kernel).
     if (ctx->ozaki && beta == 1.0 && k >= 512 && C != A && C != B) {
+        if (nb != 1) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "gemm_nt", "the int8 route takes one draw", __FILE__, __LINE__);
         const int64_t tm = ceil_div(m, 128), tn = ceil_div(n, 64), sq = ceil_div(n, 128);
         const int64_t toz = lower_only ? sq * (sq + 1) + (tm - sq) * tn : tm * tn;   // lower triangle (+ the rows below it)
         if (toz >= ctx->oz_min_tiles) {
@@ -337,35 +358,35 @@ static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t
     }
     if (lower_only && m > n) {
         // trapezoid on the fp64 kernels (their lower-only tile maps are square): the square part, then the rows below it
-        RET_IF(gemm_nt(ctx, st, n, n, k, alpha, A, lda, B, ldb, beta, C, ldc, true));
-        return gemm_nt(ctx, st, m - n, n, k, alpha, A + n * lda, lda, B, ldb, beta, C + n * ldc, ldc, false);
+        RET_IF(gemm_nt(ctx, st, n, n, k, alpha, A, lda, B, ldb, beta, C, ldc, true, bt));
+        return gemm_nt(ctx, st, m - n, n, k, alpha, A + n * lda, lda, B, ldb, beta, C + n * ldc, ldc, false, bt);
     }
     // Tile choice.  A 128x128 tile keeps one SM busy for at least 128*128*k/128 cycles (DMMA.16x8x4: 128 fp64
     // FMA/clk/SM measured on the H100), i.e. ~8 us per k = 128, however few tiles there are; when the 128x128 grid would leave most of
     // the SMs idle, spend the same flops on more, smaller tiles.  The in-place triangular-solve
     // use (C aliases A, n <= 128) needs a single column tile, which all three configurations give.
     const int64_t tm128 = ceil_div(m, 128), tn128 = ceil_div(n, 128);
-    const int64_t t128 = lower_only ? tm128 * (tm128 + 1) / 2 : tm128 * tn128;
+    const int64_t t128 = (lower_only ? tm128 * (tm128 + 1) / 2 : tm128 * tn128) * nb;
     if (t128 >= 112) {
         if (ctx->use_tma) {
-            const int rc = gemm_tma_dispatch(ctx, st, a);
+            const int rc = gemm_tma_dispatch(ctx, st, a, nb);
             if (rc != B2GP_ERR_UNSUPPORTED) return rc;
         }
         // measured (tools/gemm_cfg.py): 3 stages beat 4 at large k; 16 warps (4 per SM sub-partition) beat 8 at small k
-        if (k <= 1024) return launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a);
-        return launch_gemm_cfg<128, 128, 2, 4, 3, 1>(ctx, st, a);
+        if (k <= 1024) return launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a, nb);
+        return launch_gemm_cfg<128, 128, 2, 4, 3, 1>(ctx, st, a, nb);
     }
     if (lower_only) {
         // square tiles only for the triangular tile map
-        return launch_gemm_cfg<64, 64, 2, 4, 4, 2>(ctx, st, a);
+        return launch_gemm_cfg<64, 64, 2, 4, 4, 2>(ctx, st, a, nb);
     }
     // latency-bound regime: minimise (waves) x (time of one tile), in units of a 32x128 tile; the 128x128 kernel holds
     // one CTA per SM, the two smaller ones two
-    const int64_t t64 = ceil_div(m, 64) * tn128, t32 = ceil_div(m, 32) * tn128;
+    const int64_t t64 = ceil_div(m, 64) * tn128 * nb, t32 = ceil_div(m, 32) * tn128 * nb;
     const int64_t c128 = ceil_div(t128, ctx->sm_count) * 4, c64 = ceil_div(t64, 2 * ctx->sm_count) * 2, c32 = ceil_div(t32, 2 * ctx->sm_count) * 1;
-    if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2>(ctx, st, a);
-    if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2>(ctx, st, a);
-    return launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a);
+    if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2>(ctx, st, a, nb);
+    if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2>(ctx, st, a, nb);
+    return launch_gemm_cfg<128, 128, 4, 4, 3, 1>(ctx, st, a, nb);
 }
 
 // The fp64 panel solve of the tall-panel factorisation (potrf.cuh, panel_solve_all_rows):  rows (m x n) <- rows Li^T,
@@ -375,8 +396,9 @@ static int gemm_nt(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t
 // scratch and copying back.  128-row strips on the persistent TMA kernel from 16 strips up: with draws in flight on other
 // streams the SMs a thin solve leaves idle run their work (DESIGN.md 4.3); below that gemm_nt's latency rule in row strips.
 static int gemm_panel_solve(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, double* rows, int64_t ldr, const double* Li,
-                            int64_t ldli) {
+                            int64_t ldli, const Batch& bt = {}) {
     if (m <= 0 || n <= 0) return B2GP_OK;
+    const int nb = bt.n;
     GemmArgs a;
     a.m = (int)m;
     a.n = (int)n;
@@ -390,17 +412,18 @@ static int gemm_panel_solve(b2gp_ctx* ctx, cudaStream_t st, int64_t m, int64_t n
     a.alpha = 1.0;
     a.beta = 0.0;
     a.lower_only = 0;
-    const int64_t tm128 = ceil_div(m, 128);
+    a.bstride = bt.stride;
+    const int64_t tm128 = ceil_div(m, 128) * nb;   // strips over the batch
     if (tm128 >= 16) {
         if (ctx->use_tma) {
-            const int rc = gemm_tma_panel_dispatch(ctx, st, a);
+            const int rc = gemm_tma_panel_dispatch(ctx, st, a, nb);
             if (rc != B2GP_ERR_UNSUPPORTED) return rc;
         }
-        return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a);
+        return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a, nb);
     }
-    const int64_t c128 = ceil_div(tm128, ctx->sm_count) * 4, c64 = ceil_div(ceil_div(m, 64), 2 * ctx->sm_count) * 2,
-                  c32 = ceil_div(ceil_div(m, 32), 2 * ctx->sm_count);
-    if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2, true>(ctx, st, a);
-    if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2, true>(ctx, st, a);
-    return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a);
+    const int64_t c128 = ceil_div(tm128, ctx->sm_count) * 4, c64 = ceil_div(ceil_div(m, 64) * nb, 2 * ctx->sm_count) * 2,
+                  c32 = ceil_div(ceil_div(m, 32) * nb, 2 * ctx->sm_count);
+    if (c32 <= c64 && c32 <= c128) return launch_gemm_cfg<32, 128, 1, 8, 3, 2, true>(ctx, st, a, nb);
+    if (c64 <= c128) return launch_gemm_cfg<64, 128, 2, 4, 3, 2, true>(ctx, st, a, nb);
+    return launch_gemm_cfg<128, 128, 4, 4, 3, 1, true>(ctx, st, a, nb);
 }

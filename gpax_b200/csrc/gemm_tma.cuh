@@ -40,15 +40,18 @@ static PFN_tmapEncodeTiled tmap_encoder() {
     return fn;
 }
 
-// 2-D fp64 map of a row-major [rows x cols] matrix with leading dimension ld: box = 16 columns x 128 rows
-static bool make_tmap(CUtensorMap* map, const double* base, int64_t rows, int64_t cols, int64_t ld) {
+// 3-D fp64 map of `draws` row-major [rows x cols] matrices with leading dimension ld, `dstride` doubles apart (Batch):
+// dimensions {cols, rows, draws}, box = 16 columns x 128 rows x 1 draw
+static bool make_tmap(CUtensorMap* map, const double* base, int64_t rows, int64_t cols, int64_t ld, int draws, int64_t dstride) {
     PFN_tmapEncodeTiled enc = tmap_encoder();
     if (!enc) return false;
-    cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)ld * 8};
-    cuuint32_t box[2] = {16, 128};
-    cuuint32_t estr[2] = {1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, (void*)base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    if (draws == 1) dstride = rows * ld;   // unused, but the encoder wants a legal stride
+    if ((dstride & 1) != 0) return false;
+    cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)draws};
+    cuuint64_t gstride[2] = {(cuuint64_t)ld * 8, (cuuint64_t)dstride * 8};
+    cuuint32_t box[3] = {16, 128, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, (void*)base, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -80,6 +83,12 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
                  "l"(map), "r"(bar), "r"(c0), "r"(c1)
                  : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+                     smem_dst),
+                 "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
 
 __device__ __forceinline__ void tile_of(int x, int lower_only, int tiles_n, int& ti, int& tj) {
     if (lower_only) {
@@ -99,6 +108,7 @@ __device__ __forceinline__ void tile_of(int x, int lower_only, int tiles_n, int&
 // column tile j stops at k = 128 (j + 1) (B is zero beyond its diagonal block).  Tile j reads columns < 128 (j + 1) and
 // writes columns 128 j .. 128 j + 127, so nothing a later tile of the strip reads has been overwritten, and no other CTA
 // touches the strip's rows.  Right to left is also heaviest first.
+// Batched (Batch): the persistent loop runs over (draw, tile) pairs, tile x of the batch being tile x % tpd of draw x / tpd.
 template <int STAGES, int KSUB, bool KTRI = false>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GemmArgs p, int num_tiles) {
@@ -125,8 +135,9 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
         // ------------------------------------------------------------ producer
         if (lane == 0) {
             uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
+            for (int x = blockIdx.x; x < num_tiles; x += gridDim.x)
             for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
+                const int draw = x / p.tpd, tile = x - draw * p.tpd;
                 int ti, tj;
                 if (KTRI) {
                     ti = tile;
@@ -144,8 +155,8 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                     const uint32_t st = base + s * STAGE_BYTES;
 #pragma unroll
                     for (int sub = 0; sub < KSUB; ++sub) {
-                        tma_load_2d(st + sub * TG_SUB_BYTES, &mapA, kt * BK + 16 * sub, row0, full);
-                        tma_load_2d(st + (KSUB + sub) * TG_SUB_BYTES, &mapB, kt * BK + 16 * sub, col0, full);
+                        tma_load_3d(st + sub * TG_SUB_BYTES, &mapA, kt * BK + 16 * sub, row0, draw, full);
+                        tma_load_3d(st + (KSUB + sub) * TG_SUB_BYTES, &mapB, kt * BK + 16 * sub, col0, draw, full);
                     }
                 }
             }
@@ -164,19 +175,16 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
     const uint32_t x0 = ((uint32_t)((t4 >> 1) ^ g) << 4) + ((uint32_t)(t4 & 1) << 3);
     const uint32_t a_row = (uint32_t)(wm * 64 + g) * 128u + x0;
     const uint32_t b_row = (uint32_t)(wn * 32 + g) * 128u + x0;
-    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+    const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);   // bstride is even (make_tmap)
 
     uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
+    for (int x = blockIdx.x; x < num_tiles; x += gridDim.x)
     for (int jj = 0; jj < (KTRI ? p.tiles_n : 1); ++jj) {
-        int ti, tj;
-        if (KTRI) {
-            ti = tile;
-            tj = p.tiles_n - 1 - jj;
-        } else {
-            tile_of(tile, p.lower_only, p.tiles_n, ti, tj);
-        }
-        const int row0 = ti * TG_BM, col0 = tj * TG_BN;
+        int ti = 0, tj;
+        if (KTRI)
+            tj = p.tiles_n - 1 - jj;   // the strip (ti) is found after the k loop, see the epilogue
+        else
+            tile_of(x % p.tpd, p.lower_only, p.tiles_n, ti, tj);
         const int KTt = KTRI ? min(KT, ((tj + 1) * TG_BN + BK - 1) / BK) : KT;   // the producer's count
         double acc[MI][NI][2];
 #pragma unroll
@@ -199,7 +207,13 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
             if (lane == 0) mbar_arrive(bars + 8 * (STAGES + s));
         }
 
-        // epilogue (identical to gemm_nt_kernel); the panel solve (KTRI) has alpha = 1, beta = 0 and no lower-only map
+        // epilogue (identical to gemm_nt_kernel); the panel solve (KTRI) has alpha = 1, beta = 0 and no lower-only map.
+        // The draw (and the KTRI strip) is derived here from the shuffled tile index rather than kept live across the
+        // k loop: the accumulators leave no register to spare.
+        const int xs = __shfl_sync(0xffffffffu, x, 0), draw = xs / p.tpd;
+        if (KTRI) ti = xs - draw * p.tpd;
+        const int row0 = ti * TG_BM, col0 = tj * TG_BN;
+        double* const Cd = p.C + (int64_t)draw * p.bstride;
 #pragma unroll
         for (int i = 0; i < MI; ++i) {
             const int r = row0 + wm * 64 + i * 8 + g;
@@ -209,7 +223,7 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
                 const int c = col0 + wn * 32 + j * 8 + t4 * 2;
                 if (c >= p.n) continue;
                 if (!KTRI && p.lower_only && c > r) continue;
-                double* dst = p.C + (int64_t)r * p.ldc + c;
+                double* dst = Cd + (int64_t)r * p.ldc + c;
                 const bool two = (c + 1 < p.n) && !(!KTRI && p.lower_only && c + 1 > r);
                 double v0 = p.alpha * acc[i][j][0], v1 = p.alpha * acc[i][j][1];
                 if (two && vec_ok) {
@@ -234,17 +248,20 @@ gemm_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant_
 
 // returns B2GP_ERR_UNSUPPORTED when the operands do not meet TMA's alignment rules (caller falls back)
 template <int STAGES, int KSUB, bool KTRI = false>
-static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
+static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb = 1) {
     constexpr int smem_bytes = STAGES * 2 * KSUB * TG_SUB_BYTES + 2 * STAGES * 8 + 1024;
     const bool ok = ((a.lda & 1) == 0) && ((a.ldb & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.A) & 15) == 0) &&
                     ((reinterpret_cast<uintptr_t>(a.B) & 15) == 0);
     if (!ok) return B2GP_ERR_UNSUPPORTED;
     CUtensorMap mapA, mapB;
-    if (!make_tmap(&mapA, a.A, a.m, a.k, a.lda) || !make_tmap(&mapB, a.B, a.n, a.k, a.ldb)) return B2GP_ERR_UNSUPPORTED;
+    if (!make_tmap(&mapA, a.A, a.m, a.k, a.lda, nb, a.bstride) || !make_tmap(&mapB, a.B, a.n, a.k, a.ldb, nb, a.bstride))
+        return B2GP_ERR_UNSUPPORTED;
     a.tiles_m = (a.m + TG_BM - 1) / TG_BM;
     a.tiles_n = (a.n + TG_BN - 1) / TG_BN;
-    const int64_t tiles = KTRI ? (int64_t)a.tiles_m : a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
-    if (tiles <= 0) return B2GP_OK;
+    const int64_t tpd = KTRI ? (int64_t)a.tiles_m : a.lower_only ? (int64_t)a.tiles_m * (a.tiles_m + 1) / 2 : (int64_t)a.tiles_m * a.tiles_n;
+    if (tpd <= 0) return B2GP_OK;
+    a.tpd = (int)tpd;
+    const int64_t tiles = tpd * nb;
     static PerDeviceOnce attr;
     if (attr.need(ctx->device)) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(gemm_tma_kernel<STAGES, KSUB, KTRI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -279,5 +296,7 @@ static int launch_gemm_tma(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) {
     return B2GP_OK;
 }
 
-static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) { return launch_gemm_tma<3, 2>(ctx, st, a); }
-static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a) { return launch_gemm_tma<3, 2, true>(ctx, st, a); }
+static int gemm_tma_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb) { return launch_gemm_tma<3, 2>(ctx, st, a, nb); }
+static int gemm_tma_panel_dispatch(b2gp_ctx* ctx, cudaStream_t st, GemmArgs& a, int nb) {
+    return launch_gemm_tma<3, 2, true>(ctx, st, a, nb);
+}

@@ -17,7 +17,9 @@ constexpr int MLL_MAX_D = 16;
 constexpr int MLL_TILE = 64;
 constexpr int MLL_THREADS = 256;
 
-__global__ void set_identity_kernel(double* B, int64_t ld, int64_t n) {
+// B = I (n x n); the draw of a Batch is blockIdx.y (matrices `bstride` doubles apart)
+__global__ void set_identity_kernel(double* B, int64_t ld, int64_t n, int64_t bstride) {
+    B += (int64_t)blockIdx.y * bstride;
     const int64_t total = n * n;
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = idx / n, j = idx % n;
