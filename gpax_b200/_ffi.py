@@ -99,6 +99,8 @@ SIGNATURES = {
     "b2gp_mll": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _ip]),
     "b2gp_mll_batch": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, C.c_int64, _vp, C.c_double, C.c_uint, _vp, _vp, _vp,
                                  _vp, _vp]),
+    "b2gp_mll_draws": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_int, C.c_int64, _vp, C.c_double, C.c_uint, _vp,
+                                 _vp, _vp, _vp]),
     "b2gp_mll_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int64, C.c_uint, _dp, _vp, _vp, _ip]),
     "b2gp_posterior_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
                                       C.c_int64, C.c_uint, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
@@ -271,7 +273,8 @@ class Context:
 
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
-             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small", "potrf_tall_batch")
+             "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small", "potrf_tall_batch",
+             "mll_draws_batch")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""
@@ -496,6 +499,25 @@ class Context:
                                             _ptr(theta), float(jitter), 0, _ptr(val), _ptr(grad), _ptr(alpha), _ptr(gx),
                                             _ptr(info)))
         return val, grad, alpha, gx, info
+
+    def mll_draws(self, kind, X, yres, theta, jitter=1e-6, want_grad=True, want_alpha=False):
+        """S likelihoods on one X in lock-step (b2gp_mll_draws): draw s is ctx.mll(kind, X, yres[s], theta[s]) bit for bit.
+        X [N, d]; yres [N] (shared) or [S, N]; theta [S, d+3] (host arrays).
+        Returns (value [S], grad [S, d+3] or None, alpha [S, N] or None, info [S])."""
+        X, yres = _f64(X), _f64(yres)
+        N, d = X.shape
+        theta = _f64(theta).reshape(-1, d + 3)
+        S = theta.shape[0]
+        if yres.shape not in ((N,), (S, N)):
+            raise ValueError(f"yres must be [{N}] or [{S}, {N}], got shape {yres.shape}")
+        val = np.zeros(S)
+        grad = np.zeros((S, d + 3)) if want_grad else None
+        alpha = np.zeros((S, N)) if want_alpha else None
+        info = np.zeros(S, dtype=np.int32)
+        self._check(self.lib.b2gp_mll_draws(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(X), N, _ptr(yres),
+                                            0 if yres.ndim == 1 else N, d, S, _ptr(theta), float(jitter), 0, _ptr(val),
+                                            _ptr(grad), _ptr(alpha), _ptr(info)))
+        return val, grad, alpha, info
 
     def mll_gram(self, K, yres, dKs=(), want_grad=True, want_alpha=False):
         """log N(yres; 0, K) from a caller-supplied K [N, N] (factored as (K + K^T) / 2), the traces

@@ -176,7 +176,7 @@ class BNN:
         self.X_train, self.y_train = X, y
         lj = BNNLogJoint(self, X, y, seed_from_key(rng_key))
         try:
-            res = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+            res = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         finally:
             lj.close()
         by_chain = res.get_samples(group_by_chain=True)

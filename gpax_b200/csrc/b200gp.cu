@@ -2,6 +2,7 @@
 // reference lines each entry point replaces).  Host code here only orchestrates: workspace, streams,
 // the order of kernel launches.  No torch, no JAX, no CPU fallback: every numerical result is
 // produced by the sm_90a kernels in gram.cuh / gemm_dmma.cuh / potrf.cuh / posterior.cuh.
+#include <algorithm>
 #include <chrono>
 #include <thread>
 
@@ -1191,12 +1192,17 @@ __global__ void transpose_kernel(double* __restrict__ out, int64_t ldo, const do
     }
 }
 
-// generic <row, w> and |row|^2 reductions: dot[p] = <R[p,:], w>, nrm[p] = |R[p,:]|^2
+// generic <row, w> and |row|^2 reductions: dot[p] = <R[p,:], w>, nrm[p] = |R[p,:]|^2.  The draw of a batch is blockIdx.z
+// (R and the non-null w, dot and nrm `bstride` doubles apart).
 __global__ void __launch_bounds__(RD_THREADS)
 rowdot2_kernel(const double* __restrict__ R, int64_t ld, int64_t len, const double* __restrict__ w, double wscale,
-               double* __restrict__ dot, double* __restrict__ nrm) {
+               double* __restrict__ dot, double* __restrict__ nrm, int64_t bstride) {
     __shared__ double red1[RD_THREADS / 32], red2[RD_THREADS / 32];
-    const double* row = R + (int64_t)blockIdx.x * ld;
+    const int64_t boff = (int64_t)blockIdx.z * bstride;
+    if (w) w += boff;
+    if (dot) dot += boff;
+    if (nrm) nrm += boff;
+    const double* row = R + boff + (int64_t)blockIdx.x * ld;
     double s1 = 0.0, s2 = 0.0;
     for (int64_t k = threadIdx.x; k < len; k += RD_THREADS) {
         const double v = row[k];
@@ -1268,7 +1274,7 @@ static int sparse_partial_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* d
     CUDA_TRY(ctx, cudaMemsetAsync(Kpart, 0, (size_t)M * ldk * 8, st));
     RET_IF(gemm_nt(ctx, st, M, M, N, 1.0 / noise_h, W, ldN, W, ldN, 1.0, Kpart, ldk, true));
     // W D^{-1} y  (sparse_gp.py:203-204)
-    return launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, dy, 1.0 / noise_h, cpart, nullptr);
+    return launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, dy, 1.0 / noise_h, cpart, nullptr, (int64_t)0);
 }
 
 // Posterior from the summed statistics: K = Ksum + I, L = chol(K), then sparse_gp.py:206-217.
@@ -1293,8 +1299,8 @@ static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dX
     CUDA_TRY(ctx, cudaMemcpyAsync(R + P * ldM, cvec, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
     RET_IF(trsm_rec(ctx, st, R, ldM, P + 1, Kmat, ldk, M, LinvK));
     // mean = (L^{-1} c)^T (L^{-1} Ws)  (sparse_gp.py:213)
-    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, R, ldM, M, R + P * ldM, 1.0, dmean, rv));
-    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, Wst, ldM, M, nullptr, 1.0, nullptr, qv));
+    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, R, ldM, M, R + P * ldM, 1.0, dmean, rv, (int64_t)0));
+    RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, Wst, ldM, M, nullptr, 1.0, nullptr, qv, (int64_t)0));
     RET_IF(launch(ctx, st, grid_for(P), 256, 0, sparse_var_kernel, want_var ? dvar : nullptr, dmean, qv, rv, P, kind, d, dth,
                   noiseless ? 0.0 : 1.0, jitter, dinfo, dinfo + 1));
     if (want_cov) {
@@ -1493,7 +1499,7 @@ extern "C" int b2gp_rowdot(b2gp_ctx* ctx, int64_t rows, int64_t len, const doubl
         RET_IF(ensure(ctx, ctx->slots[0].misc, (size_t)(2 * rows + 16) * 8));
         double* t1 = (double*)ctx->slots[0].misc.p;
         double* t2 = t1 + rows;
-        RET_IF(launch(ctx, st, (unsigned)rows, RD_THREADS, 0, rowdot2_kernel, R, ldr, len, w, scale, dot ? t1 : nullptr, nrm ? t2 : nullptr));
+        RET_IF(launch(ctx, st, (unsigned)rows, RD_THREADS, 0, rowdot2_kernel, R, ldr, len, w, scale, dot ? t1 : nullptr, nrm ? t2 : nullptr, (int64_t)0));
         if (dot) RET_IF(launch(ctx, st, grid_for(rows), 256, 0, accumulate_kernel, dot, t1, rows, accumulate));
         if (nrm) RET_IF(launch(ctx, st, grid_for(rows), 256, 0, accumulate_kernel, nrm, t2, rows, accumulate));
     }
@@ -1566,7 +1572,7 @@ static int mll_gram_trace(b2gp_ctx* ctx, cudaStream_t st, const GramMll& gm, boo
             CUDA_TRY(ctx, cudaEventRecord(red[b], st));
         }
     }
-    return launch(ctx, st, (unsigned)p, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, (int64_t)tiles * tiles, p, gout);
+    return launch(ctx, st, (unsigned)p, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, (int64_t)tiles * tiles, p, gout, (int64_t)0);
 }
 
 static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int d, const double* theta,
@@ -1649,15 +1655,15 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     // the scheme of the posterior (tall-panel int8 at N >= 2048); w = L^{-1} y falls out of the panel solves instead of
     // a separate chain of 2 N / 128 strip launches for one row
     RET_IF(potrf_auto(ctx, st, A, ld, N, 1, Linv, dinfo));
-    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, A, ld, N, sc));
-    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, w, ld, N, nullptr, 1.0, nullptr, sc + 1));
+    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, A, ld, N, sc, (int64_t)0));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, w, ld, N, nullptr, 1.0, nullptr, sc + 1, (int64_t)0));
     if (grad || alpha_out) {
         RET_IF(ensure(ctx, sl.cov, (size_t)N * ld * 8));
         double* Bt = (double*)sl.cov.p;  // (L^{-1})^T
         RET_IF(launch(ctx, st, grid_for(N * N), 256, 0, set_identity_kernel, Bt, ld, N, (int64_t)0));
         RET_IF(trsm_rec(ctx, st, Bt, ld, N, A, ld, N, Linv));
         // alpha = L^{-T} w : alpha_i = <Bt[i,:], w>
-        RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Bt, ld, N, w, 1.0, alpha, nullptr));
+        RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Bt, ld, N, w, 1.0, alpha, nullptr, (int64_t)0));
         if (grad) {
             RET_IF(ensure(ctx, sl.Vt, (size_t)N * ld * 8));
             double* Kinv = (double*)sl.Vt.p;
@@ -1673,13 +1679,13 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                               d, kind, T, L, mt->group, dth, (const double*)dmt, (const double*)(dmt + (size_t)L * T * T), jitter,
                               (const double*)alpha, (const double*)Kinv, ld, partial));
                 RET_IF(launch(ctx, st, (unsigned)(L * nout), MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial,
-                              tiles * tiles, nout, gmt));
+                              tiles * tiles, nout, gmt, (int64_t)0));
                 if (grad_x_dev)   // d value / d X [N, d] of the LCM covariance on the device (dkl.cuh)
                     RET_IF(launch(ctx, st, (unsigned)ceil_div(N, DZ_ROWS), DZ_THREADS, 0, mll_lcm_dz_kernel, kind, dX, dtask, N, d, T, L,
                                   dth, (const double*)dmt, (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
             } else if (nngp) {   // nngp.cuh: self-chains, the cross chain per pair, fixed-order sums -> sc[8..11) = (var_w, noise, var_b)
                 double* chain = partial + tiles * tiles * 3;
-                if (depth > 0) RET_IF(launch(ctx, st, (unsigned)ceil_div(N, (int64_t)256), 256, 0, nngp_self_kernel, dX, N, d, kind, dth, chain));
+                if (depth > 0) RET_IF(launch(ctx, st, (unsigned)ceil_div(N, (int64_t)256), 256, 0, nngp_self_kernel, dX, N, d, kind, dth, chain, (int64_t)0));
                 static PerDeviceOnce attr;
                 if (attr.need(ctx->device)) {
                     CUDA_TRY(ctx, cudaFuncSetAttribute(mll_nngp_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1689,12 +1695,12 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                 count_path(ctx, (int)PATH_MLL_NNGP_GRAD);
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), NNGP_THREADS, nngp_grad_smem(d, depth),
                               mll_nngp_grad_kernel, dX, N, d, kind, dth, (const double*)chain, (const double*)alpha, (const double*)Kinv, ld,
-                              partial));
-                RET_IF(launch(ctx, st, 3u, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, tiles * tiles, 3, sc + 8));
+                              partial, (int64_t)0));
+                RET_IF(launch(ctx, st, 3u, MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, tiles * tiles, 3, sc + 8, (int64_t)0));
             } else {
                 RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind, dth, alpha, Kinv,
-                              ld, partial));
-                RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8));
+                              ld, partial, (int64_t)0));
+                RET_IF(launch(ctx, st, 1, 32, 0, mll_finish_kernel, partial, tiles * tiles, nth, sc + 8, (int64_t)0));
                 if (grad_x_dev)   // d value / d X [N, d] on the device (dkl.cuh)
                     RET_IF(launch(ctx, st, (unsigned)ceil_div(N, DZ_ROWS), DZ_THREADS, 0, mll_dz_kernel, kind, dX, N, d, dth,
                                   (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
@@ -1787,6 +1793,177 @@ extern "C" int b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, cons
         memcpy(grad_B, g.data() + (size_t)L * (d + 2), (size_t)L * T * T * 8);
         memcpy(grad_noise, g.data() + (size_t)L * (d + 2) + (size_t)L * T * T, (size_t)T * 8);
     }
+    return B2GP_OK;
+}
+
+// ------------------------------------------------------------------------------------------ likelihood draws in lock-step
+// b2gp_mll_draws: S likelihoods on one X, draw s with theta[s] and its own or the shared yres, run as mll_impl's sequence in
+// groups of B draws.  Each draw of a group owns one region of ctx->post, `stride` doubles apart, so that a single Batch
+// offsets every operand of a launch:
+//   [Linv | A ((N + 1) x ld: K, y under it) | Bt = L^{-T} | K^{-1} | panel scratch (tall route) | alpha | sc | partials |
+//    NNGP self-chains | theta]
+// sc is mll_impl's: [0] sum log L_ii, [1] |L^{-1} y|^2, [8 ..) the gradient.  Every kernel computes a draw exactly as its
+// unbatched launch does, and every factorisation kernel gives the same bits whatever the batch (gemm_nt, potrf.cuh), so
+// draw s returns b2gp_mll's bits on (theta[s], yres[s]) whatever S and the grouping.
+
+// p[draw][0, n) = 0; the draw is blockIdx.y (`bstride` doubles apart)
+__global__ void zero_batch_kernel(double* p, int64_t n, int64_t bstride) {
+    p += (int64_t)blockIdx.y * bstride;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = 0.0;
+}
+
+constexpr int MLLD_HS = 8 + MLL_MAX_D + 3;   // the scalars of sc read back per draw (mll_impl's hsc)
+
+extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
+                              int64_t S, const double* theta, double jitter, unsigned flags, double* value, double* grad,
+                              double* alpha_out, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags) || dev_ptrs(flags))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_mll_draws", "host fp64 arrays only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
+    const bool nngp = is_nngp(kind);
+    ARG_CHECK(ctx, X && yres && theta && value && info);
+    ARG_CHECK(ctx, N >= 1 && S >= 1 && d >= 1 && d <= (nngp ? GRAM_MAX_D : MLL_MAX_D));
+    ARG_CHECK(ctx, yres_stride == 0 || yres_stride >= N);
+    const int nth = d + 3;
+    int depth = 0;   // NNGP: the deepest draw sizes the self-chains and the gradient kernel's shared memory
+    if (nngp)
+        for (int64_t s = 0; s < S; ++s) {
+            RET_IF(nngp_check_depth(ctx, "b2gp_mll_draws", theta[s * nth]));
+            depth = std::max(depth, (int)theta[s * nth]);
+        }
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;   // the regions overwrite slot 0's matrix
+    Slot& sl = ctx->slots[0];
+    cudaStream_t st = sl.stream;
+    CallTimer tm(ctx);
+    RET_IF(tm.begin(st));
+    const int64_t ld = round_up(N, 8), tiles = ceil_div(N, MLL_TILE);
+    const bool want_k = grad || alpha_out;
+    const bool tall64 = use_tall_fp64(ctx, N);
+    // region layout (doubles)
+    const int64_t oA = linv_bytes(N) / 8, oBt = oA + (N + 1) * ld, oKi = oBt + (want_k ? N * ld : 0), oScr = oKi + (grad ? N * ld : 0);
+    const int64_t oAl = oScr + (tall64 ? panel_scratch_elems(ctx, N < ctx->panel ? N : ctx->panel) : 0), oSc = oAl + ld, oPart = oSc + 64;
+    const int64_t oCh = oPart + tiles * tiles * (nngp ? 3 : nth), oTh = oCh + (nngp ? N * depth * 3 : 0);
+    const int64_t stride = round_up(oTh + nth, 32);
+    // Group size.  The int8 route takes one draw at a time (its GEMMs and panel solves refuse batches).  Otherwise
+    // draw_batch: 0 = as many draws as an eighth of the device memory holds, 1 = one draw per group, B >= 2 = groups of B.
+    int64_t B = 1;
+    if (ctx->ozaki == 0) {
+        if (ctx->draw_batch == 0)
+            B = std::max<int64_t>(1, (int64_t)(ctx->mem_bytes / 8) / (stride * 8));
+        else
+            B = ctx->draw_batch;
+        B = std::min<int64_t>(std::min<int64_t>(B, S), 65535);
+    }
+    // inputs: X, theta [S, nth] and yres as [S, N] (a shared yres repeated), staged once
+    std::vector<double> yrows;
+    const double* ysrc = yres;
+    if (yres_stride != N) {
+        yrows.resize((size_t)S * N);
+        for (int64_t s = 0; s < S; ++s) memcpy(yrows.data() + s * N, yres + s * yres_stride, (size_t)N * 8);
+        ysrc = yrows.data();
+    }
+    const double *dX, *dy, *dth;
+    RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, false, &dX));
+    RET_IF(stage_in(ctx, st, ctx->d_in[1], ysrc, (size_t)S * N * 8, false, &dy));
+    RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)S * nth * 8, false, &dth));
+    RET_IF(ensure(ctx, ctx->d_info, (size_t)S * sizeof(int)));
+    RET_IF(ensure(ctx, ctx->d_out[0], (size_t)S * MLLD_HS * 8));
+    if (alpha_out) RET_IF(ensure(ctx, ctx->d_out[1], (size_t)S * N * 8));
+    RET_IF(ensure(ctx, ctx->post, (size_t)B * stride * 8));
+    int* dinfo = (int*)ctx->d_info.p;
+    double* dsc = (double*)ctx->d_out[0].p;
+    double* dal = (double*)ctx->d_out[1].p;
+    CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, (size_t)S * sizeof(int), st));
+    double* R = (double*)ctx->post.p;
+    double *Linv = R, *A = R + oA, *w = A + N * ld, *Bt = R + oBt, *Kinv = R + oKi, *scr = R + oScr, *alpha = R + oAl, *sc = R + oSc,
+           *partial = R + oPart, *chain = R + oCh, *th = R + oTh;
+    if (nngp && grad) {
+        static PerDeviceOnce attr;
+        if (attr.need(ctx->device)) {
+            CUDA_TRY(ctx, cudaFuncSetAttribute(mll_nngp_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)nngp_grad_smem(GRAM_MAX_D, NNGP_MAX_DEPTH)));
+            attr.done(ctx->device);
+        }
+    }
+    for (int64_t g0 = 0; g0 < S; g0 += B) {
+        const int nb = (int)std::min<int64_t>(B, S - g0);
+        const Batch bt{nb, stride};
+        const unsigned z = (unsigned)nb;
+        count_path(ctx, (int)PATH_MLL_DRAWS_BATCH);
+        RET_IF(launch(ctx, st, grid_for((int64_t)nb * nth), 256, 0, copy2d_kernel, th, stride, dth + g0 * nth, (int64_t)nth, (int64_t)nb,
+                      (int64_t)nth));
+        RET_IF(launch(ctx, st, grid_for((int64_t)nb * N), 256, 0, copy2d_kernel, w, stride, dy + g0 * N, N, (int64_t)nb, N));
+        RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, th, 1.0, jitter, 1, 1, A, ld, bt));
+        if (nb == 1) {   // mll_impl's factorisation on every route
+            RET_IF(potrf_auto(ctx, st, A, ld, N, 1, Linv, dinfo + g0));
+        } else if (tall64) {   // fp64 tall-panel route, y riding below K
+            for (int j = 0; j < nb; ++j) count_tall_entry(ctx, false);
+            RET_IF(potrf_tall(ctx, st, scr, A, ld, N, 1, Linv, dinfo + g0, 0, nullptr, bt));
+        } else {
+            RET_IF(potrf_rec(ctx, st, A, ld, N, Linv, dinfo + g0, 0, bt));
+            RET_IF(trsm_rec(ctx, st, w, ld, 1, A, ld, N, Linv, true, bt));
+        }
+        RET_IF(launch(ctx, st, dim3(1, 1, z), 256, 0, logdiag_kernel, (const double*)A, ld, N, sc, stride));
+        RET_IF(launch(ctx, st, dim3(1, 1, z), RD_THREADS, 0, rowdot2_kernel, (const double*)w, ld, N, (const double*)nullptr, 1.0,
+                      (double*)nullptr, sc + 1, stride));
+        if (want_k) {
+            RET_IF(launch(ctx, st, dim3(grid_for(N * N), z), 256, 0, set_identity_kernel, Bt, ld, N, stride));
+            RET_IF(trsm_rec(ctx, st, Bt, ld, N, A, ld, N, Linv, true, bt));
+            RET_IF(launch(ctx, st, dim3((unsigned)N, 1, z), RD_THREADS, 0, rowdot2_kernel, (const double*)Bt, ld, N, (const double*)w, 1.0,
+                          alpha, (double*)nullptr, stride));
+        }
+        if (grad) {
+            RET_IF(launch(ctx, st, dim3(grid_for(N * ld), z), 256, 0, zero_batch_kernel, Kinv, N * ld, stride));
+            RET_IF(gemm_nt(ctx, st, N, N, N, 1.0, Bt, ld, Bt, ld, 1.0, Kinv, ld, true, bt));
+            if (nngp) {
+                if (depth > 0)
+                    RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(N, (int64_t)256), 1, z), 256, 0, nngp_self_kernel, dX, N, d, kind,
+                                  (const double*)th, chain, stride));
+                for (int j = 0; j < nb; ++j) count_path(ctx, (int)PATH_MLL_NNGP_GRAD);
+                RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles, z), NNGP_THREADS, nngp_grad_smem(d, depth), mll_nngp_grad_kernel,
+                              dX, N, d, kind, (const double*)th, (const double*)chain, (const double*)alpha, (const double*)Kinv, ld, partial,
+                              stride));
+                RET_IF(launch(ctx, st, dim3(3, 1, z), MLL_FIN_THREADS, 0, mll_lcm_finish_kernel, (const double*)partial, tiles * tiles, 3,
+                              sc + 8, stride));
+            } else {
+                RET_IF(launch(ctx, st, dim3((unsigned)tiles, (unsigned)tiles, z), MLL_THREADS, 0, mll_grad_kernel, dX, N, d, kind,
+                              (const double*)th, (const double*)alpha, (const double*)Kinv, ld, partial, stride));
+                RET_IF(launch(ctx, st, dim3(1, 1, z), 32, 0, mll_finish_kernel, (const double*)partial, tiles * tiles, nth, sc + 8, stride));
+            }
+        }
+        // the group's results leave the regions before the next group reuses them
+        RET_IF(launch(ctx, st, grid_for((int64_t)nb * MLLD_HS), 256, 0, copy2d_kernel, dsc + g0 * MLLD_HS, (int64_t)MLLD_HS,
+                      (const double*)sc, stride, (int64_t)nb, (int64_t)MLLD_HS));
+        if (alpha_out)
+            RET_IF(launch(ctx, st, grid_for((int64_t)nb * N), 256, 0, copy2d_kernel, dal + g0 * N, N, (const double*)alpha, stride,
+                          (int64_t)nb, N));
+    }
+    std::vector<double> hsc((size_t)S * MLLD_HS);
+    CUDA_TRY(ctx, cudaMemcpyAsync(hsc.data(), dsc, hsc.size() * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, (size_t)S * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, dal, (size_t)S * N * 8, cudaMemcpyDeviceToHost, st));
+    RET_IF(tm.end(st, nullptr));
+    for (int64_t s = 0; s < S; ++s) {   // mll_impl's host epilogue, per draw
+        const double* h = hsc.data() + s * MLLD_HS;
+        value[s] = -0.5 * h[1] - h[0] - 0.5 * (double)N * 1.8378770664093453;  // log(2 pi)
+        double* g = grad ? grad + s * nth : nullptr;
+        if (g && nngp) {
+            for (int k = 0; k < d; ++k) g[k] = 0.0;
+            for (int k = 0; k < 3; ++k) g[d + k] = h[8 + k];
+        } else if (g) {
+            for (int k = 0; k < nth; ++k) g[k] = h[8 + k];
+        }
+        if (info[s] != 0) {
+            value[s] = NAN;
+            if (g)
+                for (int k = 0; k < nth; ++k) g[k] = NAN;
+            if (alpha_out)
+                for (int64_t i = 0; i < N; ++i) alpha_out[s * N + i] = NAN;
+        }
+    }
+    ctx->last.flops = (double)S * N * N * N * (grad ? 1.0 / 3 + 1.0 + 1.0 : 1.0 / 3);
     return B2GP_OK;
 }
 
@@ -2413,22 +2590,22 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(potrf_rec(ctx, st, Cm, ldM, M, LinvC, dinfo + 1, 0));
     CUDA_TRY(ctx, cudaMemcpyAsync(u, bvec, (size_t)M * 8, cudaMemcpyDeviceToDevice, st));
     RET_IF(trsm_rec(ctx, st, u, ldM, 1, Cm, ldM, M, LinvC));
-    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, Cm, ldM, M, scal + 0));
-    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, u, ldM, M, nullptr, 1.0, nullptr, scal + 1));
-    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, dy, ldN, N, nullptr, 1.0, nullptr, scal + 2));
-    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, nullptr, 1.0, nullptr, tmpM));
+    RET_IF(launch(ctx, st, 1, 256, 0, logdiag_kernel, Cm, ldM, M, scal + 0, (int64_t)0));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, u, ldM, M, nullptr, 1.0, nullptr, scal + 1, (int64_t)0));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, dy, ldN, N, nullptr, 1.0, nullptr, scal + 2, (int64_t)0));
+    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, nullptr, 1.0, nullptr, tmpM, (int64_t)0));
     RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 3));
     // C^{-1} = BtC BtC^T with BtC = (LC^{-1})^T, beta = C^{-1} b
     RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtC, ldM, M, (int64_t)0));
     RET_IF(trsm_rec(ctx, st, BtC, ldM, M, Cm, ldM, M, LinvC));
-    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, BtC, ldM, M, u, 1.0, beta, tmpM));
+    RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, BtC, ldM, M, u, 1.0, beta, tmpM, (int64_t)0));
     RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 4));
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtC, ldM, BtC, ldM, 0.0, Cinv, ldM, true));
     RET_IF(launch(ctx, st, gMM, b32, 0, mirror_lower_kernel, Cinv, ldM, M));
     // alpha = (y - W^T beta) / noise
-    RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Wt, ldM, M, beta, 1.0, tmpN, nullptr));
+    RET_IF(launch(ctx, st, (unsigned)N, RD_THREADS, 0, rowdot2_kernel, Wt, ldM, M, beta, 1.0, tmpN, nullptr, (int64_t)0));
     RET_IF(launch(ctx, st, grid_for(N), 256, 0, elbo_alpha_kernel, alpha, dy, tmpN, N, noise));
-    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, alpha, ldN, N, nullptr, 1.0, nullptr, scal + 5));
+    RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, alpha, ldN, N, nullptr, 1.0, nullptr, scal + 5, (int64_t)0));
     // the clip of the trace term decides a coefficient of the reverse pass: fetch the scalars now
     double hs[8];
     CUDA_TRY(ctx, cudaMemcpyAsync(hs, scal, sizeof hs, cudaMemcpyDeviceToHost, st));
@@ -3229,7 +3406,7 @@ extern "C" int b2gp_dist_posterior(b2gp_ctx* ctx, int kind, const double* Xtr, i
             if (gi < T) continue;
             const int64_t p0 = (gi - T) * nb, np = std::min<int64_t>(nb, P - p0);
             if (np <= 0) continue;
-            RET_IF(launch(ctx, cs, (unsigned)np, RD_THREADS, 0, rowdot2_kernel, A + (li * nb) * ld, ld, ld, wseg, 1.0, red + p0, red + P + p0));
+            RET_IF(launch(ctx, cs, (unsigned)np, RD_THREADS, 0, rowdot2_kernel, A + (li * nb) * ld, ld, ld, wseg, 1.0, red + p0, red + P + p0, (int64_t)0));
         }
         CUDA_TRY(ctx, cudaEventRecord(ds->ev_chunk, cs));
         CUDA_TRY(ctx, cudaStreamWaitEvent(ms, ds->ev_chunk, 0));

@@ -114,6 +114,7 @@ enum PathCounter {
     PATH_MLL_GRAM_TRACE,   // likelihood gradients reduced against caller-supplied dK (mll_gram_trace_kernel), one per call
     PATH_MLL_BATCH_SMALL,  // b2gp_mll_batch calls that took the one-launch small route (mll_batch_small_kernel), one per call
     PATH_POTRF_TALL_BATCH, // lock-step groups of posterior draws factored by one batched potrf_tall (fp64 route), one per group
+    PATH_MLL_DRAWS_BATCH,  // groups of likelihood draws b2gp_mll_draws ran in lock-step, one per group
     PATH_COUNT
 };
 

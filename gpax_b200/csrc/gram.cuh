@@ -36,6 +36,7 @@ struct GramArgs {
     int lower_only;
     double* K;
     int64_t ldk;
+    int64_t bstride = 0;  // doubles between the draws' theta and K (Batch, draw = blockIdx.z); X and Z are shared
 };
 
 __device__ __forceinline__ double cov_from_r2(int kind, double r2, double scale) {
@@ -91,15 +92,16 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_kernel(const GramArgs p) {
     const int64_t row0 = (int64_t)blockIdx.y * GRAM_BM;
     const int64_t col0 = (int64_t)blockIdx.x * GRAM_BN;
     if (p.lower_only && col0 > row0 + GRAM_BM - 1) return;
+    const double* __restrict__ theta = p.theta + (int64_t)blockIdx.z * p.bstride;
     const int tid = threadIdx.x;
     const bool nngp = (p.kind == B2GP_KERNEL_NNGP_ERF || p.kind == B2GP_KERNEL_NNGP_RELU);
     const bool periodic = (p.kind == B2GP_KERNEL_PERIODIC);
 
-    if (tid < d) ell[tid] = p.theta[tid];
+    if (tid < d) ell[tid] = theta[tid];
     __syncthreads();
-    const double scale = p.theta[d];
-    const double noise = p.theta[d + 1];
-    const double period = p.theta[d + 2];
+    const double scale = theta[d];
+    const double noise = theta[d + 1];
+    const double period = theta[d + 2];
 
     // stage the rows: scaled by 1/lengthscale (division, kernels.py:35-36) for RBF/Matern, raw for periodic
     for (int idx = tid; idx < GRAM_BM * d; idx += GRAM_THREADS) {
@@ -134,7 +136,8 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_kernel(const GramArgs p) {
     const int64_t gc = col0 + cl;
     if (gc >= p.m) return;
     const bool has2 = (gc + 1 < p.m);
-    const bool vec_ok = ((p.ldk & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.K) & 15) == 0);
+    double* const K = p.K + (int64_t)blockIdx.z * p.bstride;
+    const bool vec_ok = ((p.ldk & 1) == 0) && ((reinterpret_cast<uintptr_t>(K) & 15) == 0);
     const double diag_add = noise * p.noise_mult + p.jitter;
 
 #pragma unroll 4
@@ -181,7 +184,7 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_kernel(const GramArgs p) {
             if (gr == gc) v0 += diag_add;
             if (gr == gc + 1) v1 += diag_add;
         }
-        double* dst = p.K + gr * p.ldk + gc;
+        double* dst = K + gr * p.ldk + gc;
         const bool w1 = has2 && !(p.lower_only && gc + 1 > gr);
         if (w1 && vec_ok) {
             *reinterpret_cast<double2*>(dst) = make_double2(v0, v1);
@@ -267,11 +270,12 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_fast_kernel(const GramArgs 
     const int64_t col0 = (int64_t)blockIdx.x * GRAM_BN;
     if (p.lower_only && col0 > row0 + GRAM_BM - 1) return;
     const int tid = threadIdx.x;
+    const double* __restrict__ theta = p.theta + (int64_t)blockIdx.z * p.bstride;
     double ell[D];
 #pragma unroll
-    for (int k = 0; k < D; ++k) ell[k] = p.theta[k];
-    const double scale = p.theta[D];
-    const double diag_add = p.theta[D + 1] * p.noise_mult + p.jitter;
+    for (int k = 0; k < D; ++k) ell[k] = theta[k];
+    const double scale = theta[D];
+    const double diag_add = theta[D + 1] * p.noise_mult + p.jitter;
 
     if (tid < GRAM_BM) {
         const int64_t gr = row0 + tid;
@@ -302,7 +306,8 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_fast_kernel(const GramArgs 
     const int64_t gc = col0 + cl;
     if (gc >= p.m) return;
     const bool has2 = (gc + 1 < p.m);
-    const bool vec_ok = ((p.ldk & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.K) & 15) == 0);
+    double* const K = p.K + (int64_t)blockIdx.z * p.bstride;
+    const bool vec_ok = ((p.ldk & 1) == 0) && ((reinterpret_cast<uintptr_t>(K) & 15) == 0);
     double z0[D], z1[D];
 #pragma unroll
     for (int k = 0; k < D; ++k) {
@@ -341,7 +346,7 @@ __global__ void __launch_bounds__(GRAM_THREADS) gram_fast_kernel(const GramArgs 
             v0 = scale * (1.0 + sa + (5.0 / 3.0) * r20) * exp_nonpos(-sa);
             v1 = scale * (1.0 + sb + (5.0 / 3.0) * r21) * exp_nonpos(-sb);
         }
-        double* dst = p.K + gr * p.ldk + gc;
+        double* dst = K + gr * p.ldk + gc;
         bool w0 = true, w1 = has2;
         if (on_diag) {
             if (p.same_xz) {                        // kernels.py:63-64
@@ -382,9 +387,10 @@ __device__ __forceinline__ double cov_self(int kind, double scale) {
     return cov_from_r2(kind, 0.0, scale);
 }
 
+// `bt`: bt.n Gram matrices of the same X and Z, theta_dev and K bt.stride doubles apart per draw
 static int launch_gram(b2gp_ctx* ctx, cudaStream_t st, int kind, const double* X, int64_t n, const double* Z, int64_t m,
                        int d, const double* theta_dev, double noise_mult, double jitter, int same_xz, int lower_only,
-                       double* K, int64_t ldk) {
+                       double* K, int64_t ldk, const Batch& bt = {}) {
     if (n <= 0 || m <= 0) return B2GP_OK;
     if (d < 1 || d > GRAM_MAX_D) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "gram", "1 <= d <= 64", __FILE__, __LINE__);
     GramArgs a;
@@ -401,13 +407,14 @@ static int launch_gram(b2gp_ctx* ctx, cudaStream_t st, int kind, const double* X
     a.lower_only = lower_only;
     a.K = K;
     a.ldk = ldk;
+    a.bstride = bt.stride;
     const size_t smem = (size_t)(GRAM_BM * d + GRAM_BM + d * GRAM_BN + GRAM_BN + d) * sizeof(double);
     static PerDeviceOnce attr;
     if (attr.need(ctx->device)) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
         attr.done(ctx->device);
     }
-    dim3 grid((unsigned)ceil_div(m, GRAM_BN), (unsigned)ceil_div(n, GRAM_BM));
+    dim3 grid((unsigned)ceil_div(m, GRAM_BN), (unsigned)ceil_div(n, GRAM_BM), (unsigned)bt.n);
     GramKernel fast = nullptr;
     if (kind == B2GP_KERNEL_RBF) fast = gram_fast_for<B2GP_KERNEL_RBF>(d);
     if (kind == B2GP_KERNEL_MATERN52) fast = gram_fast_for<B2GP_KERNEL_MATERN52>(d);

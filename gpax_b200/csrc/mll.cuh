@@ -27,9 +27,11 @@ __global__ void set_identity_kernel(double* B, int64_t ld, int64_t n, int64_t bs
     }
 }
 
-// out[0] = sum_i log L_ii   (single block, fixed order)
-__global__ void logdiag_kernel(const double* L, int64_t ld, int64_t n, double* out) {
+// out[0] = sum_i log L_ii   (single block, fixed order); the draw of a batch is blockIdx.z (L and out `bstride` doubles apart)
+__global__ void logdiag_kernel(const double* L, int64_t ld, int64_t n, double* out, int64_t bstride) {
     __shared__ double red[256];
+    L += (int64_t)blockIdx.z * bstride;
+    out += (int64_t)blockIdx.z * bstride;
     double s = 0.0;
     for (int64_t i = threadIdx.x; i < n; i += blockDim.x) s += log(L[i * ld + i]);
     red[threadIdx.x] = s;
@@ -43,11 +45,20 @@ __global__ void logdiag_kernel(const double* L, int64_t ld, int64_t n, double* o
 
 // partial[block][k], k in [0, d+3): sums over the lower triangle (off-diagonal entries weighted 2) of
 //   W_ij * dK_ij/dlog(lengthscale_k) (k < d), dlog(scale) (k = d), dlog(noise) (k = d+1), dlog(period) (k = d+2)
-// with W_ij = alpha_i alpha_j - Kinv_ij.
+// with W_ij = alpha_i alpha_j - Kinv_ij.  The draw of a batch is blockIdx.z: theta, alpha, Kinv and partial `bstride`
+// doubles apart, X shared.
 __global__ void __launch_bounds__(MLL_THREADS)
 mll_grad_kernel(const double* __restrict__ X, int64_t N, int d, int kind, const double* __restrict__ theta,
-                const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ partial) {
+                const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk, double* __restrict__ partial,
+                int64_t bstride) {
     __shared__ double red[MLL_THREADS / 32][MLL_MAX_D + 3];
+    {
+        const int64_t boff = (int64_t)blockIdx.z * bstride;
+        theta += boff;
+        alpha += boff;
+        Kinv += boff;
+        partial += boff;
+    }
     const int64_t ti = blockIdx.y, tj = blockIdx.x;
     const int nout = d + 3;
     double acc[MLL_MAX_D + 3];
@@ -112,8 +123,10 @@ mll_grad_kernel(const double* __restrict__ X, int64_t N, int d, int kind, const 
     }
 }
 
-// grad[k] = 1/2 sum_blocks partial[b][k]   (fixed order)
-__global__ void mll_finish_kernel(const double* partial, int64_t nblocks, int nout, double* grad) {
+// grad[k] = 1/2 sum_blocks partial[b][k]   (fixed order); the draw of a batch is blockIdx.z (`bstride` doubles apart)
+__global__ void mll_finish_kernel(const double* partial, int64_t nblocks, int nout, double* grad, int64_t bstride) {
+    partial += (int64_t)blockIdx.z * bstride;
+    grad += (int64_t)blockIdx.z * bstride;
     const int k = threadIdx.x;
     if (k >= nout) return;
     double s = 0.0;

@@ -370,11 +370,14 @@ mll_lcm_grad_kernel(const double* __restrict__ X, const int* __restrict__ task, 
 
 // colsum[q * nout + k] = 1/2 sum over the blocks of latent q of partial[.][k]: one CTA per (q, k), thread t adding blocks
 // t, t + 256, ... in order, then a fixed tree -- deterministic.  The host assembles the gradient from these sums (dvalue/dB_q
-// with independent entries is the mean of the (a, b) and (b, a) sums; the noise sums sit in latent 0).
+// with independent entries is the mean of the (a, b) and (b, a) sums; the noise sums sit in latent 0).  The draw of a
+// batch is blockIdx.z (partial and colsum `bstride` doubles apart).
 constexpr int MLL_FIN_THREADS = 256;
 __global__ void __launch_bounds__(MLL_FIN_THREADS)
-mll_lcm_finish_kernel(const double* __restrict__ partial, int64_t nblocks, int nout, double* __restrict__ colsum) {
+mll_lcm_finish_kernel(const double* __restrict__ partial, int64_t nblocks, int nout, double* __restrict__ colsum, int64_t bstride) {
     __shared__ double red[MLL_FIN_THREADS];
+    partial += (int64_t)blockIdx.z * bstride;
+    colsum += (int64_t)blockIdx.z * bstride;
     const int q = blockIdx.x / nout, k = blockIdx.x % nout;
     double s = 0.0;
     for (int64_t b = threadIdx.x; b < nblocks; b += MLL_FIN_THREADS) s += partial[((int64_t)q * nblocks + b) * nout + k];

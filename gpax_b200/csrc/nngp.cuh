@@ -77,9 +77,12 @@ __device__ __forceinline__ void nngp_step_fwd(bool relu, double a, double ab, do
     gw = s * t / (2.0 * pi) + cst * (dsw * t + s * dtw);
 }
 
-// chain[(i * depth + l) * 3 + {0, 1, 2}] = k11^(l), dk11^(l)/dvar_b, dk11^(l)/dvar_w of point i, l = 0..depth-1
+// chain[(i * depth + l) * 3 + {0, 1, 2}] = k11^(l), dk11^(l)/dvar_b, dk11^(l)/dvar_w of point i, l = 0..depth-1.
+// The draw of a batch is blockIdx.z (theta and chain `bstride` doubles apart).
 __global__ void nngp_self_kernel(const double* __restrict__ X, int64_t n, int d, int kind, const double* __restrict__ theta,
-                                 double* __restrict__ chain) {
+                                 double* __restrict__ chain, int64_t bstride) {
+    theta += (int64_t)blockIdx.z * bstride;
+    chain += (int64_t)blockIdx.z * bstride;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const bool relu = kind == B2GP_KERNEL_NNGP_RELU;
@@ -109,13 +112,22 @@ static inline size_t nngp_grad_smem(int d, int depth) {
 
 // partial[block * 3 + {0, 1, 2}]: sums over the block's lower-triangle entries (off-diagonal entries weighted 2) of
 // W_ij dK_ij/dlog var_w, W_ii noise (the diagonal's noise term), W_ij dK_ij/dlog var_b.  Blocks above the diagonal write
-// zeros.  Fixed order: each thread's entries in sequence, warp shuffles, then the 8 warps in order.
+// zeros.  Fixed order: each thread's entries in sequence, warp shuffles, then the 8 warps in order.  The draw of a batch
+// is blockIdx.z: theta, chain, alpha, Kinv and partial `bstride` doubles apart, X shared.
 __global__ void __launch_bounds__(NNGP_THREADS)
 mll_nngp_grad_kernel(const double* __restrict__ X, int64_t N, int d, int kind, const double* __restrict__ theta,
                      const double* __restrict__ chain, const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk,
-                     double* __restrict__ partial) {
+                     double* __restrict__ partial, int64_t bstride) {
     extern __shared__ __align__(16) double sm[];
     __shared__ double red[NNGP_THREADS / 32][3];
+    {
+        const int64_t boff = (int64_t)blockIdx.z * bstride;
+        theta += boff;
+        chain += boff;
+        alpha += boff;
+        Kinv += boff;
+        partial += boff;
+    }
     const int64_t ti = blockIdx.y, tj = blockIdx.x;
     const int depth = (int)theta[0];
     double accW = 0.0, accN = 0.0, accB = 0.0;

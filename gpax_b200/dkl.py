@@ -501,7 +501,7 @@ class DKL(_MLPModel):
         self.X_train, self.y_train = X, y
         lj = DKLLogJoint(self, seed_from_key(rng_key), kwargs.get("jitter", 1e-6))
         try:
-            self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+            self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         finally:
             lj.close()
         if print_summary:

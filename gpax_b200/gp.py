@@ -343,7 +343,7 @@ class ExactGP:
         from .inference import fit_exact_gp
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
-        self.mcmc = fit_exact_gp(self, rng_key, num_warmup, num_samples, num_chains, progress_bar, **kwargs)
+        self.mcmc = fit_exact_gp(self, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method, **kwargs)
         if print_summary:
             self._print_summary()
 

@@ -69,6 +69,23 @@ class LogJoint:
         th = self.theta_of(u)
         val, g, info = self._lik(th)
         self.n_evals += 1
+        return self._joint(u, th, val, g, info, jacobian)
+
+    @property
+    def batch(self):
+        """`batch(U, jacobian) -> (values [k], grads [k, dim])`: the rows of U in one b2gp_mll_draws call, row r being
+        self(U[r], jacobian) bit for bit (run_nuts' vectorized chains); None for likelihoods other than b2gp_mll's"""
+        return self._batch if type(self)._lik is LogJoint._lik else None
+
+    def _batch(self, U, jacobian):
+        TH = np.stack([self.theta_of(u) for u in U])
+        vals, G, _, info = self.m.ctx.mll_draws(self.kind, self.X, self.y, TH, self.jitter, want_grad=True)
+        self.n_evals += len(U)
+        out = [self._joint(u, th, float(v), g, int(i), jacobian) for u, th, v, g, i in zip(U, TH, vals, G, info)]
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, th, val, g, info, jacobian):
+        """the log joint and its gradient w.r.t. u from the likelihood's value, d/dlog(theta) and info at theta(u)"""
         if info != 0 or not np.isfinite(val):
             return -np.inf, np.zeros(self.dim)
         grad = np.zeros(self.dim)
@@ -284,6 +301,36 @@ class ProgramLogJoint:
             return -np.inf, np.zeros(self.dim)
         yres = self.y0 if mean is None else self.y0 - mean
         val, g, alpha, info = self._lik(th, yres)
+        return self._joint(u, th, sites, val, g, alpha, info, jacobian)
+
+    @property
+    def batch(self):
+        """`batch(U, jacobian) -> (values [k], grads [k, dim])`: the host programs and their central differences per row,
+        the likelihoods of every valid row in one b2gp_mll_draws call with per-row residuals; row r is self(U[r],
+        jacobian) bit for bit.  None for likelihoods other than b2gp_mll's (callable kernels, multi-task, the VFE bound)."""
+        exact = type(self)._lik is ProgramLogJoint._lik and self._lik_fn is None and not self.CALLABLE_KERNEL
+        return self._batch if exact and type(self).__call__ is ProgramLogJoint.__call__ else None
+
+    def _batch(self, U, jacobian):
+        rows = []
+        for u in U:
+            u = np.asarray(u, dtype=np.float64)
+            th, mean, sites = self._run(u)
+            rows.append((u, th, sites, self.y0 if mean is None else self.y0 - mean))
+        self.n_evals += len(rows)
+        out = [(-np.inf, np.zeros(self.dim))] * len(rows)
+        live = [r for r, row in enumerate(rows) if self._valid(row[1])]
+        if live:
+            vals, G, A, info = self.m.ctx.mll_draws(self.kind, self.X, np.stack([rows[r][3] for r in live]),
+                                                    np.stack([rows[r][1] for r in live]), self.jitter, want_grad=True,
+                                                    want_alpha=self.has_mean_params)
+            for j, r in enumerate(live):
+                u, th, sites, _ = rows[r]
+                out[r] = self._joint(u, th, sites, float(vals[j]), G[j], None if A is None else A[j], int(info[j]), jacobian)
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, th, sites, val, g, alpha, info, jacobian):
+        """the log joint and its gradient w.r.t. u from the likelihood at theta(u) (value, d/dlog(theta), alpha, info)"""
         if info != 0 or not np.isfinite(val):
             return -np.inf, np.zeros(self.dim)
         # site densities: analytic gradient, unless the programs are hierarchical (then differenced with the rest below)
@@ -642,19 +689,23 @@ class MCMCResult:
         return {k: v.reshape((-1,) + v.shape[2:]) for k, v in self._s.items()}
 
 
-def _leapfrog(lj, u, r, g, eps, minv):
+# The sampler is written as generators (the *_gen functions): a chain yields each point u at which it needs the log joint and receives
+# (value, grad) = lj(u, jacobian=True) back.  One implementation then serves both chain methods: "sequential" runs one
+# chain's generator to its end before the next, "vectorized" advances every chain by one evaluation per round and hands
+# the round's points to the log joint together.  A chain consumes its own rng in the same order either way.
+def _leapfrog_gen(u, r, g, eps, minv):
     r = r + 0.5 * eps * g
     u = u + eps * minv * r
-    lp, g = lj(u, jacobian=True)
+    lp, g = yield u
     r = r + 0.5 * eps * g
     return u, r, lp, g
 
 
-def _find_eps(lj, u, lp, g, rng, minv):
+def _find_eps_gen(u, lp, g, rng, minv):
     eps = 1.0
     r = rng.standard_normal(u.size) / np.sqrt(minv)
     h0 = lp - 0.5 * np.dot(r, minv * r)
-    _, r1, lp1, _ = _leapfrog(lj, u, r, g, eps, minv)
+    _, r1, lp1, _ = yield from _leapfrog_gen(u, r, g, eps, minv)
     h1 = lp1 - 0.5 * np.dot(r1, minv * r1)
     a = 1.0 if (np.isfinite(h1) and h1 - h0 > math.log(0.5)) else -1.0
     for _ in range(50):
@@ -662,12 +713,12 @@ def _find_eps(lj, u, lp, g, rng, minv):
             if np.isfinite(h1) or a < 0:
                 break
         eps *= 2.0 ** a
-        _, r1, lp1, _ = _leapfrog(lj, u, r, g, eps, minv)
+        _, r1, lp1, _ = yield from _leapfrog_gen(u, r, g, eps, minv)
         h1 = lp1 - 0.5 * np.dot(r1, minv * r1)
     return eps
 
 
-def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
+def _nuts_draw_gen(u0, lp0, g0, eps, rng, minv, max_depth=10):
     """one transition of the no-U-turn sampler with multinomial sampling along the trajectory"""
     r0 = rng.standard_normal(u0.size) / np.sqrt(minv)
     h0 = lp0 - 0.5 * np.dot(r0, minv * r0)
@@ -680,7 +731,7 @@ def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
     def build(u_, r_, g_, v, j):
         nonlocal alpha_sum, n_alpha, diverged
         if j == 0:
-            u1, r1, lp1, g1 = _leapfrog(lj, u_, r_, g_, v * eps, minv)
+            u1, r1, lp1, g1 = yield from _leapfrog_gen(u_, r_, g_, v * eps, minv)
             h1 = lp1 - 0.5 * np.dot(r1, minv * r1) if np.isfinite(lp1) else -np.inf
             dh = h1 - h0
             if not np.isfinite(dh):
@@ -691,15 +742,15 @@ def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
             if not ok:
                 diverged = True
             return u1, r1, g1, u1, r1, g1, u1, lp1, g1, dh, ok
-        a = build(u_, r_, g_, v, j - 1)
+        a = yield from build(u_, r_, g_, v, j - 1)
         um_, rm_, gm_, up_, rp_, gp_, uc, lpc, gc, lw, ok = a
         if not ok:
             return a
         if v == -1:
-            b = build(um_, rm_, gm_, v, j - 1)
+            b = yield from build(um_, rm_, gm_, v, j - 1)
             um_, rm_, gm_ = b[0], b[1], b[2]
         else:
-            b = build(up_, rp_, gp_, v, j - 1)
+            b = yield from build(up_, rp_, gp_, v, j - 1)
             up_, rp_, gp_ = b[3], b[4], b[5]
         lw2, ok2 = b[9], b[10]
         lw_tot = np.logaddexp(lw, lw2)
@@ -712,10 +763,10 @@ def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
     while depth < max_depth:
         v = 1 if rng.uniform() < 0.5 else -1
         if v == -1:
-            t = build(um, rm, gm, v, depth)
+            t = yield from build(um, rm, gm, v, depth)
             um, rm, gm = t[0], t[1], t[2]
         else:
-            t = build(up, rp, gp, v, depth)
+            t = yield from build(up, rp, gp, v, depth)
             up, rp, gp = t[3], t[4], t[5]
         lw2, ok = t[9], t[10]
         if ok and math.log(rng.uniform()) < lw2 - logw:      # biased progressive sampling
@@ -728,52 +779,118 @@ def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
     return u, lp, g, alpha_sum / max(n_alpha, 1), depth, diverged
 
 
-def fit_exact_gp(model, rng_key, num_warmup, num_samples, num_chains, progress_bar, **kwargs):
+def _drive(gen, lj):
+    """run a sampler generator to its end against lj(u, jacobian=True), one point at a time; returns its result"""
+    try:
+        u = next(gen)
+        while True:
+            u = gen.send(lj(u, jacobian=True))
+    except StopIteration as stop:
+        return stop.value
+
+
+def _find_eps(lj, u, lp, g, rng, minv):
+    """a reasonable first step size at u (Hoffman & Gelman, algorithm 4)"""
+    return _drive(_find_eps_gen(u, lp, g, rng, minv), lj)
+
+
+def _nuts_draw(lj, u0, lp0, g0, eps, rng, minv, max_depth=10):
+    """one NUTS transition from u0: (u, lp, grad, mean acceptance, depth, diverged)"""
+    return _drive(_nuts_draw_gen(u0, lp0, g0, eps, rng, minv, max_depth), lj)
+
+
+def _chain(lj, c, seed, num_warmup, num_samples, progress_bar):
+    """one NUTS chain as a generator (see _leapfrog_gen); returns (draws [num_samples, dim], step size, divergences)"""
+    rng = np.random.default_rng(seed)
+    u = lj.init_u() + (0.0 if c == 0 else 0.1 * rng.standard_normal(lj.dim))
+    lp, g = yield u
+    minv = np.ones(lj.dim)
+    eps = yield from _find_eps_gen(u, lp, g, rng, minv)
+    mu, hbar, log_eps_bar, gamma, t0, kappa, delta = math.log(10 * eps), 0.0, 0.0, 0.05, 10.0, 0.75, 0.8
+    draws, warm_buf, div, m = [], [], 0, 0
+    metric_at = (3 * int(num_warmup)) // 4 if num_warmup >= 40 else -1
+    for it in range(int(num_warmup) + int(num_samples)):
+        u, lp, g, acc, depth, dv = yield from _nuts_draw_gen(u, lp, g, eps, rng, minv)
+        if it < num_warmup:
+            m += 1
+            hbar = (1 - 1 / (m + t0)) * hbar + (delta - acc) / (m + t0)
+            log_eps = mu - math.sqrt(m) / gamma * hbar
+            eta = m ** (-kappa)
+            log_eps_bar = eta * log_eps + (1 - eta) * log_eps_bar
+            eps = math.exp(log_eps)
+            if num_warmup // 4 <= it < metric_at:
+                warm_buf.append(u.copy())
+            if it == metric_at - 1 and len(warm_buf) >= 10:
+                var = np.var(np.array(warm_buf), axis=0)
+                minv = (len(warm_buf) * var + 1e-3 * 5) / (len(warm_buf) + 5)        # regularised, as Stan
+                eps = yield from _find_eps_gen(u, lp, g, rng, minv)                       # step size for the new metric
+                mu, hbar, log_eps_bar, m = math.log(10 * eps), 0.0, 0.0, 0            # dual averaging restarts
+            if it == num_warmup - 1:
+                eps = math.exp(log_eps_bar) if m > 0 else eps
+        else:
+            draws.append(u.copy())
+            div += int(dv)
+        if progress_bar and (it + 1) % max(1, (num_warmup + num_samples) // 10) == 0:
+            print(f"chain {c} iter {it + 1}/{num_warmup + num_samples} step {eps:.3g} depth {depth} lp {lp:.3f}")
+    return np.array(draws), eps, div
+
+
+def fit_exact_gp(model, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method="sequential", **kwargs):
     """gp.py:207-218."""
-    return run_nuts(make_log_joint(model, kwargs.get("jitter", 1e-6)), rng_key, num_warmup, num_samples, num_chains, progress_bar)
+    return run_nuts(make_log_joint(model, kwargs.get("jitter", 1e-6)), rng_key, num_warmup, num_samples, num_chains, progress_bar,
+                    chain_method=chain_method)
 
 
-def run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar):
+def run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method="sequential"):
     """NUTS over any log joint `lj(u, jacobian) -> (value, grad)` with `dim`, `init_u()`, `to_dict(U)`.  Dual-averaging
     step-size adaptation (target accept 0.8).  Warm-up windows as in Stan / NumPyro: draws of the middle of warm-up
     estimate a diagonal mass matrix, which is installed at 3/4 of warm-up; the step size is then re-initialised for the
-    new metric and dual averaging restarts over the last quarter.  Chains run one after another ('sequential')."""
+    new metric and dual averaging restarts over the last quarter.
+
+    chain_method "vectorized" runs the chains in lock-step: each round evaluates the pending point of every unfinished
+    chain, with one `lj.batch(U, jacobian) -> (values [k], grads [k, dim])` call when the log joint has one, else row by
+    row.  Every other value ("sequential", the default, and "parallel") runs the chains one after another.  Either way
+    chain c draws from the same seed in the same order, so both give the same samples bit for bit as long as `batch`
+    returns what `lj` returns row by row; stats[c]["grad_evals"] counts the evaluations of chains 0..c."""
     root = seed_from_key(rng_key)
-    chains, stats = [], []
-    for c in range(int(num_chains)):
-        rng = np.random.default_rng(root.integers(0, 2 ** 63))
-        u = lj.init_u() + (0.0 if c == 0 else 0.1 * rng.standard_normal(lj.dim))
-        lp, g = lj(u, jacobian=True)
-        minv = np.ones(lj.dim)
-        eps = _find_eps(lj, u, lp, g, rng, minv)
-        mu, hbar, log_eps_bar, gamma, t0, kappa, delta = math.log(10 * eps), 0.0, 0.0, 0.05, 10.0, 0.75, 0.8
-        draws, warm_buf, div, m = [], [], 0, 0
-        metric_at = (3 * int(num_warmup)) // 4 if num_warmup >= 40 else -1
-        for it in range(int(num_warmup) + int(num_samples)):
-            u, lp, g, acc, depth, dv = _nuts_draw(lj, u, lp, g, eps, rng, minv)
-            if it < num_warmup:
-                m += 1
-                hbar = (1 - 1 / (m + t0)) * hbar + (delta - acc) / (m + t0)
-                log_eps = mu - math.sqrt(m) / gamma * hbar
-                eta = m ** (-kappa)
-                log_eps_bar = eta * log_eps + (1 - eta) * log_eps_bar
-                eps = math.exp(log_eps)
-                if num_warmup // 4 <= it < metric_at:
-                    warm_buf.append(u.copy())
-                if it == metric_at - 1 and len(warm_buf) >= 10:
-                    var = np.var(np.array(warm_buf), axis=0)
-                    minv = (len(warm_buf) * var + 1e-3 * 5) / (len(warm_buf) + 5)        # regularised, as Stan
-                    eps = _find_eps(lj, u, lp, g, rng, minv)                              # step size for the new metric
-                    mu, hbar, log_eps_bar, m = math.log(10 * eps), 0.0, 0.0, 0            # dual averaging restarts
-                if it == num_warmup - 1:
-                    eps = math.exp(log_eps_bar) if m > 0 else eps
+    seeds = [root.integers(0, 2 ** 63) for _ in range(int(num_chains))]
+    gens = [_chain(lj, c, seed, num_warmup, num_samples, progress_bar) for c, seed in enumerate(seeds)]
+    n0 = lj.n_evals
+    results, evals = [None] * len(gens), [0] * len(gens)
+    if chain_method == "vectorized":
+        batch = getattr(lj, "batch", None)
+        pending = {}
+        for c, gen in enumerate(gens):
+            pending[c] = next(gen)
+        while pending:
+            cs = sorted(pending)
+            if batch is not None:
+                vals, grads = batch(np.stack([pending[c] for c in cs]), jacobian=True)
+                outs = [(vals[i], grads[i]) for i in range(len(cs))]
+                for c in cs:
+                    evals[c] += 1
             else:
-                draws.append(u.copy())
-                div += int(dv)
-            if progress_bar and (it + 1) % max(1, (num_warmup + num_samples) // 10) == 0:
-                print(f"chain {c} iter {it + 1}/{num_warmup + num_samples} step {eps:.3g} depth {depth} lp {lp:.3f}")
-        chains.append(np.array(draws))
-        stats.append({"step_size": eps, "divergences": div, "grad_evals": lj.n_evals})
+                outs = []
+                for c in cs:
+                    before = lj.n_evals
+                    outs.append(lj(pending[c], jacobian=True))
+                    evals[c] += lj.n_evals - before
+            for c, out in zip(cs, outs):
+                try:
+                    pending[c] = gens[c].send(out)
+                except StopIteration as stop:
+                    results[c] = stop.value
+                    del pending[c]
+    else:
+        for c, gen in enumerate(gens):
+            before = lj.n_evals
+            results[c] = _drive(gen, lj)
+            evals[c] = lj.n_evals - before
+    chains, stats, total = [], [], n0
+    for (draws, eps, div), e in zip(results, evals):
+        total += e
+        chains.append(draws)
+        stats.append({"step_size": eps, "divergences": div, "grad_evals": total})
     per_chain = [lj.to_dict(ch) for ch in chains]
     by_chain = {k: np.stack([pc[k] for pc in per_chain]) for k in per_chain[0]}
     return MCMCResult(by_chain, stats)

@@ -157,7 +157,7 @@ class _LCMModel(ExactGP):
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
         lj = MTLogJoint(self, kwargs.get("jitter", 1e-6))
-        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             self._print_summary()
 

@@ -100,7 +100,7 @@ class MeasuredNoiseGP(ExactGP):
         self.X_train, self.y_train = X, y
         self.measured_noise = np.asarray(measured_noise, dtype=np.float64)
         lj = _MeasuredNoiseLogJoint(self, self.measured_noise, kwargs.get("jitter", 1e-6))
-        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             self._print_summary()
 
@@ -253,7 +253,7 @@ class VarNoiseGP(ExactGP):
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
         lj = _VarNoiseLogJoint(self, kwargs.get("jitter", 1e-6))
-        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             s = self.get_samples(1)
             for k, v in s.items():
@@ -385,7 +385,7 @@ class vExactGP(ExactGP):
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
         lj = _VExactLogJoint(self, kwargs.get("jitter", 1e-6))
-        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             self._print_summary()
 
@@ -473,6 +473,22 @@ class _VExactLogJoint:
         th = self.theta_of(u)
         val, g, _, _, info = self.m.ctx.mll_batch(self.kind, self.X, self.y, th, self.jitter, True)
         self.n_evals += 1
+        return self._joint(u, th, val, g, info, jacobian)
+
+    def batch(self, U, jacobian):
+        """the rows of U (one per chain of a vectorized NUTS round) in one b2gp_mll_batch call over k * B members; each
+        member is its own CTA or its own b2gp_mll route, so row r is self(U[r], jacobian) bit for bit"""
+        k, B = len(U), self.B
+        TH = np.stack([self.theta_of(u) for u in U])
+        val, g, _, _, info = self.m.ctx.mll_batch(self.kind, np.tile(self.X, (k, 1, 1)), np.tile(self.y, (k, 1)),
+                                                  TH.reshape(k * B, -1), self.jitter, True)
+        self.n_evals += k
+        out = [self._joint(u, th, val[r * B:(r + 1) * B], g[r * B:(r + 1) * B], info[r * B:(r + 1) * B], jacobian)
+               for r, (u, th) in enumerate(zip(U, TH))]
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, th, val, g, info, jacobian):
+        """the log joint and its gradient w.r.t. u from the B members' likelihoods at theta(u)"""
         val = float(val.sum())
         if (info != 0).any() or not np.isfinite(val):
             return -np.inf, np.zeros(self.dim)
@@ -558,7 +574,7 @@ class UIGP(ExactGP):
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
         lj = _UIGPLogJoint(self, kwargs.get("jitter", 1e-6))
-        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar)
+        self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             self._print_summary()
 
@@ -640,10 +656,25 @@ class _UIGPLogJoint:
                                [float(p.inverse(p.median())) for p in self.kpriors]])
 
     def __call__(self, u, jacobian):
-        d = self.d
         sx, Xp, th = self._split(u)
         val, g, _, gx, info = self.m.ctx.mll_batch(self.kind, Xp[None], self.y[None], th[None], self.jitter, True, False, True)
         self.n_evals += 1
+        return self._joint(u, sx, Xp, th, val, g, gx, info, jacobian)
+
+    def batch(self, U, jacobian):
+        """the rows of U (one per chain of a vectorized NUTS round) as the members of one b2gp_mll_batch call; each member
+        is its own CTA or its own b2gp_mll route, so row r is self(U[r], jacobian) bit for bit"""
+        parts = [self._split(u) for u in U]
+        val, g, _, gx, info = self.m.ctx.mll_batch(self.kind, np.stack([p[1] for p in parts]), np.tile(self.y, (len(U), 1)),
+                                                   np.stack([p[2] for p in parts]), self.jitter, True, False, True)
+        self.n_evals += len(U)
+        out = [self._joint(u, sx, Xp, th, val[r:r + 1], g[r:r + 1], gx[r:r + 1], info[r:r + 1], jacobian)
+               for r, (u, (sx, Xp, th)) in enumerate(zip(U, parts))]
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, sx, Xp, th, val, g, gx, info, jacobian):
+        """the log joint and its gradients from the likelihood at (X_prime, theta) (b2gp_mll_batch's outputs, one member)"""
+        d = self.d
         val = float(val[0])
         if info[0] != 0 or not np.isfinite(val) or not np.all(np.isfinite(sx)) or not np.all(sx > 0):
             return -np.inf, np.zeros(self.dim)

@@ -378,6 +378,24 @@ int  b2gp_mll_batch(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                     const double* theta, double jitter, unsigned flags, double* value, double* grad, double* alpha_out,
                     double* grad_x, int* info);
 
+/* S exact-GP likelihoods on one X in lock-step (the chains of a vectorized NUTS round): draw s is b2gp_mll(kind, X,
+ * yres + s * yres_stride, theta + s * (d+3)) and returns that call's value, grad, alpha and info bit for bit on the same
+ * context options, whatever S and however the draws are grouped.  X[N,d] and yres (yres_stride = 0: one [N] vector for
+ * every draw; else >= N doubles between draws) as b2gp_mll; theta[S,d+3] (NNGP kinds: b2gp_mll's layout and depth check
+ * per draw).  HOST outputs: value[S]; grad[S,d+3] (optional) d value / dlog theta; alpha_out[S,N] (optional) K^{-1} yres;
+ * info[S].  A draw with info[s] != 0 has NaN value, grad and alpha; the others are unaffected.  Routes:
+ *   fp64, N < tall_min_fp64:   mll_impl's sequence in groups of draws, every launch (Gram build, recursive factorisation,
+ *                              solves, K^{-1}, gradient reduction) covering the whole group: the launches per call do not
+ *                              grow with S;
+ *   fp64, N >= tall_min_fp64:  the same with the batched tall-panel factorisation, y riding below K;
+ *   int8 (ozaki != 0):         one draw at a time (those GEMMs take one draw), one host sync for the call.
+ * Groups hold as many draws as an eighth of the device memory takes (option draw_batch: 1 = one draw per group, B >= 2 =
+ * groups of B); each group counts once in the route counter mll_draws_batch.  Host fp64 arrays only: B2GP_FLAG_F32 and
+ * B2GP_FLAG_DEVICE_PTRS give B2GP_ERR_UNSUPPORTED before any launch; there is no noise-vector or multi-task form.      */
+int  b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
+                    int64_t S, const double* theta, double jitter, unsigned flags, double* value, double* grad,
+                    double* alpha_out, int* info);
+
 /* The multi-task counterpart (the likelihood of viMTDKL.model, gpax/models/vi_mtdkl.py): log N(yres; 0, K) with K the
  * LCM covariance of b2gp_mll_multitask on the embedding z = MLP(X), expanded to the GP rows:
  *   X[N, D]                 the network's inputs, N points, without the task column
