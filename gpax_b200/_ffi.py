@@ -116,6 +116,8 @@ SIGNATURES = {
                                   _dp, _dp, _vp]),
     "b2gp_bnn_predict": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
                                    _vp, C.c_int64, _vp, _vp, C.c_uint]),
+    "b2gp_bnn_predict_grad": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp,
+                                        C.c_uint]),
     "b2gp_sparse_elbo": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp,
                                    _vp, _ip]),
     "b2gp_dist_unique_id": (C.c_int, [_vp]),
@@ -786,6 +788,25 @@ class Context:
         self._check(self.lib.b2gp_bnn_predict(self.h, Xp, Pn, D, int(w.size), _ptr(w), int(act), _ptr(p), S, p.shape[1], O,
                                               _ptr(sg), _ptr(eps), n, _ptr(loc), _ptr(ys), flags))
         return loc, ys
+
+    def bnn_predict_grad(self, X, widths, act, params):
+        """loc [S, P] = MLP(X) of a one-output network for S weight sets and dloc [S, P, D] = d loc / dX
+        (b2gp_bnn_predict_grad).  X [P, D] and params [S, P] or [P]: both host arrays or both DeviceArrays, so that an
+        optimisation can keep the weight sets on the device.  Returns (loc, dloc)."""
+        X, Xp, flags = self._arg(X)
+        p, pp, pflags = self._arg(params)
+        if flags != pflags:
+            raise ValueError("X and params must both be host arrays or both DeviceArrays")
+        Pn, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        shape = tuple(p.shape)
+        S, npar = (1, shape[0]) if len(shape) == 1 else shape
+        if npar != _mlp_nparams(D, w):
+            raise ValueError(f"params rows have {npar} entries, the network D={D}, widths={w.tolist()} has {_mlp_nparams(D, w)}")
+        loc, dloc = np.empty((S, Pn)), np.empty((S, Pn, D))
+        self._check(self.lib.b2gp_bnn_predict_grad(self.h, Xp, Pn, D, int(w.size), _ptr(w), int(act), pp, S, npar, _ptr(loc),
+                                                   _ptr(dloc), flags))
+        return loc, dloc
 
     @staticmethod
     def _arg(a):

@@ -5,6 +5,7 @@ acquisition.py -- acquisition functions with the reference's surface: EI / UCB /
 (b2gp_acq_moments / b2gp_acq_samples / b2gp_kg, gpax_b200/csrc/acq.cuh); the penalties of
 gpax/acquisition/penalties.py are O(P * recent) host arithmetic and stay on the host, as in the reference.
 """
+import contextlib
 from typing import Optional
 
 import numpy as np
@@ -79,9 +80,33 @@ def _check_penalty(penalty, recent_points):
 
 
 # ------------------------------------------------------------------ model-level functions (acquisition.py)
+def _is_bnn(model):
+    from .bnn import BNN
+    return isinstance(model, BNN)
+
+
+def _check_bnn(model):
+    """the acquisition functions take a fitted one-output BNN"""
+    if model.output_dim != 1:
+        raise ValueError(f"acquisition functions need a one-output BNN; this one has output_dim={model.output_dim}")
+    if model.mcmc is None:
+        raise ValueError("the BNN has no posterior samples: fit it first")
+
+
+def _num_draws(samples):
+    """the number of posterior draws: the leading length of the samples' first site"""
+    return len(next(iter(samples.values())))
+
+
 def _acq_for_model(kind, rng_key, model, X, n, noiseless, best_f, param, maximize, **kwargs):
     """acquisition.py:23-36 (_compute_mean_and_var) + the base function.  Fully Bayesian model: the moments are taken
-    over the S*n posterior samples (column reduction on the device); viGP-style model: over (mean, var) directly."""
+    over the S*n posterior samples (column reduction on the device); viGP-style model: over (mean, var) directly.  BNN:
+    over the S values y_sampled[:, p, 0], each of which BNN.predict has already averaged over its n noise draws."""
+    if _is_bnn(model):
+        _check_bnn(model)
+        _, y_sampled = model.predict(rng_key, X, n=n, noiseless=noiseless, **kwargs)
+        acq, _, _ = model.ctx.acq_samples(kind, np.asarray(y_sampled)[:, :, 0], best_f, param, maximize)
+        return acq
     if getattr(model, "mcmc", None) is not None:
         _, y_sampled = model.predict(rng_key, X, n=n, noiseless=noiseless, **kwargs)
         y = np.asarray(y_sampled, dtype=np.float64).reshape(n * y_sampled.shape[0], -1)
@@ -155,10 +180,17 @@ def kg(model, X_new, sample, rng_key=None, n: int = 10, maximize: bool = True, n
     return model.ctx.kg(mean, cov, ysim, diag_sub, noise + jitter, maximize)
 
 
+def _refuse_kg_on_bnn(model):
+    if _is_bnn(model):
+        raise ValueError("KG / qKG condition a GP posterior on simulated observations; a BNN would need a refit")
+
+
 def KG(rng_key, model, X, n: int = 1, maximize: bool = False, noiseless: bool = False, penalty: Optional[str] = None,
        recent_points=None, grid_indices=None, penalty_factor: float = 1.0, **kwargs):
     """Knowledge gradient -- acquisition.py:395-484: kg() for the variational model's parameters, or one row per
-    posterior draw ([S, P], the reference's vmap over the draws) for an MCMC model."""
+    posterior draw ([S, P], the reference's vmap over the draws) for an MCMC model.  Not for a BNN (ValueError): kg()
+    conditions a GP posterior on simulated observations, which for a network would mean a refit."""
+    _refuse_kg_on_bnn(model)
     _check_penalty(penalty, recent_points)
     X = np.asarray(X)
     X = X[:, None] if X.ndim < 2 else X
@@ -188,13 +220,24 @@ def _subsample(samples, num, rng_key):
 def _q_acq(kind, rng_key, model, X, best_f, param, maximize, noiseless, maximize_distance, subsample_size, n_evals,
            indices, **kwargs):
     """batch_acquisition.py:20-57: the acquisition function of `subsample_size` individual posterior draws, one row each
-    ([subsample_size, P]); one batched posterior call (mean + diag variance) and one epilogue launch per evaluation."""
+    ([subsample_size, P]); one batched posterior call (mean + diag variance) and one epilogue launch per evaluation.
+    BNN: draw s's moments are (loc_s, sigma_s^2), loc from one b2gp_bnn_predict call; noiseless is refused, since one
+    weight draw has no spread without its noise."""
+    bnn = _is_bnn(model)
+    if bnn:
+        _check_bnn(model)
+        if noiseless:
+            raise ValueError("q-batch acquisitions on a BNN need noiseless=False: one weight draw has no spread without noise")
     if getattr(model, "mcmc", None) is None:
         raise ValueError("The model needs to be fully Bayesian")
     X = np.asarray(X)
     X = X[:, None] if X.ndim < 2 else X
 
     def rows(samples, Xq):
+        if bnn:
+            loc, _ = model._predict_draws(model._set_data(Xq), np.atleast_2d(model.to_flat(samples)))
+            var = np.broadcast_to(np.asarray(samples["noise"], np.float64).reshape(-1, 1) ** 2, loc.shape[:2])
+            return model.ctx.acq_moments(kind, loc[:, :, 0], var, best_f, param, maximize)
         out = model._posterior_batched(Xq, samples, True, noiseless, ("mean", "var"), **kwargs)
         return model.ctx.acq_moments(kind, out["mean"], out["var"], best_f, param, maximize)
 
@@ -241,7 +284,8 @@ def qKG(rng_key, model, X, n: int = 10, maximize: bool = False, noiseless: bool 
         subsample_size: int = 1, n_evals: int = 10, indices=None, **kwargs):
     """batch_acquisition.py:235-282: kg() of each sub-sampled posterior draw, one row per draw ([subsample_size, P]),
     with the draw sub-sampling and the `maximize_distance` selection of the other q-batch functions.  Every draw's kg()
-    uses `rng_key` for its simulated observations, as the reference's single_acq does."""
+    uses `rng_key` for its simulated observations, as the reference's single_acq does.  Not for a BNN (ValueError)."""
+    _refuse_kg_on_bnn(model)
     if getattr(model, "mcmc", None) is None:
         raise ValueError("The model needs to be fully Bayesian")
     X = np.asarray(X)
@@ -260,12 +304,19 @@ def Thompson(rng_key, model, X, n: int = 1, noiseless: bool = False, **kwargs):
     """Thompson sampling -- acquisition.py:487-524.  MCMC model: one hyper-parameter draw picked by
     `prng.randint(rng_key, (1,), 0, S)` (jax.random.randint), then `predict` with that draw and `rng_key`; the n samples
     are averaged when n > 1.  Otherwise the reference calls `model.sample_from_posterior`, which ExactGP and viGP do
-    not have (there as here), so they raise AttributeError."""
+    not have (there as here), so they raise AttributeError.  The draws are counted along the samples' first site, so a BNN
+    (which has no k_length) works too; its y_sampled [1, P, 1] is already averaged over the n noise draws and comes back
+    in the GP's layout, [1, 1, P] for n = 1 and [P] for n > 1."""
+    bnn = _is_bnn(model)
+    if bnn:
+        _check_bnn(model)
     if getattr(model, "mcmc", None) is not None:
         posterior_samples = model.get_samples()
-        idx = prng.randint(prng.as_key(rng_key), (1,), 0, len(posterior_samples["k_length"]))
+        idx = prng.randint(prng.as_key(rng_key), (1,), 0, _num_draws(posterior_samples))
         samples = {k: np.asarray(v)[idx] for k, v in posterior_samples.items()}
         _, tsample = model.predict(rng_key, X, samples, n, noiseless=noiseless, **kwargs)
+        if bnn:
+            tsample = np.asarray(tsample)[:, None, :, 0]
         if n > 1:
             tsample = tsample.mean(1).squeeze()
         return tsample
@@ -343,13 +394,18 @@ def _analytic_kind(acq_fn, model, kwargs):
 
     A plain ExactGP or viGP qualifies: their predict() is the exact-GP posterior that b2gp_posterior_grad
     differentiates.  So do a plain viDKL or DKL with single-channel targets: their predict() is that posterior on the
-    network's embedding, which b2gp_dkl_posterior_grad differentiates w.r.t. the raw inputs.  Every other subclass
-    (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, viMTDKL, iBNN, or a user's own) predicts something else, so
-    it takes the finite-difference branch even though it inherits _posterior_grad; so does a multi-channel viDKL."""
+    network's embedding, which b2gp_dkl_posterior_grad differentiates w.r.t. the raw inputs.  So does a one-output BNN:
+    its samples are loc + sigma * (mean noise draw) per weight draw, and b2gp_bnn_predict_grad differentiates loc.  Every
+    other subclass (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, viMTDKL, iBNN, or a user's own) predicts
+    something else, so it takes the finite-difference branch even though it inherits _posterior_grad; so does a
+    multi-channel viDKL."""
+    from .bnn import BNN
     from .dkl import DKL, viDKL
     from .gp import ExactGP
     from .vigp import viGP
     kind = {EI: "EI", UCB: "UCB", POI: "POI", UE: "UE"}.get(acq_fn)
+    if kind is not None and not kwargs.get("penalty") and type(model) is BNN:
+        return kind if model.output_dim == 1 else None
     if kind is None or kwargs.get("penalty") or type(model) not in (ExactGP, viGP, viDKL, DKL):
         return None
     if model.mean_fn is not None or model._fused is None:
@@ -359,10 +415,8 @@ def _analytic_kind(acq_fn, model, kwargs):
     return kind
 
 
-def _analytic_objective(kind, rng_key, model, d, kwargs):
-    """x [d] -> (acq(x), d acq / dx) through one model._posterior_grad call per evaluation (b2gp_posterior_grad, or
-    b2gp_dkl_posterior_grad for viDKL / DKL)"""
-    from .gp import _eps_dtype
+def _analytic_args(kind, kwargs):
+    """(the keywords left for the model, n, noiseless, maximize, best_f, param) of acquisition `kind` called with kwargs"""
     kw = dict(kwargs)
     n = int(kw.pop("n", 1))
     noiseless = bool(kw.pop("noiseless", False))
@@ -374,6 +428,14 @@ def _analytic_objective(kind, rng_key, model, d, kwargs):
         kw.pop(k, None)
     if kind == "UE":
         maximize = False
+    return kw, n, noiseless, maximize, best_f, param
+
+
+def _analytic_objective(kind, rng_key, model, d, kwargs):
+    """x [d] -> (acq(x), d acq / dx) through one model._posterior_grad call per evaluation (b2gp_posterior_grad, or
+    b2gp_dkl_posterior_grad for viDKL / DKL)"""
+    from .gp import _eps_dtype
+    kw, n, noiseless, maximize, best_f, param = _analytic_args(kind, kwargs)
     mcmc = getattr(model, "mcmc", None) is not None
     samples = model.get_samples()
     S = len(next(iter(samples.values()))) if mcmc else 1
@@ -383,6 +445,39 @@ def _analytic_objective(kind, rng_key, model, d, kwargs):
         mean, var, dmean, dvar = model._posterior_grad(np.asarray(x, np.float64).reshape(1, d), samples, mcmc, noiseless, **kw)
         return acq_value_grad(kind, mean[:, 0], var[:, 0], dmean[:, 0, :], dvar[:, 0, :], eps, best_f, param, maximize)
     return f
+
+
+@contextlib.contextmanager
+def _bnn_objective(kind, rng_key, model, d, kwargs):
+    """x [d] -> (acq(x), d acq / dx) on a one-output BNN, one b2gp_bnn_predict_grad call per evaluation.  The weight
+    sets go to the device once for the whole optimisation.  BNN.predict's samples at one point are y_s = loc_s + sigma_s
+    e_s, e_s the mean of the n normals of draw s in the stream predict draws at P = 1 (sigma_s = 0 when noiseless), so
+    dy_s = dloc_s; their pooled mean and population variance and those moments' gradients go to acq_value_grad."""
+    from ._ffi import ACT_TANH
+    from .gp import _eps_dtype
+    kw, n, noiseless, maximize, best_f, param = _analytic_args(kind, kwargs)
+    samples = kw.get("samples") or model.get_samples()
+    flat = np.atleast_2d(model.to_flat(samples))
+    S = flat.shape[0]
+    eps = np.asarray(posterior_eps(rng_key, S, n, 1, _eps_dtype()), np.float64).reshape(S, n)
+    sigma = 0.0 if noiseless else np.asarray(samples["noise"], np.float64).reshape(S)
+    e = sigma * (eps.sum(1) / n)
+    ctx = model.ctx
+    Pd, Xd = ctx.to_device(flat), ctx.alloc((1, d))
+    try:
+        def f(x):
+            Xd.upload(np.asarray(x, np.float64).reshape(1, d))
+            loc, dloc = ctx.bnn_predict_grad(Xd, model.widths, ACT_TANH, Pd)
+            y, dy = loc[:, 0] + e, dloc[:, 0, :]
+            M = y.mean()
+            dM = dy.mean(0)
+            V = ((y - M) ** 2).mean()
+            dV = 2.0 * ((y - M)[:, None] * (dy - dM)).mean(0)
+            return acq_value_grad(kind, [M], [V], dM[None], dV[None], None, best_f, param, maximize)
+        yield f
+    finally:
+        Pd.free()
+        Xd.free()
 
 
 def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, upper_bound, **kwargs):
@@ -397,7 +492,9 @@ def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, 
     posterior's own derivatives w.r.t. the test input (b2gp_posterior_grad: one posterior call per evaluation, value and
     gradient together).  On a viDKL or DKL with single-channel targets the posterior's gradient w.r.t. the embedding is
     pulled back through the network to the raw input (b2gp_dkl_posterior_grad, one call per evaluation); viDKL's single
-    weight set keeps the factor of the training embedding cached across the evaluations.  Every other acquisition (KG,
+    weight set keeps the factor of the training embedding cached across the evaluations.  On a one-output BNN the
+    network's gradient w.r.t. the input comes from b2gp_bnn_predict_grad, one call per evaluation with the weight sets
+    resident on the device for the whole run.  Every other acquisition (KG,
     Thompson, the q-batch functions, penalties, user callables), model (mean functions, viMTDKL, multi-channel viDKL,
     iBNN, other subclasses) is handed to L-BFGS-B without a gradient: SciPy then takes finite differences, d + 1
     posterior calls per gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
@@ -416,13 +513,14 @@ def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, 
     bounds = list(zip(np.broadcast_to(lower_bound, (d,)).astype(float), np.broadcast_to(upper_bound, (d,)).astype(float)))
     kind = _analytic_kind(acq_fn, model, kwargs)
     if kind is not None:
-        f = _analytic_objective(kind, rng_key, model, d, kwargs)
-
-        def fun(x):
-            v, g = f(x)
-            return -float(v), -np.asarray(g, np.float64).reshape(-1)
-        res = minimize(fun, np.asarray(x0, np.float64).reshape(-1), jac=True, method="L-BFGS-B", bounds=bounds,
-                       options={"maxiter": 500})
+        objective = (_bnn_objective(kind, rng_key, model, d, kwargs) if _is_bnn(model)
+                     else contextlib.nullcontext(_analytic_objective(kind, rng_key, model, d, kwargs)))
+        with objective as f:
+            def fun(x):
+                v, g = f(x)
+                return -float(v), -np.asarray(g, np.float64).reshape(-1)
+            res = minimize(fun, np.asarray(x0, np.float64).reshape(-1), jac=True, method="L-BFGS-B", bounds=bounds,
+                           options={"maxiter": 500})
     else:
         def fun(x):   # optimize.py:70-74
             x = np.array([x]).reshape(1, -1)

@@ -227,17 +227,23 @@ class BNN:
         return loc[0], y[0]
 
     def predict(self, rng_key, X_new, samples: Optional[Dict[str, np.ndarray]] = None, n: int = 1, filter_nans: bool = False,
-                take_point_predictions_mean: bool = True, device=None) -> Tuple[np.ndarray, np.ndarray]:
+                take_point_predictions_mean: bool = True, device=None, noiseless: bool = False) -> Tuple[np.ndarray, np.ndarray]:
         """spm.py:173-208: (mean over draws of loc [P, O], or loc [S, P, O] without take_point_predictions_mean; y_sampled
         [S, P, O]).  Draw s uses the s-th key of jax.random.split(rng_key, S) and jax.random.normal(key, (n, P, O)); the
-        whole batch of draws is one b2gp_bnn_predict call."""
+        whole batch of draws is one b2gp_bnn_predict call.  noiseless=True (not in the reference; the analogue of the GP's
+        noiseless predictive, which the acquisition functions pass on) returns y_sampled = loc: the network's output
+        without the observation noise, and draws no normals."""
         X_new = self._set_data(X_new)
         if samples is None:
             samples = self.get_samples(chain_dim=False)
         flat = np.atleast_2d(self.to_flat(samples))
         S, Pn, O = flat.shape[0], X_new.shape[0], self.output_dim
-        eps = posterior_eps(rng_key, S, int(n), Pn * O, _eps_dtype()).reshape(S, int(n), Pn, O)
-        y_pred, y_sampled = self._predict_draws(X_new, flat, np.asarray(samples["noise"]).reshape(S), eps)
+        if noiseless:
+            y_pred, _ = self._predict_draws(X_new, flat)
+            y_sampled = y_pred.copy()
+        else:
+            eps = posterior_eps(rng_key, S, int(n), Pn * O, _eps_dtype()).reshape(S, int(n), Pn, O)
+            y_pred, y_sampled = self._predict_draws(X_new, flat, np.asarray(samples["noise"]).reshape(S), eps)
         if filter_nans:
             y_sampled = y_sampled[[i for i in range(S) if not np.isnan(y_sampled[i]).any()]]
         if take_point_predictions_mean:

@@ -2421,6 +2421,7 @@ static int bnn_optin(b2gp_ctx* ctx) {
         CUDA_TRY(ctx, cudaFuncSetAttribute(bnn_loglik_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)(ctx->smem_optin - 8 * BNN_THREADS)));
         CUDA_TRY(ctx, cudaFuncSetAttribute(bnn_predict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin));
+        CUDA_TRY(ctx, cudaFuncSetAttribute(bnn_predict_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin));
         attr.done(ctx->device);
     }
     return B2GP_OK;
@@ -2529,6 +2530,90 @@ extern "C" int b2gp_bnn_predict(b2gp_ctx* ctx, const double* X, int64_t P, int64
     }
     CUDA_TRY(ctx, cudaMemcpyAsync(loc, dloc, (size_t)S * PO * 8, cudaMemcpyDeviceToHost, st));
     if (eps) CUDA_TRY(ctx, cudaMemcpyAsync(y_sampled, dys, (size_t)S * PO * 8, cudaMemcpyDeviceToHost, st));
+    RET_IF(tm.end(st, nullptr));
+    return B2GP_OK;
+}
+
+// hidden activations the layered route of b2gp_bnn_predict_grad keeps at once (doubles, 1 GiB): draws are taken in
+// chunks that stay under it
+constexpr int64_t BNN_GRAD_KEEP = (int64_t)1 << 27;
+
+// loc[s] = MLP(X; weight set s) for a one-output network and dloc[s, p, :] = d loc[s, p] / d X[p, :]: one launch per
+// 65535 draws on the fused route (bnn_predict_grad_kernel); on the layered one the DKL forward pass per draw keeps the
+// hidden activations of a chunk of draws and one mlp_input_vjp_kernel launch per chunk pulls the unit cotangent back.
+extern "C" int b2gp_bnn_predict_grad(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int n_layers, const int64_t* widths,
+                                     int act, const double* params, int64_t S, int64_t params_stride, double* loc, double* dloc,
+                                     unsigned flags) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_bnn_predict_grad", "fp64 arrays only", __FILE__, __LINE__);
+    MlpShape s;
+    RET_IF(mlp_shape(ctx, P, D, n_layers, widths, act, s));
+    ARG_CHECK(ctx, X && params && loc && dloc && n_layers >= 1 && s.d == 1 && S >= 1 && params_stride >= s.nparams);
+    ARG_CHECK(ctx, D <= (int64_t)VJP_TILE * 65535);
+    CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+    ctx->fcache.valid = false;
+    cudaStream_t st = ctx->slots[0].stream;
+    CallTimer tm(ctx);
+    RET_IF(tm.begin(st));
+    const bool dev = dev_ptrs(flags);
+    const double *dX, *dP;
+    RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)P * D * 8, dev, &dX));
+    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)((S - 1) * params_stride + s.nparams) * 8, dev, &dP));
+    const int64_t nloc = round_up(S * P, 8);
+    RET_IF(ensure(ctx, ctx->d_out[0], (size_t)(nloc + S * P * D) * 8));
+    double* dl = (double*)ctx->d_out[0].p;
+    double* ddl = dl + nloc;
+    std::vector<double> ones;   // the layered route's cotangents; alive until the copies that read it are done
+    const size_t smem = ctx->bnn_fused ? bnn_fused_smem(D, n_layers, widths, false, ctx->smem_optin) : 0;
+    if (smem) {
+        RET_IF(bnn_optin(ctx));
+        const BnnNet net = bnn_net(D, n_layers, widths);
+        for (int64_t s0 = 0; s0 < S; s0 += 65535) {   // grid.y holds at most 65535 draws
+            const dim3 grid((unsigned)ceil_div(P, BNN_ROWS), (unsigned)std::min<int64_t>(S - s0, 65535));
+            RET_IF(launch(ctx, st, grid, BNN_THREADS, smem, bnn_predict_grad_kernel, net, act, dX, P, dP, params_stride, dl, ddl, s0));
+        }
+    } else {
+        // mlp[3]: the hidden activations H_1 .. H_{L-1} of a chunk of draws (mlp_forward_dev's layout) | ones [chunk, P] |
+        // the kernel's G buffers when they do not fit in shared memory
+        const int L = n_layers;
+        int64_t hstride = 0, wmax = 0;
+        for (int l = 0; l + 1 < L; ++l) hstride += round_up(P * s.out[l], 8);
+        for (int l = 0; l < L; ++l) wmax = std::max(wmax, s.out[l]);
+        const int64_t chunk = std::min<int64_t>({S, std::max<int64_t>(1, BNN_GRAD_KEEP / std::max<int64_t>(hstride, 1)),
+                                                 std::max<int64_t>(1, (int64_t)INT_MAX / P)});
+        const size_t vsm = (size_t)2 * VJP_MAX_R * wmax * 8;
+        const bool use_smem = vsm <= VJP_SMEM_MAX;
+        const int64_t ntile = ceil_div(D, (int64_t)VJP_TILE);
+        const int64_t o_one = round_up(chunk * hstride, 8), o_g = o_one + round_up(chunk * P, 8);
+        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(o_g + (use_smem ? 0 : chunk * P * ntile * 2 * VJP_MAX_R * wmax)) * 8));
+        double* work = (double*)ctx->mlp[3].p;
+        ones.assign((size_t)chunk * P, 1.0);
+        CUDA_TRY(ctx, cudaMemcpyAsync(work + o_one, ones.data(), (size_t)chunk * P * 8, cudaMemcpyHostToDevice, st));
+        VjpNet net{};
+        net.L = L;
+        net.R = 1;
+        net.width[0] = D;
+        for (int l = 0; l < L; ++l) {
+            net.width[l + 1] = s.out[l];
+            net.woff[l] = s.woff[l];
+        }
+        std::vector<double*> H;
+        for (int64_t c0 = 0; c0 < S; c0 += chunk) {
+            const int64_t nc = std::min(chunk, S - c0);
+            for (int64_t m = c0; m < c0 + nc; ++m) {
+                RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP + m * params_stride, H));
+                if (hstride > 0)
+                    CUDA_TRY(ctx, cudaMemcpyAsync(work + (m - c0) * hstride, H[1], (size_t)hstride * 8, cudaMemcpyDeviceToDevice, st));
+                CUDA_TRY(ctx, cudaMemcpyAsync(dl + m * P, H[L], (size_t)P * 8, cudaMemcpyDeviceToDevice, st));
+            }
+            const dim3 grid((unsigned)(nc * P), (unsigned)ntile);
+            RET_IF(launch(ctx, st, grid, VJP_THREADS, use_smem ? vsm : 0, mlp_input_vjp_kernel, net, dP + c0 * params_stride,
+                          params_stride, (const double*)work, hstride, P, act, (const double*)(work + o_one), (const double*)nullptr,
+                          ddl + c0 * P * D, use_smem ? (double*)nullptr : work + o_g, wmax));
+        }
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(loc, dl, (size_t)S * P * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(dloc, ddl, (size_t)S * P * D * 8, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
     return B2GP_OK;
 }

@@ -19,6 +19,13 @@
 // loc[s, p, :] and, given eps, y[s, p, :] = loc + sigma_s * (sum_k eps[s, k, p, :]) / n (k in order): spm.py:150-154,
 // Normal(loc, sigma).sample(key, (n,)).mean(0).
 //
+// bnn_predict_grad_kernel: the same grid and forward pass for a one-output network, then d loc / dX per row: the unit
+// cotangent at the output, G <- (G W_l^T) * act'(H_l) in place over the activations for l = L-1 .. 1 (the likelihood
+// kernel's step, bnn_tile_pullback) and dX = G W_0^T into the input buffer.  Every element has one owning thread and a
+// fixed order: identical calls give identical bits.  Its shared memory is predict's, so it runs wherever predict runs
+// fused; otherwise b2gp_bnn_predict_grad keeps the layered forward pass's hidden activations and runs dkl.cuh's
+// mlp_input_vjp_kernel with unit cotangents.
+//
 // Route rule (bnn_fused_smem): the fused kernels run when 8 * (W + T) bytes fit in the device's opt-in shared memory
 // per block (227 KB on the H100), with W = 2 * nparams for the likelihood (weights + gradient accumulator) and nparams
 // for predict, T = BNN_ROWS * sum_l ld_l one tile's activations (ld_l = width_l rounded up to odd, for conflict-free
@@ -103,6 +110,29 @@ static __device__ void bnn_tile_forward(const BnnNet& net, int act, const double
     }
 }
 
+// one step of the tile's backward pass below layer l: G W_l^T with G = H[l+1], written in place over H[l] and masked by
+// act'(H[l]) when MASK (the lanes of a warp take the 32 rows of one k: W[k, j] is a broadcast and G, H_l are read at the
+// odd row stride, so the loop is free of bank conflicts; lanes along k would read W at a stride of `out` doubles).  Each
+// element is read and written by one thread, in a fixed order over j.
+template <bool MASK>
+static __device__ __forceinline__ void bnn_tile_pullback(const BnnNet& net, int act, const double* Ws, double* H, int l) {
+    const int in = net.dims[l], out = net.dims[l + 1], li = net.ld[l], lo = net.ld[l + 1];
+    double* Hin = H + net.hoff[l];
+    const double* G = H + net.hoff[l + 1];
+    const double* W = Ws + net.woff[l];
+    for (int idx = threadIdx.x; idx < BNN_ROWS * in; idx += BNN_THREADS) {
+        const int k = idx / BNN_ROWS, r = idx % BNN_ROWS;
+        double s = 0.0;
+        for (int j = 0; j < out; ++j) s = fma(G[r * lo + j], W[k * out + j], s);
+        if (MASK) {
+            const double h = Hin[r * li + k];
+            Hin[r * li + k] = act == B2GP_ACT_RELU ? (h > 0.0 ? s : 0.0) : s * (1.0 - h * h);
+        } else {
+            Hin[r * li + k] = s;
+        }
+    }
+}
+
 // stage the tile's input rows (zero beyond `rows`)
 static __device__ void bnn_stage_x(const BnnNet& net, const double* __restrict__ X, int64_t row0, int64_t rows, double* H) {
     const int D = net.dims[0];
@@ -164,16 +194,7 @@ bnn_loglik_tile_kernel(const BnnNet net, int act, const double* __restrict__ X, 
             }
             __syncthreads();
             if (l == 0) break;
-            const double* W = Ws + net.woff[l];
-            // the lanes of a warp take the 32 rows of one k: W[k, j] is a broadcast and G, H_l are read at the odd row
-            // stride, so the loop is free of bank conflicts (lanes along k would read W at a stride of `out` doubles)
-            for (int idx = threadIdx.x; idx < BNN_ROWS * in; idx += BNN_THREADS) {
-                const int k = idx / BNN_ROWS, r = idx % BNN_ROWS;
-                double s = 0.0;
-                for (int j = 0; j < out; ++j) s = fma(G[r * lo + j], W[k * out + j], s);
-                const double h = Hin[r * li + k];
-                Hin[r * li + k] = act == B2GP_ACT_RELU ? (h > 0.0 ? s : 0.0) : s * (1.0 - h * h);
-            }
+            bnn_tile_pullback<true>(net, act, Ws, H, l);
             __syncthreads();
         }
     }
@@ -226,6 +247,41 @@ bnn_predict_kernel(const BnnNet net, int act, const double* __restrict__ X, int6
     for (int idx = threadIdx.x; idx < BNN_ROWS * O; idx += BNN_THREADS) {
         const int r = idx / O, o = idx % O;
         if (row0 + r < Pn) bnn_sample_out(Z[r * lz + o], s, row0 * O + idx, Pn * O, sigma, eps, n, loc, ys);
+    }
+}
+
+// bnn_predict_kernel's grid and forward pass for a one-output network, then the gradient of loc w.r.t. the inputs:
+// the unit cotangent seeds the (linear) output layer, bnn_tile_pullback runs down the layers over the activations and
+// dX = G W_0^T lands in the input buffer, free by then.  Writes loc[s, p] (bit-identical to bnn_predict_kernel's) and
+// dloc[s, p, :].  Same shared memory as predict: the weights and one tile.
+__global__ void __launch_bounds__(BNN_THREADS)
+bnn_predict_grad_kernel(const BnnNet net, int act, const double* __restrict__ X, int64_t Pn, const double* __restrict__ P,
+                        int64_t stride, double* __restrict__ loc, double* __restrict__ dloc, int64_t s0) {
+    extern __shared__ double sm[];
+    double* Ws = sm;
+    double* H = sm + net.nparams;
+    const int64_t s = s0 + blockIdx.y, row0 = (int64_t)blockIdx.x * BNN_ROWS;
+    for (int i = threadIdx.x; i < net.nparams; i += BNN_THREADS) Ws[i] = P[s * stride + i];
+    bnn_stage_x(net, X, row0, Pn, H);
+    __syncthreads();
+    bnn_tile_forward(net, act, Ws, H);
+    if (threadIdx.x < BNN_ROWS) {
+        double* z = H + net.hoff[net.L] + threadIdx.x * net.ld[net.L];
+        if (row0 + threadIdx.x < Pn) loc[s * Pn + row0 + threadIdx.x] = *z;
+        *z = 1.0;
+    }
+    __syncthreads();
+    for (int l = net.L - 1; l >= 1; --l) {
+        bnn_tile_pullback<true>(net, act, Ws, H, l);
+        __syncthreads();
+    }
+    bnn_tile_pullback<false>(net, act, Ws, H, 0);
+    __syncthreads();
+    const int D = net.dims[0];
+    const int64_t rows = Pn - row0 < BNN_ROWS ? Pn - row0 : BNN_ROWS;
+    for (int idx = threadIdx.x; idx < rows * D; idx += BNN_THREADS) {
+        const int r = idx / D, k = idx % D;
+        dloc[(s * Pn + row0) * D + idx] = H[r * net.ld[0] + k];
     }
 }
 

@@ -437,6 +437,18 @@ int  b2gp_bnn_predict(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int 
                       const double* params, int64_t S, int64_t params_stride, int64_t O, const double* sigma,
                       const double* eps, int64_t n, double* loc, double* y_sampled, unsigned flags);
 
+/* b2gp_bnn_predict_grad: loc[s] = MLP(X; params + s * params_stride) for S weight sets of a one-output network
+ *   (widths[n_layers-1] = 1, else B2GP_ERR_ARG), [S,P], and its gradient w.r.t. the inputs, dloc[s,p,k] = d loc[s,p] /
+ *   d X[p,k], [S,P,D] -- what optimize_acq needs of a BNN at each evaluation.  X and params follow `flags`: under
+ *   B2GP_FLAG_DEVICE_PTRS both are device pointers, so the weight sets can stay resident across calls; B2GP_FLAG_F32 gives
+ *   B2GP_ERR_UNSUPPORTED.  widths and both outputs are HOST pointers.  Every argument is checked before any launch.
+ *   loc is bit-identical to b2gp_bnn_predict's on the same route.  Fused exactly where b2gp_bnn_predict is (one launch
+ *   per 65535 draws: the forward pass, then the backward recursion over the tile's activations); otherwise the
+ *   b2gp_mlp_forward pass per draw and one input vector-Jacobian product launch per chunk of draws whose hidden
+ *   activations fit in 1 GiB.  Deterministic: identical calls give identical bits.                                     */
+int  b2gp_bnn_predict_grad(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int n_layers, const int64_t* widths, int act,
+                           const double* params, int64_t S, int64_t params_stride, double* loc, double* dloc, unsigned flags);
+
 /* Samples of S multivariate normals: y[s,i,:] = mean[s,:] + chol(cov[s]) eps[s,i,:], i < n -- replaces
  * numpyro.distributions.MultivariateNormal(mean, cov).sample (gpax/models/gp.py:292, gpax/acquisition/base_acq.py:221)
  * where the caller changed cov after the posterior call (gpax/models/hskgp.py:201-204 adds the predicted noise variance).
