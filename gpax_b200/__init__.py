@@ -14,11 +14,13 @@ from .mtgp import CoregGP, MultiTaskGP
 from .dkl import DKL, viDKL, viMTDKL
 from .ibnn import iBNN, vi_iBNN
 from .bnn import BNN
-from . import acquisition, mtkernels
+from .spm import sPM
+from .hypo import sample_next
+from . import acquisition, diagnostics, hypo, mtkernels
 from .kernels import NNGPKernel
 from .mtkernels import LCMKernel, MultitaskKernel, MultivariateKernel
 from ._ffi import B200GPError, Context, default_context
 
 __version__ = "0.1.0"
-__all__ = ["ExactGP", "iBNN", "vi_iBNN", "BNN", "DKL", "viDKL", "viMTDKL", "MultiTaskGP", "CoregGP", "viGP", "viSparseGP", "MeasuredNoiseGP", "VarNoiseGP", "vExactGP", "UIGP", "acquisition", "RBFKernel", "MaternKernel", "PeriodicKernel", "NNGPKernel", "MultitaskKernel", "MultivariateKernel", "LCMKernel", "mtkernels", "get_kernel",
+__all__ = ["ExactGP", "iBNN", "vi_iBNN", "BNN", "sPM", "sample_next", "DKL", "viDKL", "viMTDKL", "MultiTaskGP", "CoregGP", "viGP", "viSparseGP", "MeasuredNoiseGP", "VarNoiseGP", "vExactGP", "UIGP", "acquisition", "RBFKernel", "MaternKernel", "PeriodicKernel", "NNGPKernel", "MultitaskKernel", "MultivariateKernel", "LCMKernel", "mtkernels", "get_kernel",
            "kernels", "utils", "Context", "default_context", "B200GPError"]

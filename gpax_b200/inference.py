@@ -208,11 +208,15 @@ class ProgramLogJoint:
         if model.mean_fn is not None and not self.has_mean_params:
             self.fixed_mean = np.asarray(model.mean_fn(X), dtype=np.float64).squeeze()
         self._lik_fn = lik
+        self._find_sites()
+        self.n_evals = 0
+
+    def _find_sites(self):
+        """the model program's sites, the dimension of u, and whether any site's distribution depends on the values of
+        the others (two runs at different values)"""
         _, sites, _ = P.run_program(self._model_program)
         self.sites = list(sites.values())
         self.dim = sum(s.size for s in self.sites)
-        self.n_evals = 0
-        # does any site's distribution depend on the values of the others?  (two runs at different values)
         vals = {s.name: np.asarray(s.prior.transform(np.full(s.shape, 0.37))) for s in self.sites}
         _, sites2, _ = P.run_program(self._model_program, vals)
         self.hierarchical = any(vars(sites[k].prior) != vars(sites2[k].prior) for k in sites)
@@ -220,13 +224,17 @@ class ProgramLogJoint:
     def _model_program(self):
         return gp_model_program(self.m, self.d, self.kind)
 
-    def _program_at(self, u):
-        """u -> the model program's (kernel-parameter dict, noise, mean-function parameters) and its sites with values"""
+    def _site_values(self, u):
+        """u -> {site name: constrained value, shaped as the program sampled it}"""
         vals, o = {}, 0
         for s in self.sites:
             vals[s.name] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
             o += s.size
-        (kp, noise, mp), sites, _ = P.run_program(self._model_program, vals)
+        return vals
+
+    def _program_at(self, u):
+        """u -> the model program's (kernel-parameter dict, noise, mean-function parameters) and its sites with values"""
+        (kp, noise, mp), sites, _ = P.run_program(self._model_program, self._site_values(u))
         return kp, noise, mp, sites
 
     def _run(self, u):
@@ -502,11 +510,7 @@ class MTLogJoint(ProgramLogJoint):
         return self.m._model_program(self.T, self.R, self.L)
 
     def _run(self, u):
-        vals, o = {}, 0
-        for s in self.sites:
-            vals[s.name] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
-            o += s.size
-        (kp, noise, mp), sites, _ = P.run_program(self._model_program, vals)
+        (kp, noise, mp), sites, _ = P.run_program(self._model_program, self._site_values(u))
         theta, B, nz = self.m._pack(dict(kp, noise=noise), batched=False)
         p = np.concatenate([theta.ravel(), B.ravel(), nz.ravel()])
         mean = None
