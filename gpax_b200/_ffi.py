@@ -91,6 +91,9 @@ SIGNATURES = {
     "b2gp_posterior_multitask": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int, C.c_int,
                                            C.c_int, C.c_int, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_double, C.c_uint, _vp, _vp, _vp,
                                            _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
+    "b2gp_posterior_multitask_grad": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64, C.c_int,
+                                                C.c_int, C.c_int, C.c_int, C.c_int64, _vp, _vp, _vp, C.c_int, C.c_double, C.c_uint,
+                                                _vp, _vp, _vp, _vp, _vp, C.POINTER(Timing)]),
     "b2gp_mll_multitask": (C.c_int, [_vp, C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp,
                                      C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _ip]),
     "b2gp_mll_v": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _ip]),
@@ -623,6 +626,36 @@ class Context:
             P, d, int(group), T, L, S, _ptr(theta), _ptr(B), _ptr(noise), int(bool(noiseless)), float(jitter), flags, _ptr(mean),
             _ptr(var), _ptr(cov), _ptr(eps), n_samp, _ptr(samp), info.ctypes.data_as(_vp), C.byref(t) if timing else None))
         out = {"mean": mean, "var": var, "cov": cov, "y_sampled": samp, "info": info}
+        if timing:
+            out["timing"] = t.as_dict()
+        return out
+
+    def posterior_multitask_grad(self, kind, Xtr, task_tr, yres, Xnew, task_new, theta, B, noise, group=1, noiseless=False,
+                                 jitter=1e-6, want=("mean", "var", "dmean", "dvar"), timing=False, flags=0):
+        """The LCM posterior and its gradients w.r.t. the test inputs (b2gp_posterior_multitask_grad).  Arguments as
+        posterior_multitask().  Returns a dict with mean / var [S, P], dmean / dvar [S, P, d] (None where not in `want`)
+        and info [S]."""
+        Xtr, Xnew = _f64(Xtr), _f64(Xnew)
+        N, d = Xtr.shape
+        P = Xnew.shape[0]
+        B = _f64(B)
+        S, L, T = B.shape[0], B.shape[1], B.shape[2]
+        theta, noise = _f64(theta, (S, L, d + 2)), _f64(noise, (S, T))
+        ttr, tnew = np.ascontiguousarray(task_tr, dtype=np.int32), np.ascontiguousarray(task_new, dtype=np.int32)
+        yres = _f64(yres)
+        stride = 0 if yres.ndim == 1 else yres.shape[1]
+        bits = {"mean": (OUT_MEAN, (S, P)), "var": (OUT_VAR, (S, P)), "dmean": (OUT_DMEAN, (S, P, d)), "dvar": (OUT_DVAR, (S, P, d))}
+        out = {}
+        for name, (bit, shape) in bits.items():
+            out[name] = np.empty(shape) if name in want else None
+            flags |= bit if name in want else 0
+        info = np.zeros(S, dtype=np.int32)
+        t = Timing()
+        self._check(self.lib.b2gp_posterior_multitask_grad(
+            self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(Xtr), _ptr(ttr), N, _ptr(yres), stride, _ptr(Xnew), _ptr(tnew),
+            P, d, int(group), T, L, S, _ptr(theta), _ptr(B), _ptr(noise), int(bool(noiseless)), float(jitter), flags, _ptr(out["mean"]),
+            _ptr(out["var"]), _ptr(out["dmean"]), _ptr(out["dvar"]), info.ctypes.data_as(_vp), C.byref(t) if timing else None))
+        out["info"] = info
         if timing:
             out["timing"] = t.as_dict()
         return out

@@ -395,17 +395,22 @@ def _analytic_kind(acq_fn, model, kwargs):
     A plain ExactGP or viGP qualifies: their predict() is the exact-GP posterior that b2gp_posterior_grad
     differentiates.  So do a plain viDKL or DKL with single-channel targets: their predict() is that posterior on the
     network's embedding, which b2gp_dkl_posterior_grad differentiates w.r.t. the raw inputs.  So does a one-output BNN:
-    its samples are loc + sigma * (mean noise draw) per weight draw, and b2gp_bnn_predict_grad differentiates loc.  Every
-    other subclass (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, viMTDKL, iBNN, or a user's own) predicts
-    something else, so it takes the finite-difference branch even though it inherits _posterior_grad; so does a
-    multi-channel viDKL."""
+    its samples are loc + sigma * (mean noise draw) per weight draw, and b2gp_bnn_predict_grad differentiates loc.  So
+    does a MultiTaskGP in the multitask form (task id in the last column) or a CoregGP, without a mean function: their
+    predict() at one point is the LCM posterior that b2gp_posterior_multitask_grad differentiates.  Every other subclass
+    (viSparseGP, MeasuredNoiseGP, VarNoiseGP, vExactGP, UIGP, viMTDKL, iBNN, or a user's own) predicts something else,
+    so it takes the finite-difference branch even though it inherits _posterior_grad; so do a multi-channel viDKL and
+    a MultiTaskGP in the Kronecker form."""
     from .bnn import BNN
     from .dkl import DKL, viDKL
     from .gp import ExactGP
+    from .mtgp import CoregGP, MultiTaskGP
     from .vigp import viGP
     kind = {EI: "EI", UCB: "UCB", POI: "POI", UE: "UE"}.get(acq_fn)
     if kind is not None and not kwargs.get("penalty") and type(model) is BNN:
         return kind if model.output_dim == 1 else None
+    if kind is not None and not kwargs.get("penalty") and type(model) in (MultiTaskGP, CoregGP):
+        return kind if not model.shared_input and model.mean_fn is None else None
     if kind is None or kwargs.get("penalty") or type(model) not in (ExactGP, viGP, viDKL, DKL):
         return None
     if model.mean_fn is not None or model._fused is None:
@@ -432,8 +437,8 @@ def _analytic_args(kind, kwargs):
 
 
 def _analytic_objective(kind, rng_key, model, d, kwargs):
-    """x [d] -> (acq(x), d acq / dx) through one model._posterior_grad call per evaluation (b2gp_posterior_grad, or
-    b2gp_dkl_posterior_grad for viDKL / DKL)"""
+    """x [d] -> (acq(x), d acq / dx) through one model._posterior_grad call per evaluation (b2gp_posterior_grad,
+    b2gp_dkl_posterior_grad for viDKL / DKL, or b2gp_posterior_multitask_grad for MultiTaskGP / CoregGP)"""
     from .gp import _eps_dtype
     kw, n, noiseless, maximize, best_f, param = _analytic_args(kind, kwargs)
     mcmc = getattr(model, "mcmc", None) is not None
@@ -494,10 +499,12 @@ def optimize_acq(rng_key, model, acq_fn, num_initial_guesses: int, lower_bound, 
     pulled back through the network to the raw input (b2gp_dkl_posterior_grad, one call per evaluation); viDKL's single
     weight set keeps the factor of the training embedding cached across the evaluations.  On a one-output BNN the
     network's gradient w.r.t. the input comes from b2gp_bnn_predict_grad, one call per evaluation with the weight sets
-    resident on the device for the whole run.  Every other acquisition (KG,
-    Thompson, the q-batch functions, penalties, user callables), model (mean functions, viMTDKL, multi-channel viDKL,
-    iBNN, other subclasses) is handed to L-BFGS-B without a gradient: SciPy then takes finite differences, d + 1
-    posterior calls per gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
+    resident on the device for the whole run.  On a MultiTaskGP in the multitask form or a CoregGP the LCM posterior's
+    gradient comes from b2gp_posterior_multitask_grad, one call per evaluation, with 0 on the task column (the
+    reference's astype(int) passes no gradient; fix the task by equal lower and upper bounds).  Every other acquisition
+    (KG, Thompson, the q-batch functions, penalties, user callables), model (mean functions, viMTDKL, multi-channel
+    viDKL, the Kronecker form of MultiTaskGP, iBNN, other subclasses) is handed to L-BFGS-B without a gradient: SciPy
+    then takes finite differences, d + 1 posterior calls per gradient.  Returns the maximiser with the shape of the reference's `result.params`: that of the squeezed best initial
     guess, [d], or a 0-d array in one dimension."""
     from scipy.optimize import minimize
     from .utils import x64_enabled

@@ -640,8 +640,9 @@ struct GramPost {
 // The posterior with everything that may vary per draw: the training inputs (xtr_stride doubles between draws; 0 =
 // shared), the test inputs (xnew_stride), the targets (yres_stride) and an optional vector of per-point noise variances
 // added to the diagonal of k_XX (nv_stride between draws; 0 = shared).  b2gp_posterior is the all-shared special case.
-// With B2GP_OUT_DMEAN / B2GP_OUT_DVAR (b2gp_posterior_grad only) the P*d derivative rows of grad.cuh ride under
-// [k_pX; y^T] through the same factorisation or solve, and dmean / dvar [S, P, d] are their row dots.
+// With B2GP_OUT_DMEAN / B2GP_OUT_DVAR (b2gp_posterior_grad and b2gp_posterior_multitask_grad only) the P*d derivative
+// rows of grad.cuh (gram_dx_lcm_kernel, mtgp.cuh, for the LCM covariance) ride under [k_pX; y^T] through the same
+// factorisation or solve, and dmean / dvar [S, P, d] are their row dots.
 static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xtr_stride, int64_t N, const double* yres,
                           int64_t yres_stride, const double* Xnew, int64_t xnew_stride, int64_t P, int d, int64_t S,
                           const double* theta, const double* noise_vec, int64_t nv_stride, int noiseless, double jitter,
@@ -871,7 +872,10 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
             else
                 RET_IF(launch_gram(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, 0.0, 0.0, 0, 0, Vt, ldV));
             CUDA_TRY(ctx, cudaMemcpyAsync(Vt + P * ldV, dy + (yres_stride ? s * yres_stride : 0), (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
-            if (G) RET_IF(launch_gram_dx(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, Vt + (P + 1) * ldV, ldV));
+            if (G && mt)
+                RET_IF(launch_gram_dx_lcm(ctx, st, kind, dXnew_s, dtn, P, dXtr_s, dtr, N, d, T, L, th, Bs, Vt + (P + 1) * ldV, ldV));
+            else if (G)
+                RET_IF(launch_gram_dx(ctx, st, kind, dXnew_s, P, dXtr_s, N, d, th, Vt + (P + 1) * ldV, ldV));
             return B2GP_OK;
         };
         if (front) {
@@ -1083,7 +1087,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
     const double n = (double)N, p = (double)P;
     t.flops = (double)S * (n * n * n / 3.0 + n * n * (p + 1.0) + 4.0 * n * p + (need_cov ? n * p * p : 0.0));
     t.gram_bytes = (double)S * (8.0 * n * n / 2.0 + 8.0 * n * p + (need_cov ? 8.0 * p * p : 0.0));
-    if (G) {   // the derivative rows: their solve and row dots, and the bytes gram_dx_kernel writes
+    if (G) {   // the derivative rows: their solve and row dots, and the bytes gram_dx_kernel / gram_dx_lcm_kernel write
         t.flops += (double)S * (n * n * (double)G + 4.0 * n * (double)G);
         t.gram_bytes += (double)S * 8.0 * n * (double)G;
     }
@@ -1173,6 +1177,25 @@ extern "C" int b2gp_posterior_multitask(b2gp_ctx* ctx, int kind, const double* X
     return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter,
                           flags & ~(unsigned)(B2GP_OUT_DMEAN | B2GP_OUT_DVAR), mean, var, cov, eps, n_samp, y_sampled, info, timing,
                           nullptr, nullptr, &mt);
+}
+
+// The multi-task posterior and its gradient w.r.t. the test inputs: b2gp_posterior_multitask's call with the derivative
+// rows of gram_dx_lcm_kernel (mtgp.cuh) solved alongside k_pX.  Host fp64 arrays, no covariance or samples.
+extern "C" int b2gp_posterior_multitask_grad(b2gp_ctx* ctx, int kind, const double* Xtr, const int* task_tr, int64_t N,
+                                             const double* yres, int64_t yres_stride, const double* Xnew, const int* task_new,
+                                             int64_t P, int d, int group, int T, int L, int64_t S, const double* theta,
+                                             const double* B, const double* noise, int noiseless, double jitter, unsigned flags,
+                                             double* mean, double* var, double* dmean, double* dvar, int* info,
+                                             b2gp_timing* timing) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (flags & (B2GP_FLAG_F32 | B2GP_FLAG_DEVICE_PTRS | B2GP_OUT_COV | B2GP_OUT_SAMPLE))
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_posterior_multitask_grad",
+                       "host fp64 arrays, outputs mean / var / dmean / dvar only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, B && noise && task_new && N >= 1 && P >= 1);
+    RET_IF(mt_check(ctx, "b2gp_posterior_multitask_grad", kind, flags, d, group, T, L, task_tr, N, task_new, P));
+    const MtDesc mt{task_tr, task_new, group, T, L, B, noise};
+    return posterior_impl(ctx, kind, Xtr, 0, N, yres, yres_stride, Xnew, 0, P, d, S, theta, nullptr, 0, noiseless, jitter, flags, mean,
+                          var, nullptr, nullptr, 0, nullptr, info, timing, dmean, dvar, &mt);
 }
 
 // ------------------------------------------------------------------------------------------ sparse posterior

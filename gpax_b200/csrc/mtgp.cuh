@@ -19,10 +19,14 @@
 // the lower triangle and the same thread -> entry map (a thread's column j, and so t_j, is fixed), k_q recomputed on the
 // fly, a fixed-order two-pass reduction (no atomics: deterministic).
 //
+// gram_dx_lcm_kernel writes the derivative rows of k_pX w.r.t. the test inputs (b2gp_posterior_multitask_grad), which
+// the posterior solves under [k_pX; y^T] as it solves grad.cuh's rows for the single-task kernel.
+//
 // Limits: T <= MT_MAX_T tasks, L <= MT_MAX_L latents, d <= MLL_MAX_D input features (checked by the host entries).
 #pragma once
 #include "common.cuh"
 #include "gram.cuh"
+#include "grad.cuh"
 #include "mll.cuh"
 
 constexpr int MT_MAX_T = 8;
@@ -237,6 +241,139 @@ static int launch_gram_lcm(b2gp_ctx* ctx, cudaStream_t st, int mode, int kind, c
     if (mode == LCM_DIAG) return launch(ctx, st, (unsigned)ceil_div(n, (int64_t)GRAM_THREADS), GRAM_THREADS, 0, gram_lcm_kernel, a);
     dim3 grid((unsigned)ceil_div(m, GRAM_BN), (unsigned)ceil_div(n, (int64_t)LCM_BM));
     return launch(ctx, st, grid, GRAM_THREADS, gram_lcm_smem(d, T, L), gram_lcm_kernel, a);
+}
+
+// Derivative rows of the LCM cross-covariance k_pX w.r.t. the test inputs (the multi-task counterpart of grad.cuh's
+// gram_dx_kernel, solved and reduced by the posterior exactly as those rows are):
+//     D[p*d + k, i] = sum_{q=0..L-1} B_q[t_p, t_i] * d k_q(x_p, x_i) / d x_p[k]
+// for every GP row p of the test block (the Kronecker form's repeated rows each w.r.t. their own point: same code).  k_pX
+// carries no jitter or noise term, so nothing else depends on x_p.  d k_q / d x_p is gram_dx_kernel's formula with
+// latent q's lengthscales, scale and period: stationary_dk_dr2 on r2 = (x2 - 2 xz) + z2 of the inputs divided by ell_q
+// (clipped as the Gram clips), or the periodic form with one sincos per dimension.  Each thread owns one column i and
+// GDX_BP / 4 rows; an element's latents are summed in registers in the order q = 0..L-1 and stored once: identical calls
+// give identical bits.  HBM-bound: 8 P d N bytes written.
+constexpr int GDXL_BN = 64;     // training points (columns) per CTA
+constexpr int GDXL_THREADS = 256;
+
+static inline size_t gram_dx_lcm_smem(int d, int T, int L) {
+    return (size_t)(L * d * GDXL_BN + L * GDX_BP * d + L * GDXL_BN + L * GDX_BP + L * (d + 2) + L * T * T) * sizeof(double) +
+           (size_t)(GDX_BP + GDXL_BN) * sizeof(int);
+}
+
+// grid (ceil(N / GDXL_BN), ceil(P / GDX_BP)); dynamic shared memory gram_dx_lcm_smem(d, T, L) (under 48 KB for d <= 16,
+// L <= 4, T <= 8): per latent the scaled columns and rows and their squared norms, theta_q, B_q, the task ids
+__global__ void __launch_bounds__(GDXL_THREADS)
+gram_dx_lcm_kernel(int kind, const double* __restrict__ Xnew, const int* __restrict__ tNew, int64_t P, const double* __restrict__ Xtr,
+                   const int* __restrict__ tTr, int64_t N, int d, int T, int L, const double* __restrict__ theta,
+                   const double* __restrict__ B, double* __restrict__ D, int64_t ldd) {
+    extern __shared__ __align__(16) double sm[];
+    // layout: Zs[L][d][GDXL_BN] | Xs[L][GDX_BP][d] | z2[L][GDXL_BN] | x2[L][GDX_BP] | th[L][d+2] | Bs[L][T][T] | tXs | tZs
+    double* Zs = sm;
+    double* Xs = Zs + L * d * GDXL_BN;
+    double* z2 = Xs + L * GDX_BP * d;
+    double* x2 = z2 + L * GDXL_BN;
+    double* th = x2 + L * GDX_BP;
+    double* Bs = th + L * (d + 2);
+    int* tXs = reinterpret_cast<int*>(Bs + L * T * T);
+    int* tZs = tXs + GDX_BP;
+    const int tid = threadIdx.x, nth = d + 2;
+    const int64_t col0 = (int64_t)blockIdx.x * GDXL_BN, p0 = (int64_t)blockIdx.y * GDX_BP;
+    const bool periodic = (kind == B2GP_KERNEL_PERIODIC);
+    for (int i = tid; i < L * nth; i += GDXL_THREADS) th[i] = theta[i];
+    for (int i = tid; i < L * T * T; i += GDXL_THREADS) Bs[i] = B[i];
+    if (tid < GDX_BP) tXs[tid] = (p0 + tid < P) ? tNew[p0 + tid] : 0;
+    else if (tid < GDX_BP + GDXL_BN) tZs[tid - GDX_BP] = (col0 + tid - GDX_BP < N) ? tTr[col0 + tid - GDX_BP] : 0;
+    __syncthreads();
+    // staged as gram_lcm_kernel stages them: divided by latent q's lengthscale for RBF / Matern, raw for periodic
+    for (int idx = tid; idx < L * GDXL_BN * d; idx += GDXL_THREADS) {
+        const int q = idx / (GDXL_BN * d), k = idx / GDXL_BN % d, c = idx % GDXL_BN;
+        const int64_t gc = col0 + c;
+        const double v = gc < N ? Xtr[gc * d + k] : 0.0;
+        Zs[idx] = periodic ? v : v / th[q * nth + k];
+    }
+    for (int idx = tid; idx < L * GDX_BP * d; idx += GDXL_THREADS) {
+        const int q = idx / (GDX_BP * d), r = idx / d % GDX_BP, k = idx % d;
+        const int64_t gp = p0 + r;
+        const double v = gp < P ? Xnew[gp * d + k] : 0.0;
+        Xs[idx] = periodic ? v : v / th[q * nth + k];
+    }
+    __syncthreads();
+    if (!periodic) {
+        for (int idx = tid; idx < L * (GDXL_BN + GDX_BP); idx += GDXL_THREADS) {
+            const bool col = idx < L * GDXL_BN;
+            const int j = col ? idx : idx - L * GDXL_BN;
+            const int q = col ? j / GDXL_BN : j / GDX_BP, e = col ? j % GDXL_BN : j % GDX_BP;
+            double s = 0.0;
+            for (int k = 0; k < d; ++k) {
+                const double v = col ? Zs[(q * d + k) * GDXL_BN + e] : Xs[(q * GDX_BP + e) * d + k];
+                s = fma(v, v, s);
+            }
+            (col ? z2 : x2)[j] = s;
+        }
+        __syncthreads();
+    }
+    const int c = tid % GDXL_BN;
+    const int64_t gc = col0 + c;
+    if (gc >= N) return;
+    const int tc = tZs[c];
+    for (int r = tid / GDXL_BN; r < GDX_BP; r += GDXL_THREADS / GDXL_BN) {
+        const int64_t gp = p0 + r;
+        if (gp >= P) break;
+        const int tr = tXs[r];
+        double acc[MLL_MAX_D];
+#pragma unroll
+        for (int k = 0; k < MLL_MAX_D; ++k) acc[k] = 0.0;
+        for (int q = 0; q < L; ++q) {
+            const double* ell = th + q * nth;
+            const double scale = ell[d], period = ell[d + 1];
+            const double b = Bs[(q * T + tr) * T + tc];
+            const double* x = Xs + (q * GDX_BP + r) * d;
+            const double* z = Zs + q * d * GDXL_BN + c;      // z[k * GDXL_BN]
+            if (periodic) {
+                // -2 pi sin(2 a_k) / (period l_k^2) = -4 pi sin a_k cos a_k / ..., times k_q once the exponent is known
+                double g[MLL_MAX_D], s = 0.0;
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k) {
+                    if (k < d) {
+                        double sa, ca;
+                        sincos(3.141592653589793 * (x[k] - z[k * GDXL_BN]) / period, &sa, &ca);
+                        const double a = sa / ell[k];                               // kernels.py:111-113
+                        s += a * a;
+                        g[k] = -(4.0 * 3.141592653589793) * sa * ca / (period * ell[k] * ell[k]);
+                    }
+                }
+                const double bk = b * (scale * exp(-2.0 * s));
+#pragma unroll
+                for (int k = 0; k < MLL_MAX_D; ++k)
+                    if (k < d) acc[k] += bk * g[k];
+                continue;
+            }
+            double xz = 0.0;
+            for (int k = 0; k < d; ++k) xz = fma(x[k], z[k * GDXL_BN], xz);
+            const double r2raw = (x2[q * GDX_BP + r] - 2.0 * xz) + z2[q * GDXL_BN + c];   // kernels.py:40
+            const double bg = b * stationary_dk_dr2(kind, r2raw, scale);
+#pragma unroll
+            for (int k = 0; k < MLL_MAX_D; ++k)
+                if (k < d) acc[k] += bg * (2.0 * (x[k] - z[k * GDXL_BN]) / ell[k]);
+        }
+        double* out = D + gp * d * ldd + gc;
+#pragma unroll
+        for (int k = 0; k < MLL_MAX_D; ++k)
+            if (k < d) out[k * ldd] = acc[k];
+    }
+}
+
+// D[P*d, N] (leading dimension ldd) of the LCM cross-covariance for test rows Xnew[P, d] / tNew[P] against Xtr[N, d] /
+// tTr[N], one draw's theta[L, d+2] and B[L, T, T] (device pointers; task ids validated by the caller)
+static int launch_gram_dx_lcm(b2gp_ctx* ctx, cudaStream_t st, int kind, const double* Xnew, const int* tNew, int64_t P,
+                              const double* Xtr, const int* tTr, int64_t N, int d, int T, int L, const double* theta,
+                              const double* B, double* D, int64_t ldd) {
+    if (P <= 0 || N <= 0) return B2GP_OK;
+    if (kind < 0 || kind > B2GP_KERNEL_PERIODIC || d < 1 || d > MLL_MAX_D || T < 1 || T > MT_MAX_T || L < 1 || L > MT_MAX_L)
+        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "gram_dx_lcm", "RBF / Matern / Periodic, d <= 16, T <= 8, L <= 4", __FILE__, __LINE__);
+    dim3 grid((unsigned)ceil_div(N, (int64_t)GDXL_BN), (unsigned)ceil_div(P, (int64_t)GDX_BP));
+    return launch(ctx, st, grid, GDXL_THREADS, gram_dx_lcm_smem(d, T, L), gram_dx_lcm_kernel, kind, Xnew, tNew, P, Xtr, tTr, N, d, T,
+                  L, theta, B, D, ldd);
 }
 
 // var[i] += prior[i]: the posterior variance from rowdot_kernel's -|V^T[i,:]|^2 (run with a zero prior) and the LCM

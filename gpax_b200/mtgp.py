@@ -2,8 +2,8 @@
 mtgp.py -- `MultiTaskGP` and `CoregGP` with the reference's surface (gpax/models/mtgp.py:57-90, gpax/models/corgp.py:38-53):
 exact GPs whose covariance is the linear model of coregionalisation (LCM) of mtkernels.py:197-233.  The posterior is one
 b2gp_posterior_multitask call per predict (the LCM Gram matrices built on the GPU by gram_lcm_kernel, then ExactGP's
-factorisation and solves); `fit` runs the host NUTS on the multi-task log marginal likelihood and its gradient
-(b2gp_mll_multitask).  Both forms of the reference:
+factorisation and solves), and b2gp_posterior_multitask_grad adds its gradient w.r.t. the test inputs; `fit` runs the
+host NUTS on the multi-task log marginal likelihood and its gradient (b2gp_mll_multitask).  Both forms of the reference:
   * multitask form (shared_input_space=False, and CoregGP): one row per observation, its task id in the last column of X;
   * Kronecker form (MultiTaskGP with shared_input_space=True): every task observed at every input, y of length N*T in
     point-major order (point i, task t at i*T + t); predictions have length P*T in the same order.
@@ -124,7 +124,28 @@ class _LCMModel(ExactGP):
         return out
 
     def _posterior_grad(self, X_new, params, batched, noiseless, **kwargs):
-        raise NotImplementedError("multi-task models have no analytic posterior gradient; optimize_acq differences them")
+        """Per-draw posterior mean [S, P], variance [S, P] and their gradients dmean, dvar [S, P, d + 1] w.r.t. the test
+        inputs, task column included (b2gp_posterior_multitask_grad): what jax.grad through the acquisition w.r.t. x needs
+        (optimize.py:70-88).  The task column reaches the kernel through astype(int), whose gradient is 0, so its entries
+        are 0.  Multitask form only: the Kronecker form predicts T values per input, so its acquisition is not one scalar
+        per x.  A mean function (an arbitrary host callable) has no analytic gradient either."""
+        if self.shared_input:
+            raise NotImplementedError("posterior gradients take the multitask form (task id in the last column of X)")
+        if self.mean_fn is not None:
+            raise NotImplementedError("posterior gradients need a model without a mean function")
+        X, y = self._train_arrays()
+        Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
+        Xn = Xn if Xn.ndim > 1 else Xn[:, None]
+        if self._data_dim(X) != self.kernel_dim:
+            raise ValueError(f"X_train has {self._data_dim(X)} input features, the model input_dim={self.kernel_dim}")
+        theta, B, noise = self._pack(params, batched)
+        Xd, ttr, group = self._rows(X)
+        Xnd, tnew, _ = self._rows(Xn)
+        out = self.ctx.posterior_multitask_grad(self._fused, Xd, ttr, y, Xnd, tnew, theta, B, noise, group, noiseless,
+                                                float(kwargs.get("jitter", 1e-6)))
+        dmean, dvar = (np.zeros(out[k].shape[:2] + (Xn.shape[1],)) for k in ("dmean", "dvar"))
+        dmean[..., :-1], dvar[..., :-1] = out["dmean"], out["dvar"]
+        return out["mean"], out["var"], dmean, dvar
 
     def _predict(self, rng_key, X_new, params, n: int, noiseless: bool = False, **kwargs):
         """gp.py:279-293: (mean [P'], samples [n, P']) with P' = P, or P*T for the Kronecker form"""
@@ -195,8 +216,10 @@ class MultiTaskGP(_LCMModel):
         W_prior_dist, v_prior_dist, output_scale: as in the reference; priors are gpax_b200.priors objects / programs
 
     Limits of the GPU path: T <= 8, L <= 4, input_dim <= 16.  Task labels outside [0, T) raise ValueError (the reference's
-    JAX gather would clamp them silently).  Acquisition functions work through `predict`; `acquisition.optimize_acq`
-    takes finite differences for these models.
+    JAX gather would clamp them silently).  Acquisition functions work through `predict`.  In the multitask form without
+    a mean function, `acquisition.optimize_acq` with EI / UCB / POI / UE takes the posterior's closed-form gradient w.r.t.
+    x (one b2gp_posterior_multitask_grad call per evaluation, 0 on the task column); the Kronecker form and models with a
+    mean function take finite differences.
     """
 
     def __init__(self, input_dim: int, data_kernel: str, num_latents: Optional[int] = None, shared_input_space: bool = False,
@@ -238,7 +261,9 @@ class CoregGP(_LCMModel):
     """
     Coregionalised GP -- gpax/models/corgp.py:38-53: the multitask form with one latent, k_scale fixed at 1, W [T, rank],
     v [T], noise [T]; T is the number of distinct task labels of X_train.  Task labels outside [0, T) raise ValueError.
-    Acquisition functions work through `predict`; `acquisition.optimize_acq` takes finite differences for this model.
+    Acquisition functions work through `predict`.  Without a mean function, `acquisition.optimize_acq` with EI / UCB / POI
+    / UE takes the posterior's closed-form gradient w.r.t. x (one b2gp_posterior_multitask_grad call per evaluation, 0 on
+    the task column); with one it takes finite differences.
     """
 
     def __init__(self, input_dim: int, data_kernel: str, mean_fn: Optional[Callable] = None,

@@ -64,7 +64,7 @@ enum {
     B2GP_OUT_VAR          = 1u << 5, /* ... var[S,P] = diag(cov)     (viGP.predict, vigp.py:184-185)         */
     B2GP_OUT_COV          = 1u << 6, /* ... cov[S,P,P]               (get_mvn_posterior, gp.py:272)          */
     B2GP_OUT_SAMPLE       = 1u << 7, /* ... y_sampled[S,n,P] = mean + chol(cov) eps   (gp.py:292)            */
-    B2GP_OUT_DMEAN        = 1u << 8, /* b2gp_posterior_grad: dmean[S,P,d] = d mean[s,p] / d Xnew[p,:]        */
+    B2GP_OUT_DMEAN        = 1u << 8, /* the *_grad posteriors: dmean[S,P,d] = d mean[s,p] / d Xnew[p,:]      */
     B2GP_OUT_DVAR         = 1u << 9  /* ... dvar[S,P,d] = d var[s,p] / d Xnew[p,:]                            */
 };
 
@@ -234,6 +234,27 @@ int  b2gp_posterior_multitask(b2gp_ctx* ctx, int kind, const double* Xtr, const 
                               int L, int64_t S, const double* theta, const double* B, const double* noise, int noiseless,
                               double jitter, unsigned flags, double* mean, double* var, double* cov, const double* eps,
                               int64_t n_samp, double* y_sampled, int* info, b2gp_timing* timing);
+
+/* The posterior of b2gp_posterior_multitask and its gradient w.r.t. the test inputs -- what jax.grad of the acquisition
+ * w.r.t. x needs in gpax/acquisition/optimize.py:70-88 (optimize_acq) on a MultiTaskGP / CoregGP.  Arguments as
+ * b2gp_posterior_multitask without cov / eps / n_samp / y_sampled; flags: any of B2GP_OUT_MEAN, B2GP_OUT_VAR,
+ * B2GP_OUT_DMEAN, B2GP_OUT_DVAR.  B2GP_FLAG_F32, B2GP_FLAG_DEVICE_PTRS, B2GP_OUT_COV and B2GP_OUT_SAMPLE give
+ * B2GP_ERR_UNSUPPORTED; kinds, limits (T <= 8, L <= 4, d <= 16) and task ids are checked as there, before any launch.
+ *   dmean[S,P,d]  d mean[s,p] / d Xnew[p,k]
+ *   dvar[S,P,d]   d var[s,p]  / d Xnew[p,k]   (the prior diagonal sum_q (k_q(x,x) + jitter) B_q[t,t] + L (noise[t] +
+ *                 jitter) does not depend on x for the three kinds, so the same with and without noiseless)
+ * with P and d counting GP rows and data features: each row is differentiated w.r.t. its own inputs, the Kronecker form's
+ * repeated rows included; the task ids are constants.  The P*d rows sum_q B_q[t_p, t_i] d k_q(Xnew[p], X[i]) / d Xnew[p,k]
+ * are solved with the factor of k_XX like k_pX.  mean and var are those of b2gp_posterior_multitask for the same inputs,
+ * bit for bit under the default "ozaki" = 0.  Under the int8 options (ozaki != 0) the extra rows can move a GEMM of the
+ * factorisation or solve to the other side of a dispatch threshold (trsm_rec's 1024-row panel route, the "oz_min_tiles"
+ * tile count); mean and var then agree within the digit-plane error.  NaN outputs where info[s] != 0; the other draws
+ * are unaffected.  Identical calls give identical bits.  No factor cache, as b2gp_posterior_multitask.                 */
+int  b2gp_posterior_multitask_grad(b2gp_ctx* ctx, int kind, const double* Xtr, const int* task_tr, int64_t N,
+                                   const double* yres, int64_t yres_stride, const double* Xnew, const int* task_new, int64_t P,
+                                   int d, int group, int T, int L, int64_t S, const double* theta, const double* B,
+                                   const double* noise, int noiseless, double jitter, unsigned flags, double* mean, double* var,
+                                   double* dmean, double* dvar, int* info, b2gp_timing* timing);
 
 /* The posterior of b2gp_posterior_batch with the Gram blocks supplied by the caller: the route of a user kernel callable
  * k(X, Z, params, noise, jitter) (gpax/kernels/kernels.py:227-241; gp.py:267-269).  Per draw s:
