@@ -123,6 +123,12 @@ SIGNATURES = {
                                         C.c_uint]),
     "b2gp_sparse_elbo": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp, _vp,
                                    _vp, _ip]),
+    "b2gp_sparse_elbo_ex": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int, _vp, C.c_double, C.c_uint, _dp,
+                                      _vp, _vp, _vp, _ip]),
+    "b2gp_sparse_elbo_gram": (C.c_int, [_vp, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_double, _vp, _vp, _vp, C.c_int64, _vp, _vp,
+                                        C.c_int64, C.c_uint, _dp, _vp, _dp, _vp, _vp, _ip]),
+    "b2gp_sparse_posterior_gram": (C.c_int, [_vp, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_double, _vp, _vp, C.c_int64, C.c_uint, _vp,
+                                             _vp, _vp, _ip, C.POINTER(Timing)]),
     "b2gp_dist_unique_id": (C.c_int, [_vp]),
     "b2gp_dist_init": (C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int]),
     "b2gp_dist_info": (C.c_int, [_vp, _ip, _ip, _ip, _ip]),
@@ -279,7 +285,7 @@ class Context:
     # cumulative counters of b2gp_debug_path_counts, in its order (PathCounter in csrc/common.cuh)
     PATHS = ("gemm_nt", "gemm_tma", "oz_mma", "oz_slice", "trsm_strip", "potrf_diag", "panel_solve", "trsm_tall", "potrf_tall",
              "potrf_tall_fp64", "mll_nngp_grad", "mll_gram_trace", "mll_batch_small", "potrf_tall_batch",
-             "mll_draws_batch")
+             "mll_draws_batch", "sparse_gram_trace")
 
     def path_counts(self):
         """development aid: how often each kernel was launched / each solver route entered on this context so far"""
@@ -849,18 +855,80 @@ class Context:
         a = _f64(a)
         return a, _ptr(a), 0
 
-    def sparse_elbo(self, kind, Xu, X, yres, theta, jitter=1e-6):
-        """VFE bound of the sparse GP, its gradient w.r.t. log(lengthscale[d], k_scale, noise, period) and w.r.t. Xu"""
+    def sparse_elbo(self, kind, Xu, X, yres, theta, jitter=1e-6, want_alpha=False):
+        """VFE bound of the sparse GP, its gradient w.r.t. log(lengthscale[d], k_scale, noise, period) and w.r.t. Xu:
+        (value, grad_theta, grad_Xu, info), with alpha = (W^T W + noise I)^-1 yres = d value / d mean appended when
+        want_alpha (b2gp_sparse_elbo_ex)"""
         Xu, X, yres = _f64(Xu), _f64(X), _f64(yres)
         M, d = Xu.shape
         N = X.shape[0]
         theta = _f64(theta).reshape(d + 3)
         val, info = C.c_double(0.0), C.c_int(0)
         g, gx = np.zeros(d + 3), np.zeros((M, d))
-        self._check(self.lib.b2gp_sparse_elbo(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(Xu), M, _ptr(X), N,
-                                              _ptr(yres), d, _ptr(theta), float(jitter), 0, C.byref(val), _ptr(g), _ptr(gx),
-                                              C.byref(info)))
+        alpha = np.zeros(N) if want_alpha else None
+        self._check(self.lib.b2gp_sparse_elbo_ex(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(Xu), M, _ptr(X), N,
+                                                 _ptr(yres), d, _ptr(theta), float(jitter), 0, C.byref(val), _ptr(g), _ptr(gx),
+                                                 _ptr(alpha), C.byref(info)))
+        if want_alpha:
+            return val.value, g, gx, info.value, alpha
         return val.value, g, gx, info.value
+
+    def sparse_elbo_gram(self, Kuu, Kuf, kff_diag, yres, noise, dirs=(), rdirs=(), want_alpha=False, flags=0):
+        """The VFE bound from caller-supplied blocks (b2gp_sparse_elbo_gram): Kuu [M, M], Kuf [M, N], kff_diag [N], yres [N].
+        `dirs` is a list of (dKuu, dKuf, dkff) triples and `rdirs` of (rKuu, rKuf) pairs; any block may be None.  All
+        arrays are NumPy, or all DeviceArrays (B2GP_FLAG_DEVICE_PTRS); `flags` adds further bits.  Returns a dict: value,
+        grad [len(dirs)],
+        grad_log_noise, grad_rows [len(rdirs), M], alpha [N] or None, info."""
+        dev = isinstance(Kuu, DeviceArray)
+        conv = (lambda a: a) if dev else (lambda a: None if a is None else _f64(a))
+        Kuu, Kuf, kff_diag, yres = conv(Kuu), conv(Kuf), conv(kff_diag), conv(yres)
+        dirs = [tuple(conv(b) for b in t) for t in dirs]
+        rdirs = [tuple(conv(b) for b in t) for t in rdirs]
+        M, N = Kuu.shape[0], Kuf.shape[1]
+        shapes = [((M, M), (M, N), (N,))[t] for t in range(3)]
+        for a, shp in [(Kuu, shapes[0]), (Kuf, shapes[1]), (kff_diag, shapes[2]), (yres, shapes[2])] + \
+                [(b, shapes[t]) for tr in dirs for t, b in enumerate(tr)] + [(b, shapes[t]) for pr in rdirs for t, b in enumerate(pr)]:
+            if a is not None and tuple(a.shape) != shp:
+                raise ValueError(f"block of shape {tuple(a.shape)}: expected {shp}")
+        ptr = (lambda a: None if a is None else a.ptr.value) if dev else (lambda a: None if a is None else a.ctypes.data)
+        p, q = len(dirs), len(rdirs)
+        tables = [(C.c_void_p * max(n, 1))(*[ptr(t[k]) for t in seq])
+                  for seq, n, ks in ((dirs, p, 3), (rdirs, q, 2)) for k in range(ks)]
+        val, gln, info = C.c_double(0.0), C.c_double(0.0), C.c_int(0)
+        grad, rows = np.zeros(p), np.zeros((q, M))
+        alpha = np.zeros(N) if want_alpha else None
+        vp = (lambda a: a.ptr) if dev else _ptr
+        self._check(self.lib.b2gp_sparse_elbo_gram(
+            self.h, vp(Kuu), M, vp(Kuf), N, vp(kff_diag), vp(yres), float(noise), C.cast(tables[0], _vp), C.cast(tables[1], _vp),
+            C.cast(tables[2], _vp), p, C.cast(tables[3], _vp), C.cast(tables[4], _vp), q, (FLAG_DEVICE_PTRS if dev else 0) | flags,
+            C.byref(val), _ptr(grad), C.byref(gln), _ptr(rows), _ptr(alpha), C.byref(info)))
+        return {"value": val.value, "grad": grad, "grad_log_noise": gln.value, "grad_rows": rows, "alpha": alpha,
+                "info": info.value}
+
+    def sparse_posterior_gram(self, Kuu, Kuf, yres, noise, Kus, Kss=None, want=("mean", "cov"), kss_diag=False):
+        """The sparse posterior from caller-supplied blocks (b2gp_sparse_posterior_gram): Kuu [M, M], Kuf [M, N], Kus [M, P]
+        and Kss [P, P] -- or with kss_diag its diagonal [P] (mean / var only) -- host fp64 arrays; outputs as
+        sparse_posterior()."""
+        Kuu, Kuf, Kus, yres = _f64(Kuu), _f64(Kuf), _f64(Kus), _f64(yres)
+        M, N, P = Kuu.shape[0], Kuf.shape[1], Kus.shape[1]
+        Kss = None if Kss is None else _f64(Kss)
+        for a, shp in ((Kuu, (M, M)), (Kuf, (M, N)), (Kus, (M, P)), (yres, (N,)), (Kss, (P,) if kss_diag else (P, P))):
+            if a is not None and a.shape != shp:
+                raise ValueError(f"block of shape {a.shape}: expected {shp}")
+        flags = FLAG_KPP_DIAG if kss_diag else 0
+        out = {"mean": None, "var": None, "cov": None}
+        for name, bit, shape in (("mean", OUT_MEAN, (P,)), ("var", OUT_VAR, (P,)), ("cov", OUT_COV, (P, P))):
+            if name in want:
+                flags |= bit
+                out[name] = np.empty(shape)
+        info = np.zeros(1, dtype=np.int32)
+        t = Timing()
+        self._check(self.lib.b2gp_sparse_posterior_gram(
+            self.h, _ptr(Kuu), M, _ptr(Kuf), N, _ptr(yres), float(noise), _ptr(Kus), _ptr(Kss), P, flags, _ptr(out["mean"]),
+            _ptr(out["var"]), _ptr(out["cov"]), info.ctypes.data_as(_ip), C.byref(t)))
+        out["info"] = int(info[0])
+        out["timing"] = t.as_dict()
+        return out
 
     def sparse_posterior(self, kind, Xu, Xtr, yres, Xnew, theta, noiseless=False, jitter=1e-6, want=("mean", "cov")):
         Xu, Xtr, Xnew = _f64(Xu), _f64(Xtr), _f64(Xnew)

@@ -1253,15 +1253,16 @@ rowdot2_kernel(const double* __restrict__ R, int64_t ld, int64_t len, const doub
     }
 }
 
-// var[p] = kdiag - q[p] + r[p];  NaN when the factorisations failed
+// var[p] = kdiag - q[p] + r[p];  NaN when the factorisations failed.  kss (caller-supplied blocks): kdiag = kss[p * kss_step]
 __global__ void sparse_var_kernel(double* var, double* mean, const double* q, const double* r, int64_t P, int kind, int d,
-                                  const double* theta, double noise_mult, double jitter, const int* info, const int* info2) {
+                                  const double* theta, double noise_mult, double jitter, const int* info, const int* info2,
+                                  const double* kss, int64_t kss_step) {
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P) return;
     const bool bad = (*info != 0) || (*info2 != 0);
     const double nan = __longlong_as_double(0x7ff8000000000000LL);
     if (var) {
-        const double kd = cov_self(kind, theta[d]) + (theta[d + 1] * noise_mult + jitter);
+        const double kd = kss ? kss[p * kss_step] : cov_self(kind, theta[d]) + (theta[d + 1] * noise_mult + jitter);
         var[p] = bad ? nan : (kd - q[p]) + r[p];
     }
     if (mean && bad) mean[p] = nan;
@@ -1272,12 +1273,25 @@ __global__ void scale_by_inv_noise_kernel(double* v, int64_t n, const double* th
     if (i < n) v[i] = v[i] / theta[d + 1];
 }
 
+// The sparse GP's Gram blocks from the caller (b2gp_sparse_elbo_gram, b2gp_sparse_posterior_gram), host arrays or
+// device arrays as `dev`: Kuu [M, M], factored as (Kuu + Kuu^T) / 2 with no jitter added (the caller's Kuu holds it, as
+// the reference's kernel call adds it), Kuf [M, N]; posterior only: Kus [M, P] and Kss [P, P], or its diagonal [P]
+// (kss_diag).  nullptr for the entry points that build the blocks with the fused kernels.
+struct SparseGram {
+    const double* Kuu;
+    const double* Kuf;
+    const double* Kus;
+    const double* Kss;
+    bool kss_diag, dev;
+};
+
 // Partial Nystrom statistics of a shard of the training set (all device pointers):
 //   Luu = chol(Kuu + jitter I), W = Luu^{-1} K(Xu, Xtr_shard),  Kpart = W W^T / noise (lower),  cpart = W y / noise.
-// Summed over shards these are the K (before "+ I") and W D^{-1} y of sparse_gp.py:198-204.
+// Summed over shards these are the K (before "+ I") and W D^{-1} y of sparse_gp.py:198-204.  With `sg` Kuu and Kuf are
+// the caller's (dXu, dXtr, dth, kind and jitter unused); host blocks are staged through ctx->eb[10] and sl.cov.
 static int sparse_partial_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dXu, int64_t M, const double* dXtr, int64_t N,
                               const double* dy, int d, const double* dth, double jitter, double noise_h, double* Luu, int64_t ldM,
-                              double* LinvU, double* Kpart, int64_t ldk, double* cpart, int* dinfo) {
+                              double* LinvU, double* Kpart, int64_t ldk, double* cpart, int* dinfo, const SparseGram* sg = nullptr) {
     cudaStream_t st = sl.stream;
     const int64_t ldN = round_up(N, 8);
     RET_IF(ensure(ctx, sl.Vt, (size_t)N * ldM * 8));
@@ -1285,10 +1299,25 @@ static int sparse_partial_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* d
     double* Wt = (double*)sl.Vt.p;
     double* W = (double*)sl.cov.p;
     // Kuu = kernel(Xu, Xu, params, **kwargs): noise defaults to 0, so the diagonal gets jitter only (sparse_gp.py:193)
-    RET_IF(launch_gram(ctx, st, kind, dXu, M, dXu, M, d, dth, 0.0, jitter, 1, 1, Luu, ldM));
+    if (sg)
+        RET_IF(gram_copyin(ctx, st, ctx->eb[10], sg->Kuu, M, M, sg->dev, Luu, ldM));
+    else
+        RET_IF(launch_gram(ctx, st, kind, dXu, M, dXu, M, d, dth, 0.0, jitter, 1, 1, Luu, ldM));
     RET_IF(potrf_auto(ctx, st, Luu, ldM, M, 0, LinvU, dinfo));                                  // sparse_gp.py:194
     // W^T = K_fu Luu^{-T}  (W = Luu^{-1} Kuf, sparse_gp.py:195-197), one training point per row
-    RET_IF(launch_gram(ctx, st, kind, dXtr, N, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wt, ldM));
+    if (sg) {   // Kuf^T; a host Kuf is staged in W, which is written only after the solve
+        const double* src = sg->Kuf;
+        int64_t lds = N;
+        if (!sg->dev) {
+            CUDA_TRY(ctx, cudaMemcpy2DAsync(W, (size_t)ldN * 8, sg->Kuf, (size_t)N * 8, (size_t)N * 8, (size_t)M, cudaMemcpyHostToDevice, st));
+            src = W;
+            lds = ldN;
+        }
+        RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(N, 32), (unsigned)ceil_div(M, 32)), dim3(32, 8), 0, transpose_kernel, Wt, ldM, src, lds,
+                      M, N));
+    } else {
+        RET_IF(launch_gram(ctx, st, kind, dXtr, N, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wt, ldM));
+    }
     RET_IF(trsm_rec(ctx, st, Wt, ldM, N, Luu, ldM, M, LinvU));   // tall right-hand sides: int8 panel GEMMs (potrf.cuh)
     RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(M, 32), (unsigned)ceil_div(N, 32)), dim3(32, 8), 0, transpose_kernel, W, ldN, Wt, ldM, N, M));
     // W D^{-1} W^T with D = noise * 1  (sparse_gp.py:198-199).  Accumulated onto a zeroed matrix (beta = 1) so that the
@@ -1300,11 +1329,14 @@ static int sparse_partial_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* d
     return launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, dy, 1.0 / noise_h, cpart, nullptr, (int64_t)0);
 }
 
-// Posterior from the summed statistics: K = Ksum + I, L = chol(K), then sparse_gp.py:206-217.
+// Posterior from the summed statistics: K = Ksum + I, L = chol(K), then sparse_gp.py:206-217.  With `sg` Kus and Kss
+// are the caller's (dXu, dXnew, dth, kind, noiseless and jitter unused: noise_p is inside Kss); host blocks are staged
+// through ctx->eb[10] (Kus) and ctx->eb[11] (Kss).
 static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dXu, int64_t M, const double* Luu, int64_t ldM,
                              const double* LinvU, double* Kmat, int64_t ldk, double* LinvK, const double* cvec,
                              const double* dXnew, int64_t P, int d, const double* dth, int noiseless, double jitter,
-                             bool want_var, bool want_cov, double* dmean, double* dvar, double* C, int64_t ldc, int* dinfo) {
+                             bool want_var, bool want_cov, double* dmean, double* dvar, double* C, int64_t ldc, int* dinfo,
+                             const SparseGram* sg = nullptr) {
     cudaStream_t st = sl.stream;
     RET_IF(ensure(ctx, sl.LinvC, (size_t)2 * (P + 1) * ldM * 8));
     RET_IF(ensure(ctx, sl.misc, (size_t)(2 * P + 16) * 8));
@@ -1315,7 +1347,26 @@ static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dX
     RET_IF(launch(ctx, st, grid_for(M), 256, 0, add_diag_kernel, Kmat, ldk, M, 1.0));           // sparse_gp.py:200
     RET_IF(potrf_auto(ctx, st, Kmat, ldk, M, 0, LinvK, dinfo + 1));                             // sparse_gp.py:201
     // Ws^T = K_su Luu^{-T}  (sparse_gp.py:206-207)
-    RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wst, ldM));
+    const double* kss = nullptr;   // caller-supplied Kss on the device
+    if (sg) {
+        const double* kus = sg->Kus;
+        if (!sg->dev) {
+            RET_IF(ensure(ctx, ctx->eb[10], (size_t)M * P * 8));
+            CUDA_TRY(ctx, cudaMemcpyAsync(ctx->eb[10].p, sg->Kus, (size_t)M * P * 8, cudaMemcpyHostToDevice, st));
+            kus = (const double*)ctx->eb[10].p;
+        }
+        RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(P, 32), (unsigned)ceil_div(M, 32)), dim3(32, 8), 0, transpose_kernel, Wst, ldM, kus,
+                      P, M, P));
+        kss = sg->Kss;
+        if (kss && !sg->dev) {
+            const size_t n = sg->kss_diag ? (size_t)P : (size_t)P * P;
+            RET_IF(ensure(ctx, ctx->eb[11], n * 8));
+            CUDA_TRY(ctx, cudaMemcpyAsync(ctx->eb[11].p, sg->Kss, n * 8, cudaMemcpyHostToDevice, st));
+            kss = (const double*)ctx->eb[11].p;
+        }
+    } else {
+        RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXu, M, d, dth, 0.0, 0.0, 0, 0, Wst, ldM));
+    }
     RET_IF(trsm_rec(ctx, st, Wst, ldM, P, Luu, ldM, M, LinvU));
     // pack = [c | Ws]; L^{-1} pack  (sparse_gp.py:208-212)
     RET_IF(launch(ctx, st, grid_for(P * M), 256, 0, copy2d_kernel, R, ldM, Wst, ldM, P, M));
@@ -1325,10 +1376,14 @@ static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dX
     RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, R, ldM, M, R + P * ldM, 1.0, dmean, rv, (int64_t)0));
     RET_IF(launch(ctx, st, (unsigned)P, RD_THREADS, 0, rowdot2_kernel, Wst, ldM, M, nullptr, 1.0, nullptr, qv, (int64_t)0));
     RET_IF(launch(ctx, st, grid_for(P), 256, 0, sparse_var_kernel, want_var ? dvar : nullptr, dmean, qv, rv, P, kind, d, dth,
-                  noiseless ? 0.0 : 1.0, jitter, dinfo, dinfo + 1));
+                  noiseless ? 0.0 : 1.0, jitter, dinfo, dinfo + 1, kss, (sg && !sg->kss_diag) ? P + 1 : (int64_t)1));
     if (want_cov) {
         // cov = Kss - Ws^T Ws + (L^{-1}Ws)^T (L^{-1}Ws)  (sparse_gp.py:215-217)
-        RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXnew, P, d, dth, noiseless ? 0.0 : 1.0, jitter, 1, 1, C, ldc));
+        if (sg)   // the lower triangle of (Kss + Kss^T) / 2
+            RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(P, (int64_t)GCOPY_TILE), (unsigned)ceil_div(P, (int64_t)GCOPY_TILE)),
+                          dim3(GCOPY_TILE, 8), 0, gram_copyin_kernel, kss, P, P, C, ldc));
+        else
+            RET_IF(launch_gram(ctx, st, kind, dXnew, P, dXnew, P, d, dth, noiseless ? 0.0 : 1.0, jitter, 1, 1, C, ldc));
         RET_IF(gemm_nt(ctx, st, P, P, M, -1.0, Wst, ldM, Wst, ldM, 1.0, C, ldc, true));
         RET_IF(gemm_nt(ctx, st, P, P, M, 1.0, R, ldM, R, ldM, 1.0, C, ldc, true));
         RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(P, 32), (unsigned)ceil_div(P, 32)), dim3(32, 32), 0, mirror_lower_kernel, C, ldc, P));
@@ -1337,13 +1392,15 @@ static int sparse_finish_dev(b2gp_ctx* ctx, Slot& sl, int kind, const double* dX
     return B2GP_OK;
 }
 
-extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* Xtr, int64_t N,
-                                     const double* yres, const double* Xnew, int64_t P, int d, const double* theta, int noiseless,
-                                     double jitter, unsigned flags, double* mean, double* var, double* cov, int* info,
-                                     b2gp_timing* timing) {
+// b2gp_sparse_posterior; with `sg` (b2gp_sparse_posterior_gram) the blocks are the caller's and the noise is `noise_g`
+// (Xu, Xtr, Xnew, theta, kind, d, noiseless and jitter unused)
+static int sparse_posterior_impl(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* Xtr, int64_t N,
+                                 const double* yres, const double* Xnew, int64_t P, int d, const double* theta, int noiseless,
+                                 double jitter, unsigned flags, double* mean, double* var, double* cov, int* info,
+                                 b2gp_timing* timing, double noise_g = 0.0, const SparseGram* sg = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
     ARG_CHECK(ctx, kind >= 0 && kind <= 2);
-    ARG_CHECK(ctx, Xu && Xtr && yres && Xnew && theta && info);
+    ARG_CHECK(ctx, (sg || (Xu && Xtr && Xnew && theta)) && yres && info);
     ARG_CHECK(ctx, M >= 1 && N >= 1 && P >= 1 && d >= 1 && d <= GRAM_MAX_D);
     const bool want_mean = flags & B2GP_OUT_MEAN, want_var = flags & B2GP_OUT_VAR, want_cov = flags & B2GP_OUT_COV;
     ARG_CHECK(ctx, !want_mean || mean);
@@ -1357,14 +1414,18 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
     const int nth = d + 3;
-    const double *dXu, *dXtr, *dy, *dXnew, *dth;
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ctx->f32_in[0], Xtr, (size_t)N * d, dev, f32, &dXtr));
+    const double *dXu = nullptr, *dXtr = nullptr, *dy, *dXnew = nullptr, *dth = nullptr;
     RET_IF(stage_in_t(ctx, st, ctx->d_in[1], ctx->f32_in[1], yres, (size_t)N, dev, f32, &dy));
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[2], ctx->f32_in[2], Xnew, (size_t)P * d, dev, f32, &dXnew));
-    RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, dev, &dth));
-    RET_IF(stage_in_t(ctx, st, ctx->d_in[5], ctx->f32_in[5], Xu, (size_t)M * d, dev, f32, &dXu));
+    if (!sg) {
+        RET_IF(stage_in_t(ctx, st, ctx->d_in[0], ctx->f32_in[0], Xtr, (size_t)N * d, dev, f32, &dXtr));
+        RET_IF(stage_in_t(ctx, st, ctx->d_in[2], ctx->f32_in[2], Xnew, (size_t)P * d, dev, f32, &dXnew));
+        RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, dev, &dth));
+        RET_IF(stage_in_t(ctx, st, ctx->d_in[5], ctx->f32_in[5], Xu, (size_t)M * d, dev, f32, &dXu));
+    }
     double noise_h = 0.0;
-    if (dev) {
+    if (sg) {
+        noise_h = noise_g;
+    } else if (dev) {
         CUDA_TRY(ctx, cudaMemcpyAsync(&noise_h, dth + d + 1, 8, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(ctx, cudaStreamSynchronize(st));
     } else {
@@ -1385,14 +1446,14 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
     double* mv = (double*)ctx->d_out[0].p;
     double* vv = mv + P;
     double* cvec = vv + P;
-    RET_IF(sparse_partial_dev(ctx, sl, kind, dXu, M, dXtr, N, dy, d, dth, jitter, noise_h, Luu, ldM, LinvU, Kmat, ldM, cvec, dinfo));
+    RET_IF(sparse_partial_dev(ctx, sl, kind, dXu, M, dXtr, N, dy, d, dth, jitter, noise_h, Luu, ldM, LinvU, Kmat, ldM, cvec, dinfo, sg));
     const bool direct = dev && !f32;     // results written straight into the caller's (device, fp64) arrays
     double* dmean = (want_mean && direct) ? mean : mv;
     double* dvar = (want_var && direct) ? var : vv;
     double* C = direct ? cov : (double*)ctx->d_out[2].p;
     const int64_t ldc = direct ? P : ldC;
     RET_IF(sparse_finish_dev(ctx, sl, kind, dXu, M, Luu, ldM, LinvU, Kmat, ldM, LinvK, cvec, dXnew, P, d, dth, noiseless, jitter,
-                             want_var, want_cov, dmean, dvar, C, ldc, dinfo));
+                             want_var, want_cov, dmean, dvar, C, ldc, dinfo, sg));
     if (want_cov) RET_IF(store_out(ctx, st, ctx->f32_out[2], cov, P, C, ldc, P, P, dev, f32));
     int hinfo[2] = {0, 0};
     CUDA_TRY(ctx, cudaMemcpyAsync(hinfo, dinfo, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1405,6 +1466,27 @@ extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, 
     ctx->last.gram_bytes = 8.0 * (m * n + m * m / 2.0 + m * p);
     if (timing) *timing = ctx->last;
     return B2GP_OK;
+}
+
+extern "C" int b2gp_sparse_posterior(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* Xtr, int64_t N,
+                                     const double* yres, const double* Xnew, int64_t P, int d, const double* theta, int noiseless,
+                                     double jitter, unsigned flags, double* mean, double* var, double* cov, int* info,
+                                     b2gp_timing* timing) {
+    return sparse_posterior_impl(ctx, kind, Xu, M, Xtr, N, yres, Xnew, P, d, theta, noiseless, jitter, flags, mean, var, cov, info, timing);
+}
+
+extern "C" int b2gp_sparse_posterior_gram(b2gp_ctx* ctx, const double* Kuu, int64_t M, const double* Kuf, int64_t N, const double* yres,
+                                          double noise, const double* Kus, const double* Kss, int64_t P, unsigned flags, double* mean,
+                                          double* var, double* cov, int* info, b2gp_timing* timing) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_sparse_posterior_gram", "fp64 arrays only", __FILE__, __LINE__);
+    const bool kss_diag = flags & B2GP_FLAG_KPP_DIAG;
+    ARG_CHECK(ctx, !(kss_diag && (flags & B2GP_OUT_COV)));
+    ARG_CHECK(ctx, Kss || !(flags & (B2GP_OUT_VAR | B2GP_OUT_COV)));
+    ARG_CHECK(ctx, Kuu && Kuf && Kus);
+    const SparseGram sg{Kuu, Kuf, Kus, Kss, kss_diag, dev_ptrs(flags)};
+    return sparse_posterior_impl(ctx, B2GP_KERNEL_RBF, nullptr, M, nullptr, N, yres, nullptr, P, 1, nullptr, 0, 0.0, flags, mean, var, cov,
+                                 info, timing, noise, &sg);
 }
 
 // ---- sharded sparse path (SURVEY.md section 8e, "N-sharded sparse GP"): each rank calls _partial on its shard of
@@ -2641,15 +2723,95 @@ extern "C" int b2gp_bnn_predict_grad(b2gp_ctx* ctx, const double* X, int64_t P, 
     return B2GP_OK;
 }
 
+// b2gp_sparse_elbo_gram: the blocks and the directions to contract the bound's adjoints with come from the caller.
+// blocks.Kuu / Kuf, kff_diag [N] and every direction block follow blocks.dev.  Direction j < p is (dKuu[j] [M, M],
+// dKuf[j] [M, N], dkff[j] [N]); direction p + k, k < q, is (rKuu[k], rKuf[k]) and gives the row sums grad_rows[k, :].
+// Each pointer array may be NULL, and so may each block in it (a zero block).
+struct SparseElboGram {
+    SparseGram blocks;
+    const double* kff_diag;
+    double noise;
+    const double* const* dKuu;
+    const double* const* dKuf;
+    const double* const* dkff;
+    int64_t p;
+    const double* const* rKuu;
+    const double* const* rKuf;
+    int64_t q;
+    double* grad;            // [p]
+    double* grad_log_noise;  // [1]
+    double* grad_rows;       // [q, M]
+};
+
+// The reverse pass of the bound contracted with the caller's directions: one sparse_gram_trace_kernel pass per block over
+// the resident adjoints Gs (M x M, symmetric) and Guf (M x N), then the fixed-order sums of sparse_gram_finish_kernel.
+// Device blocks: one launch over every direction.  Host blocks: streamed through ctx->eb[10] / eb[11] as in
+// mll_gram_trace -- the copy of direction j+1 on a second stream overlaps the reduction of direction j, and the copy into a
+// buffer waits for the reduction that last read it.  `rows` [(p+q), M], `ksum` [p+q], `gdev` [p], `dptrs` [3 (p+q)].
+static int sparse_gram_trace(b2gp_ctx* ctx, cudaStream_t st, const SparseElboGram& g, int64_t M, int64_t N, const double* Gs,
+                             int64_t ldgs, const double* Guf, int64_t ldguf, double gd, double* rows, double* ksum, double* gdev,
+                             const double** dptrs) {
+    const int64_t J = g.p + g.q;
+    count_path(ctx, (int)PATH_SPARSE_GRAM_TRACE);
+    if (J == 0) return B2GP_OK;
+    auto blk = [&](int64_t j, int t) -> const double* {   // direction j's block t (0: Kuu, 1: Kuf, 2: kff) or NULL
+        const double* const* arr = j < g.p ? (t == 0 ? g.dKuu : t == 1 ? g.dKuf : g.dkff) : (t == 0 ? g.rKuu : t == 1 ? g.rKuf : nullptr);
+        return arr ? arr[j < g.p ? j : j - g.p] : nullptr;
+    };
+    const int64_t off[3] = {0, M * M, M * M + M * N}, len[3] = {M * M, M * N, N};
+    std::vector<const double*> table((size_t)3 * J);
+    if (g.blocks.dev) {
+        for (int64_t j = 0; j < J; ++j)
+            for (int t = 0; t < 3; ++t) table[3 * j + t] = blk(j, t);
+        CUDA_TRY(ctx, cudaMemcpyAsync(dptrs, table.data(), table.size() * sizeof(double*), cudaMemcpyHostToDevice, st));
+        RET_IF(launch(ctx, st, dim3((unsigned)(M + 1), (unsigned)J), SGT_THREADS, 0, sparse_gram_trace_kernel, Gs, ldgs, Guf, ldguf, M, N,
+                      (const double* const*)dptrs, M, N, (int64_t)0, rows, ksum));
+    } else {
+        const size_t bytes = (size_t)(M * M + M * N + N) * 8;
+        RET_IF(ensure(ctx, ctx->eb[10], bytes));
+        RET_IF(ensure(ctx, ctx->eb[11], bytes));
+        double* bufs[2] = {(double*)ctx->eb[10].p, (double*)ctx->eb[11].p};
+        for (int64_t j = 0; j < J; ++j)
+            for (int t = 0; t < 3; ++t) table[3 * j + t] = blk(j, t) ? bufs[j & 1] + off[t] : nullptr;
+        CUDA_TRY(ctx, cudaMemcpyAsync(dptrs, table.data(), table.size() * sizeof(double*), cudaMemcpyHostToDevice, st));
+        cudaStream_t cs = ctx->slots[1].stream;
+        cudaEvent_t free_ev = ctx->pool.get(), cp[2] = {ctx->pool.get(), ctx->pool.get()}, red[2] = {ctx->pool.get(), ctx->pool.get()};
+        ARG_CHECK(ctx, free_ev && cp[0] && cp[1] && red[0] && red[1]);
+        CUDA_TRY(ctx, cudaEventRecord(free_ev, st));   // the staging of the caller's Kuu in eb[10] is done with
+        CUDA_TRY(ctx, cudaStreamWaitEvent(cs, free_ev, 0));
+        for (int64_t j = 0; j < J; ++j) {
+            const int b = (int)(j & 1);
+            if (j >= 2) CUDA_TRY(ctx, cudaStreamWaitEvent(cs, red[b], 0));
+            for (int t = 0; t < 3; ++t)
+                if (const double* src = blk(j, t))
+                    CUDA_TRY(ctx, cudaMemcpyAsync(bufs[b] + off[t], src, (size_t)len[t] * 8, cudaMemcpyHostToDevice, cs));
+            CUDA_TRY(ctx, cudaEventRecord(cp[b], cs));
+            CUDA_TRY(ctx, cudaStreamWaitEvent(st, cp[b], 0));
+            RET_IF(launch(ctx, st, dim3((unsigned)(M + 1), 1u), SGT_THREADS, 0, sparse_gram_trace_kernel, Gs, ldgs, Guf, ldguf, M, N,
+                          (const double* const*)(dptrs + 3 * j), M, N, j, rows, ksum));
+            CUDA_TRY(ctx, cudaEventRecord(red[b], st));
+        }
+    }
+    if (g.p == 0) return B2GP_OK;
+    return launch(ctx, st, (unsigned)ceil_div(g.p, (int64_t)128), 128, 0, sparse_gram_finish_kernel, (const double*)rows, M,
+                  (const double*)ksum, gd, g.p, gdev);
+}
+
 // value and gradient of the VFE bound of the sparse GP (see sparse_elbo.cuh): d/dlog(lengthscale[d], k_scale, noise, period)
-// in grad_theta[d+3] and d/dXu in grad_Xu[M,d].  Xu, X, yres follow `flags`; theta is a HOST pointer; outputs are HOST.
-extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N, const double* yres,
-                                int d, const double* theta, double jitter, unsigned flags, double* value, double* grad_theta,
-                                double* grad_Xu, int* info) {
+// in grad_theta[d+3] and d/dXu in grad_Xu[M,d], alpha_out[N] = (W^T W + noise I)^{-1} yres.  Xu, X, yres follow `flags`;
+// theta is a HOST pointer; outputs are HOST.  With `g` the blocks and directions are the caller's (b2gp_sparse_elbo_gram):
+// Xu, X, theta, kind, d and jitter are unused and the gradients go to g's outputs.
+static int sparse_elbo_impl(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N, const double* yres,
+                            int d, const double* theta, double jitter, unsigned flags, double* value, double* grad_theta,
+                            double* grad_Xu, double* alpha_out, int* info, const SparseElboGram* g = nullptr) {
     if (!ctx) return B2GP_ERR_ARG;
-    ARG_CHECK(ctx, kind >= 0 && kind <= 2);
-    ARG_CHECK(ctx, Xu && X && yres && theta && value && grad_theta && grad_Xu && info);
-    ARG_CHECK(ctx, M >= 1 && N >= 1 && d >= 1 && d <= MLL_MAX_D);
+    if (!g) {
+        ARG_CHECK(ctx, kind >= 0 && kind <= 2);
+        ARG_CHECK(ctx, Xu && X && theta && grad_theta && grad_Xu);
+        ARG_CHECK(ctx, d >= 1 && d <= MLL_MAX_D);
+    }
+    ARG_CHECK(ctx, yres && value && info);
+    ARG_CHECK(ctx, M >= 1 && N >= 1);
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     ctx->fcache.valid = false;
     const bool dev = dev_ptrs(flags);
@@ -2658,12 +2820,17 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     CallTimer tm(ctx);
     RET_IF(tm.begin(st));
     const int nth = d + 3;
-    const double noise = theta[d + 1], scale = theta[d];
-    const double *dXu, *dX, *dy, *dth;
-    RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, dev, &dX));
+    const double noise = g ? g->noise : theta[d + 1], scale = g ? 0.0 : theta[d];
+    const int64_t J = g ? g->p + g->q : 0;
+    const double *dXu = nullptr, *dX = nullptr, *dy, *dth = nullptr, *dkff = nullptr;
     RET_IF(stage_in(ctx, st, ctx->d_in[1], yres, (size_t)N * 8, dev, &dy));
-    RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
-    RET_IF(stage_in(ctx, st, ctx->d_in[5], Xu, (size_t)M * d * 8, dev, &dXu));
+    if (g) {
+        RET_IF(stage_in(ctx, st, ctx->d_in[2], g->kff_diag, (size_t)N * 8, dev, &dkff));
+    } else {
+        RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, dev, &dX));
+        RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)nth * 8, false, &dth));
+        RET_IF(stage_in(ctx, st, ctx->d_in[5], Xu, (size_t)M * d * 8, dev, &dXu));
+    }
     const int64_t ldM = round_up(M, 8), ldN = round_up(N, 8);
     double *slA = nullptr, *slLinv = nullptr;   // slot 0's matrix and inverted diagonal blocks
     RET_IF(slot0_buffers(ctx, (size_t)2 * M * ldM * 8, (size_t)2 * linv_bytes(M), &slA, &slLinv));
@@ -2672,7 +2839,10 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(ensure(ctx, ctx->eb[6], (size_t)N * ldM * 8));
     RET_IF(ensure(ctx, ctx->eb[7], (size_t)N * ldM * 8));
     RET_IF(ensure(ctx, ctx->eb[8], (size_t)M * ldN * 8));
-    RET_IF(ensure(ctx, ctx->eb[9], (size_t)(4 * ldM + 3 * ldN + 64 + M * (nth + d)) * 8));
+    // tail after the 64 scalars: fused M x (d+3) partials | M x d grad_Xu;  caller blocks: rows [J, M] | ksum [J] |
+    // grad [p] | the device table of 3 J direction pointers
+    const int64_t tail = g ? J * M + J + g->p + 3 * J + 8 : M * (nth + d);
+    RET_IF(ensure(ctx, ctx->eb[9], (size_t)(4 * ldM + 3 * ldN + 64 + tail) * 8));
     int* dinfo = (int*)ctx->d_info.p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, 16, st));
     double* Luu = slA;
@@ -2685,13 +2855,15 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     double* vec = (double*)ctx->eb[9].p;
     double *bvec = vec, *u = vec + ldM, *beta = vec + 2 * ldM, *tmpM = vec + 3 * ldM;
     double *tmpN = vec + 4 * ldM, *alpha = tmpN + ldN, *tmpN2 = alpha + ldN;
-    double* scal = tmpN2 + ldN;          // [0] sum log LC_ii, [1] u'u, [2] y'y, [3] |W|_F^2, [4] tr(C^-1), [5] alpha'alpha, [8..] chain
+    double* scal = tmpN2 + ldN;          // [0] sum log LC_ii, [1] u'u, [2] y'y, [3] |W|_F^2, [4] tr(C^-1), [5] alpha'alpha,
+                                         // [6] sum kff_diag (caller blocks), [8..] chain
     double* partial = scal + 64;         // M x (d+3)
     double* gXu = partial + M * nth;     // M x d
     dim3 b32(32, 32), gMM((unsigned)ceil_div(M, 32), (unsigned)ceil_div(M, 32));
 
     // forward pieces shared with the posterior: Luu, W (both layouts), W W^T / noise, W y / noise
-    RET_IF(sparse_partial_dev(ctx, sl, kind, dXu, M, dX, N, dy, d, dth, jitter, noise, Luu, ldM, LinvU, Cm, ldM, bvec, dinfo));
+    RET_IF(sparse_partial_dev(ctx, sl, kind, dXu, M, dX, N, dy, d, dth, jitter, noise, Luu, ldM, LinvU, Cm, ldM, bvec, dinfo,
+                              g ? &g->blocks : nullptr));
     double* Wt = (double*)sl.Vt.p;
     double* W = (double*)sl.cov.p;
     RET_IF(launch(ctx, st, grid_for(M), 256, 0, add_diag_kernel, Cm, ldM, M, 1.0));
@@ -2703,6 +2875,7 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(launch(ctx, st, 1, RD_THREADS, 0, rowdot2_kernel, dy, ldN, N, nullptr, 1.0, nullptr, scal + 2, (int64_t)0));
     RET_IF(launch(ctx, st, (unsigned)M, RD_THREADS, 0, rowdot2_kernel, W, ldN, N, nullptr, 1.0, nullptr, tmpM, (int64_t)0));
     RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, tmpM, M, scal + 3));
+    if (g) RET_IF(launch(ctx, st, 1, 256, 0, vecsum_kernel, dkff, N, scal + 6));
     // C^{-1} = BtC BtC^T with BtC = (LC^{-1})^T, beta = C^{-1} b
     RET_IF(launch(ctx, st, grid_for(M * M), 256, 0, set_identity_kernel, BtC, ldM, M, (int64_t)0));
     RET_IF(trsm_rec(ctx, st, BtC, ldM, M, Cm, ldM, M, LinvC));
@@ -2719,11 +2892,12 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     CUDA_TRY(ctx, cudaMemcpyAsync(hs, scal, sizeof hs, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaStreamSynchronize(st));
     double kd = scale;
-    if (kind == B2GP_KERNEL_MATERN52) {
+    if (!g && kind == B2GP_KERNEL_MATERN52) {
         const double r = sqrt(1e-12), s5r = 2.23606797749979 * r;
         kd = scale * (1.0 + s5r) * exp(-s5r);
     }
-    const double T = (double)N * kd - hs[3];
+    // sum_n Kff_nn - |W|_F^2: N k(x, x) for the fused kernels, the caller's diagonal otherwise
+    const double T = (g ? hs[6] : (double)N * kd) - hs[3];
     const double coef = (T > 0.0) ? 1.0 : 0.0;
     // dELBO/dW^T = alpha beta^T + (coef W^T - W^T C^{-1}) / noise
     RET_IF(gemm_nt(ctx, st, N, M, M, 1.0, Wt, ldM, Cinv, ldM, 0.0, E, ldM, false));
@@ -2744,30 +2918,85 @@ extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtU, ldM, T2, ldM, 0.0, T1, ldM, false));  // T1 = BtU P^T
     RET_IF(gemm_nt(ctx, st, M, M, M, 1.0, BtU, ldM, T1, ldM, 0.0, T3, ldM, false));  // T3 = dELBO/dKuu
     RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T2, ldM, T3, ldM, M, 3));                  // T2 = T3 + T3^T
-    // contract with the kernel derivatives
-    RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dX, N, GKuf, ldN, GKuf, ldN, 0, 0, partial, gXu));
-    RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dXu, M, T3, ldM, T2, ldM, 1, 1, partial, gXu));
-    RET_IF(launch(ctx, st, 1, 32, 0, colsum_kernel, partial, M, nth, scal + 8));
+    double* rows = partial;              // caller blocks: [J, M] row sums | ksum [J] | grad [p] | direction table
+    double* ksum = rows + J * M;
+    double* gdev = ksum + J;
+    if (g) {   // Gs = (T3 + T3^T) / 2, the adjoint of the symmetrised Kuu the factorisation reads; Guf = GKuf
+        RET_IF(launch(ctx, st, gMM, b32, 0, tri_kernel, T1, ldM, T3, ldM, M, 4));
+        RET_IF(sparse_gram_trace(ctx, st, *g, M, N, T1, ldM, GKuf, ldN, -coef / (2.0 * noise), rows, ksum, gdev,
+                                 (const double**)(gdev + g->p)));
+    } else {   // contract with the kernel derivatives
+        RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dX, N, GKuf, ldN, GKuf, ldN, 0, 0, partial, gXu));
+        RET_IF(launch(ctx, st, (unsigned)M, 256, 0, elbo_chain_kernel, kind, d, dth, dXu, (int)M, dXu, M, T3, ldM, T2, ldM, 1, 1, partial, gXu));
+        RET_IF(launch(ctx, st, 1, 32, 0, colsum_kernel, partial, M, nth, scal + 8));
+    }
     double hs2[8 + MLL_MAX_D + 3];
     int hinfo[2] = {0, 0};
     CUDA_TRY(ctx, cudaMemcpyAsync(hs2, scal, sizeof hs2, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(ctx, cudaMemcpyAsync(grad_Xu, gXu, (size_t)M * d * 8, cudaMemcpyDeviceToHost, st));
+    if (g) {
+        if (g->p) CUDA_TRY(ctx, cudaMemcpyAsync(g->grad, gdev, (size_t)g->p * 8, cudaMemcpyDeviceToHost, st));
+        if (g->q) CUDA_TRY(ctx, cudaMemcpyAsync(g->grad_rows, rows + g->p * M, (size_t)(g->q * M) * 8, cudaMemcpyDeviceToHost, st));
+    } else {
+        CUDA_TRY(ctx, cudaMemcpyAsync(grad_Xu, gXu, (size_t)M * d * 8, cudaMemcpyDeviceToHost, st));
+    }
+    if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, alpha, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(hinfo, dinfo, sizeof hinfo, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
     *info = hinfo[0] != 0 ? hinfo[0] : -hinfo[1];
     const double n = (double)N, m = (double)M;
     const double loglik = -0.5 * (n * 1.8378770664093453 + n * log(noise) + 2.0 * hs2[0] + hs2[2] / noise - hs2[1]);
     *value = loglik - 0.5 * (T > 0.0 ? T / noise : 0.0);
-    for (int k = 0; k < nth; ++k) grad_theta[k] = hs2[8 + k];
-    grad_theta[d] += (T > 0.0) ? -0.5 * n * kd / noise : 0.0;
     const double trSinv = (n - m + hs2[4]) / noise;
-    grad_theta[d + 1] = noise * (-0.5 * trSinv + 0.5 * hs2[5] + ((T > 0.0) ? 0.5 * T / (noise * noise) : 0.0));
+    const double glog_noise = noise * (-0.5 * trSinv + 0.5 * hs2[5] + ((T > 0.0) ? 0.5 * T / (noise * noise) : 0.0));
+    if (g) {
+        if (g->grad_log_noise) *g->grad_log_noise = glog_noise;
+    } else {
+        for (int k = 0; k < nth; ++k) grad_theta[k] = hs2[8 + k];
+        grad_theta[d] += (T > 0.0) ? -0.5 * n * kd / noise : 0.0;
+        grad_theta[d + 1] = glog_noise;
+    }
     if (*info != 0) {   // grad_Xu too: it was reduced from the failed factor and would otherwise come back finite
         *value = NAN;
-        for (int k = 0; k < nth; ++k) grad_theta[k] = NAN;
-        for (int64_t i = 0; i < M * d; ++i) grad_Xu[i] = NAN;
+        if (g) {
+            for (int64_t k = 0; k < g->p; ++k) g->grad[k] = NAN;
+            for (int64_t k = 0; k < g->q * M; ++k) g->grad_rows[k] = NAN;
+            if (g->grad_log_noise) *g->grad_log_noise = NAN;
+        } else {
+            for (int k = 0; k < nth; ++k) grad_theta[k] = NAN;
+            for (int64_t i = 0; i < M * d; ++i) grad_Xu[i] = NAN;
+        }
+        if (alpha_out)
+            for (int64_t i = 0; i < N; ++i) alpha_out[i] = NAN;
     }
     return B2GP_OK;
+}
+
+extern "C" int b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N, const double* yres,
+                                int d, const double* theta, double jitter, unsigned flags, double* value, double* grad_theta,
+                                double* grad_Xu, int* info) {
+    return b2gp_sparse_elbo_ex(ctx, kind, Xu, M, X, N, yres, d, theta, jitter, flags, value, grad_theta, grad_Xu, nullptr, info);
+}
+
+extern "C" int b2gp_sparse_elbo_ex(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N, const double* yres,
+                                   int d, const double* theta, double jitter, unsigned flags, double* value, double* grad_theta,
+                                   double* grad_Xu, double* alpha_out, int* info) {
+    return sparse_elbo_impl(ctx, kind, Xu, M, X, N, yres, d, theta, jitter, flags, value, grad_theta, grad_Xu, alpha_out, info);
+}
+
+extern "C" int b2gp_sparse_elbo_gram(b2gp_ctx* ctx, const double* Kuu, int64_t M, const double* Kuf, int64_t N, const double* kff_diag,
+                                     const double* yres, double noise, const double* const* dKuu, const double* const* dKuf,
+                                     const double* const* dkff, int64_t p, const double* const* rKuu, const double* const* rKuf,
+                                     int64_t q, unsigned flags, double* value, double* grad, double* grad_log_noise, double* grad_rows,
+                                     double* alpha_out, int* info) {
+    if (!ctx) return B2GP_ERR_ARG;
+    if (f32_io(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_sparse_elbo_gram", "fp64 arrays only", __FILE__, __LINE__);
+    ARG_CHECK(ctx, Kuu && Kuf && kff_diag && p >= 0 && q >= 0);
+    ARG_CHECK(ctx, p == 0 || grad);
+    ARG_CHECK(ctx, q == 0 || grad_rows);
+    const SparseElboGram g{{Kuu, Kuf, nullptr, nullptr, false, dev_ptrs(flags)}, kff_diag, noise, dKuu, dKuf, dkff, p, rKuu, rKuf, q,
+                           grad, grad_log_noise, grad_rows};
+    return sparse_elbo_impl(ctx, B2GP_KERNEL_RBF, nullptr, M, nullptr, N, yres, 1, nullptr, 0.0, flags, value, nullptr, nullptr, alpha_out,
+                            info, &g);
 }
 
 // ------------------------------------------------------------------------------------------ MVN sampling

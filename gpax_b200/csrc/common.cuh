@@ -115,6 +115,7 @@ enum PathCounter {
     PATH_MLL_BATCH_SMALL,  // b2gp_mll_batch calls that took the one-launch small route (mll_batch_small_kernel), one per call
     PATH_POTRF_TALL_BATCH, // lock-step groups of posterior draws factored by one batched potrf_tall (fp64 route), one per group
     PATH_MLL_DRAWS_BATCH,  // groups of likelihood draws b2gp_mll_draws ran in lock-step, one per group
+    PATH_SPARSE_GRAM_TRACE,  // VFE-bound gradients reduced against caller-supplied blocks (sparse_gram_trace_kernel), one per call
     PATH_COUNT
 };
 
@@ -152,7 +153,7 @@ struct b2gp_ctx {
     DevBuf theta1;     // one-draw theta for b2gp_gram
     DevBuf potrf_buf;  // staging for host-pointer b2gp_potrf / trsm / gemm
     DevBuf gemm_buf[3];
-    DevBuf eb[12];     // scratch of b2gp_sparse_elbo
+    DevBuf eb[12];     // scratch of b2gp_sparse_elbo; [10], [11] stage the caller's blocks of the *_gram sparse entry points
     DevBuf f32_in[8];  // fp32 staging of the inputs / outputs of calls made with B2GP_FLAG_F32
     DevBuf f32_out[4];
     DevBuf mlp[4];     // b2gp_mlp_forward / b2gp_dkl_mll: staged X and yres | weights | activations | backward scratch

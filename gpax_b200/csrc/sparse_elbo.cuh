@@ -135,7 +135,8 @@ __global__ void vecsum_kernel(const double* v, int64_t n, double* out) {
 }
 
 // mode 0: dst = tril(src);  1: dst = -triu(src);  2: dst = tril(src) with the diagonal halved (the Phi of the Cholesky
-// backward pass);  3: dst = src + src^T.  Square n x n, separate leading dimensions; dst may not alias src.
+// backward pass);  3: dst = src + src^T;  4: dst = (src + src^T) / 2.  Square n x n, separate leading dimensions; dst may
+// not alias src.
 __global__ void tri_kernel(double* dst, int64_t ldd, const double* src, int64_t lds, int64_t n, int mode) {
     const int64_t i = (int64_t)blockIdx.y * 32 + threadIdx.y, j = (int64_t)blockIdx.x * 32 + threadIdx.x;
     if (i >= n || j >= n) return;
@@ -147,8 +148,10 @@ __global__ void tri_kernel(double* dst, int64_t ldd, const double* src, int64_t 
         o = (j >= i) ? -v : 0.0;
     else if (mode == 2)
         o = (j < i) ? v : (j == i ? 0.5 * v : 0.0);
-    else
+    else if (mode == 3)
         o = v + src[j * lds + i];
+    else
+        o = 0.5 * (v + src[j * lds + i]);
     dst[i * ldd + j] = o;
 }
 
@@ -166,4 +169,54 @@ __global__ void elbo_gw_kernel(double* E, int64_t lde, const double* Wt, int64_t
         const int64_t n = idx / M, m = idx % M;
         E[n * lde + m] = alpha[n] * beta[m] + (coef * Wt[n * ldw + m] - E[n * lde + m]) / noise;
     }
+}
+
+// ---- caller-supplied blocks (b2gp_sparse_elbo_gram: a user kernel callable's fit)
+// One CTA (m, y) per row m of the M x M adjoint Gs and of the M x N adjoint Guf, and direction j = j0 + y:
+//   rows[j * M + m] = sum_i Gs[m, i] dKuu_j[m, i] + sum_n Guf[m, n] dKuf_j[m, n]
+// and CTA (M, y): ksum[j] = sum_n dkff_j[n].  `ptrs` + 3 y holds the direction's (Kuu block [M, ldu], Kuf block [M, ldf],
+// kff vector [N]); a NULL pointer is a zero block.  Every sum runs in a fixed order (strided per thread, then the warp
+// shuffles, then the 8 warps in turn), so identical calls give identical bits.
+constexpr int SGT_THREADS = 256;
+__global__ void __launch_bounds__(SGT_THREADS)
+sparse_gram_trace_kernel(const double* __restrict__ Gs, int64_t ldgs, const double* __restrict__ Guf, int64_t ldguf, int64_t M,
+                         int64_t N, const double* const* __restrict__ ptrs, int64_t ldu, int64_t ldf, int64_t j0,
+                         double* __restrict__ rows, double* __restrict__ ksum) {
+    __shared__ double red[SGT_THREADS / 32];
+    const int64_t m = blockIdx.x, j = j0 + blockIdx.y;
+    const double* const* pj = ptrs + 3 * (int64_t)blockIdx.y;
+    double s = 0.0;
+    if (m < M) {
+        const double* du = pj[0];
+        const double* df = pj[1];
+        if (du)
+            for (int64_t i = threadIdx.x; i < M; i += SGT_THREADS) s = fma(Gs[m * ldgs + i], du[m * ldu + i], s);
+        if (df)
+            for (int64_t n = threadIdx.x; n < N; n += SGT_THREADS) s = fma(Guf[m * ldguf + n], df[m * ldf + n], s);
+    } else if (pj[2]) {
+        const double* dk = pj[2];
+        for (int64_t n = threadIdx.x; n < N; n += SGT_THREADS) s += dk[n];
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < SGT_THREADS / 32; ++w) t += red[w];
+        if (m < M)
+            rows[j * M + m] = t;
+        else
+            ksum[j] = t;
+    }
+}
+
+// grad[j] = sum_m rows[j * M + m] + gd * ksum[j], j < p  (fixed order)
+__global__ void sparse_gram_finish_kernel(const double* __restrict__ rows, int64_t M, const double* __restrict__ ksum, double gd,
+                                          int64_t p, double* __restrict__ grad) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= p) return;
+    double s = 0.0;
+    for (int64_t m = 0; m < M; ++m) s += rows[j * M + m];
+    grad[j] = s + gd * ksum[j];
 }

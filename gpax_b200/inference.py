@@ -628,10 +628,9 @@ class SparseLogJoint(LogJoint):
 
 
 def _sparse_program_log_joint(model, Xu0, jitter):
-    """ProgramLogJoint over the VFE bound; carries `Xu` / `grad_Xu` like SparseLogJoint.  (The bound's derivative w.r.t.
-    the mean vector is not computed on the device, so a probabilistic mean function is refused.)"""
-    if model.mean_fn is not None and model.mean_fn_prior is not None:
-        raise NotImplementedError("viSparseGP.fit with a probabilistic mean function is not implemented")
+    """ProgramLogJoint over the VFE bound; carries `Xu` / `grad_Xu` like SparseLogJoint.  With a probabilistic mean
+    function the device also returns alpha = (W^T W + noise I)^-1 (y - m) = d value / d m (b2gp_sparse_elbo_ex), and
+    ProgramLogJoint adds alpha . dm/du_k."""
     lj = ProgramLogJoint(model, jitter, lik=None)
     lj.Xu = np.array(Xu0, dtype=np.float64, copy=True)
     if lj.Xu.ndim == 1:
@@ -639,17 +638,131 @@ def _sparse_program_log_joint(model, Xu0, jitter):
     lj.grad_Xu = np.zeros_like(lj.Xu)
 
     def lik(th, yres):
-        val, g, gx, info = model.ctx.sparse_elbo(lj.kind, lj.Xu, lj.X, yres, th, lj.jitter)
+        alpha = None
+        if lj.has_mean_params:
+            val, g, gx, info, alpha = model.ctx.sparse_elbo(lj.kind, lj.Xu, lj.X, yres, th, lj.jitter, want_alpha=True)
+        else:
+            val, g, gx, info = model.ctx.sparse_elbo(lj.kind, lj.Xu, lj.X, yres, th, lj.jitter)
         lj.grad_Xu = gx
-        return val, g, None, info
+        return val, g, alpha, info
     lj._lik_fn = lik
     return lj
+
+
+def _same_params(a, b):
+    """two kernel-parameter dicts hold the same values"""
+    return a.keys() == b.keys() and all(
+        (a[k] is None and b[k] is None) or (a[k] is not None and b[k] is not None and np.array_equal(np.asarray(a[k]), np.asarray(b[k])))
+        for k in a)
+
+
+class SparseGramLogJoint(GramLogJoint):
+    """The log joint of viSparseGP.model (sparse_gp.py:62-114) whose kernel is a user callable k(X, Z, params, noise,
+    jitter); carries `Xu` / `grad_Xu` like SparseLogJoint.  Sites are GramLogJoint's.
+
+    One evaluation at u runs the program and makes the model's kernel calls: Kuu = k(Xu, Xu, params, jitter=jitter),
+    Kuf = k(Xu, X, params) with the callable's default jitter (so with M == N its shape rule adds it, as in the
+    reference), and diag(k(X, X, params, jitter=0)) from diagonal blocks of KFF_CHUNK rows (the reference forms all N x N
+    entries; the diagonal is the same for a kernel that evaluates pairs independently; the blocks cost N * KFF_CHUNK
+    entries, so the chunk is small).  One b2gp_sparse_elbo_gram call
+    then returns the bound, its contractions with the directions below, d value / d log noise and alpha = d value / dm.
+
+      kernel coordinates  central differences (FD_STEP) of the three blocks, as GramLogJoint;
+      noise               d noise / du_k by a difference of the program (no kernel call) times the analytic derivative;
+      mean_fn_prior sites alpha . dm/du_k;
+      Xu                  row m of k(Xu + h e_k, Z) depends on inducing point m alone, so two shifted Kuf calls give
+                          d Kuf / d Xu[:, k] for every m at once, and four shifted Kuu calls (first and second argument)
+                          give rKuu_k = D1_k + D2_k^T; the row sums the library returns are grad_Xu[:, k].
+
+    The Xu directions assume that the kernel evaluates pairs independently (k(X, Z)[i, j] depends on X[i] and Z[j]
+    only): every built-in kernel and every set_kernel_fn kernel does.  The input step is XU_STEP * max(1, max |Xu[:, k]|),
+    near the cube root of the fp64 epsilon that balances the O(h^2) truncation of a central difference against its
+    O(eps / h) rounding."""
+
+    KFF_CHUNK = 256
+    XU_STEP = 1e-5
+
+    def __init__(self, model, Xu, jitter=1e-6):
+        super().__init__(model, jitter)
+        self.Xu = np.array(Xu, dtype=np.float64, copy=True)
+        if self.Xu.ndim == 1:
+            self.Xu = self.Xu[:, None]
+        self.grad_Xu = np.zeros_like(self.Xu)
+
+    def _k(self, A, B, kp, **kw):
+        self.kernel_evals += 1
+        return np.asarray(self.m.kernel(A, B, kp, **kw), dtype=np.float64)
+
+    def _blocks(self, kp):
+        """(Kuu, Kuf, kff_diag) at the kernel parameters kp"""
+        X, c = self.X, self.KFF_CHUNK
+        kff = np.concatenate([np.diagonal(self._k(X[a:a + c], X[a:a + c], kp, jitter=0)) for a in range(0, X.shape[0], c)])
+        return self._k(self.Xu, self.Xu, kp, jitter=self.jitter), self._k(self.Xu, X, kp), kff
+
+    def _xu_dirs(self, kp):
+        """[(rKuu_k, rKuf_k)] for every input dimension k"""
+        Xu, out = self.Xu, []
+        for k in range(Xu.shape[1]):
+            h = self.XU_STEP * max(1.0, float(np.abs(Xu[:, k]).max()))
+            e = np.zeros_like(Xu)
+            e[:, k] = h
+            rKuf = (self._k(Xu + e, self.X, kp) - self._k(Xu - e, self.X, kp)) / (2 * h)
+            D1 = (self._k(Xu + e, Xu, kp, jitter=self.jitter) - self._k(Xu - e, Xu, kp, jitter=self.jitter)) / (2 * h)
+            D2 = (self._k(Xu, Xu + e, kp, jitter=self.jitter) - self._k(Xu, Xu - e, kp, jitter=self.jitter)) / (2 * h)
+            out.append((D1 + D2.T, rKuf))
+        return out
+
+    def __call__(self, u, jacobian):
+        u = np.asarray(u, dtype=np.float64)
+        kp, noise, mp, sites = self._program_at(u)
+        self.n_evals += 1
+        self.grad_Xu = np.zeros_like(self.Xu)
+        noise = float(np.asarray(noise).reshape(-1)[0])
+        blocks = self._blocks(kp)
+        if not (noise > 0 and all(np.all(np.isfinite(b)) for b in blocks)):
+            return -np.inf, np.zeros(self.dim)
+        mean = self._mean(mp)
+        yres = self.y0 if mean is None else self.y0 - mean
+        h = self.FD_STEP
+        dirs, kcoords, dnoise, dmean = [], [], np.zeros(self.dim), {}
+        for k in range(self.dim):
+            e = np.zeros(self.dim)
+            e[k] = h
+            kpp, npl, mpp, _ = self._program_at(u + e)
+            kpm, nmi, mpm, _ = self._program_at(u - e)
+            if not (_same_params(kpp, kp) and _same_params(kpm, kp)):
+                bp, bm = self._blocks(kpp), self._blocks(kpm)
+                dirs.append(tuple((p_ - m_) / (2 * h) for p_, m_ in zip(bp, bm)))
+                kcoords.append(k)
+            dnoise[k] = (float(np.asarray(npl).reshape(-1)[0]) - float(np.asarray(nmi).reshape(-1)[0])) / (2 * h)
+            if self.has_mean_params:
+                dmean[k] = (self._mean(mpp) - self._mean(mpm)) / (2 * h)
+        r = self.m.ctx.sparse_elbo_gram(*blocks, yres, noise, dirs, self._xu_dirs(kp), want_alpha=self.has_mean_params)
+        val = r["value"]
+        if r["info"] != 0 or not np.isfinite(val):
+            return -np.inf, np.zeros(self.dim)
+        self.grad_Xu = r["grad_rows"].T.copy()
+        lp, grad = self._log_prior(u, sites, jacobian, want_grad=not self.hierarchical)
+        grad[kcoords] += r["grad"]
+        grad += r["grad_log_noise"] / noise * dnoise
+        for k, dm in dmean.items():
+            grad[k] += float(np.dot(r["alpha"], dm))
+        if self.hierarchical:
+            for k in range(self.dim):
+                e = np.zeros(self.dim)
+                e[k] = h
+                lpp, _ = self._log_prior(u + e, self._program_at(u + e)[3], jacobian, want_grad=False)
+                lpm, _ = self._log_prior(u - e, self._program_at(u - e)[3], jacobian, want_grad=False)
+                grad[k] += (lpp - lpm) / (2 * h)
+        return val + lp, grad
 
 
 def fit_sparse_gp(model, rng_key, Xu0, num_steps, step_size, progress_bar, **kwargs):
     """sparse_gp.py:116-171: SVI with Adam(b1=0.5) over the hyper-parameters (delta or normal guide, as viGP) and over
     the inducing inputs Xu (a plain parameter, no prior).  Returns (state, dict with the guide median and 'Xu')."""
-    if model.kernel_prior is not None or model.noise_prior is not None or \
+    if model._fused is None:
+        lj = SparseGramLogJoint(model, Xu0, kwargs.get("jitter", 1e-6))
+    elif model.kernel_prior is not None or model.noise_prior is not None or \
             (model.mean_fn is not None and model.mean_fn_prior is not None):
         lj = _sparse_program_log_joint(model, Xu0, kwargs.get("jitter", 1e-6))
     else:

@@ -1,6 +1,7 @@
 """
 sparse_gp.py -- `viSparseGP` with the reference's surface (gpax/models/sparse_gp.py:49-60 constructor,
-116-171 fit, 173-223 get_mvn_posterior).  The Nystrom / VFE posterior is one b2gp_sparse_posterior call.
+116-171 fit, 173-223 get_mvn_posterior).  The Nystrom / VFE posterior is one b2gp_sparse_posterior call, or with a user
+kernel callable one b2gp_sparse_posterior_gram call on the blocks the callable returns.
 """
 from typing import Callable, Dict, Optional, Tuple
 
@@ -35,11 +36,42 @@ class viSparseGP(viGP):
         if print_summary:
             self._print_summary()
 
+    KSS_CHUNK = 256      # rows of the diagonal blocks k(X_new[a:b], X_new[a:b]) predict takes diag(Kss) from (P * KSS_CHUNK entries)
+
+    def _posterior_callable_sparse(self, X_new, params, noiseless, want, **kwargs):
+        """User kernel callable: the blocks of sparse_gp.py:193-215 from the reference's own kernel calls, then one
+        b2gp_sparse_posterior_gram call.  Without "cov" only diag(Kss) is needed: it is taken from diagonal blocks
+        k(X_new[a:b], X_new[a:b], ...) of KSS_CHUNK rows, which put noise_p and the jitter on their diagonal by the same
+        shape rule as the full call, so no P x P matrix is formed."""
+        X, y = self._train_arrays()
+        Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
+        Xu = np.asarray(self._set_data(self.Xu), dtype=np.float64)
+        noise = float(np.asarray(params["noise"]).reshape(-1)[0])
+        noise_p = noise * (1 - int(bool(noiseless)))
+        yres = self._residuals(X, y, params, False, 1)
+        k = self.kernel
+        Kuu = np.asarray(k(Xu, Xu, params, **kwargs), dtype=np.float64)
+        Kuf = np.asarray(k(Xu, X, params, jitter=0), dtype=np.float64)
+        Kus = np.asarray(k(Xu, Xn, params, jitter=0), dtype=np.float64)
+        if "cov" in want:
+            Kss = np.asarray(k(Xn, Xn, params, noise_p, **kwargs), dtype=np.float64)
+        else:
+            P, c = Xn.shape[0], self.KSS_CHUNK
+            Kss = np.concatenate([np.diagonal(np.asarray(k(Xn[a:a + c], Xn[a:a + c], params, noise_p, **kwargs), dtype=np.float64))
+                                  for a in range(0, P, c)])
+        out = self.ctx.sparse_posterior_gram(Kuu, Kuf, yres, noise, Kus, Kss, want, kss_diag="cov" not in want)
+        pm = self._prior_mean(Xn, params, False, 1)
+        if pm is not None:
+            out["mean"] = out["mean"] + pm
+        return out
+
     def get_mvn_posterior(self, X_new, params: Dict[str, np.ndarray], noiseless: bool = False,
                           **kwargs: float) -> Tuple[np.ndarray, np.ndarray]:
         """sparse_gp.py:173-223: mean [P] and covariance [P, P] for a single theta."""
         if self._fused is None:
-            raise NotImplementedError("viSparseGP needs 'RBF', 'Matern' or 'Periodic'")
+            out = self._posterior_callable_sparse(X_new, params, noiseless, ("mean", "cov"), **kwargs)
+            dt = self._out_dtype(X_new)
+            return out["mean"].astype(dt, copy=False), out["cov"].astype(dt, copy=False)
         X, y = self._train_arrays()
         Xn = np.asarray(self._set_data(X_new), dtype=np.float64)
         Xu = np.asarray(self._set_data(self.Xu), dtype=np.float64)
@@ -61,6 +93,10 @@ class viSparseGP(viGP):
         X_new = self._set_data(X_new)
         if samples is None:
             samples = self.get_samples()
+        if self._fused is None:
+            out = self._posterior_callable_sparse(X_new, samples, noiseless, ("mean", "var"), **kwargs)
+            dt = self._out_dtype(X_new)
+            return out["mean"].astype(dt, copy=False), out["var"].astype(dt, copy=False)
         X, y = self._train_arrays()
         Xn = np.asarray(X_new, dtype=np.float64)
         Xu = np.asarray(self._set_data(self.Xu), dtype=np.float64)

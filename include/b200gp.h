@@ -283,6 +283,20 @@ int  b2gp_sparse_posterior(b2gp_ctx* ctx, int kind,
                            double* mean, double* var, double* cov,
                            int* info, b2gp_timing* timing);
 
+/* The posterior of b2gp_sparse_posterior with the Gram blocks supplied by the caller: the route of a user kernel callable
+ * k(X, Z, params, noise, jitter) in viSparseGP.get_mvn_posterior (gpax/models/sparse_gp.py:173-223):
+ *   Kuu [M, M]  kernel(Xu, Xu, params, **kwargs); the library factors (Kuu + Kuu^T) / 2 and adds no jitter (it is in Kuu)
+ *   Kuf [M, N]  kernel(Xu, X_train, params, jitter=0)
+ *   Kus [M, P]  kernel(Xu, X_new, params, jitter=0)
+ *   Kss [P, P]  kernel(X_new, X_new, params, noise_p, **kwargs) (noise_p already inside); its lower triangle is read.
+ *               With B2GP_FLAG_KPP_DIAG only its diagonal [P], and the outputs are limited to mean / var.  May be NULL for
+ *               mean-only calls.
+ * yres [N] and `noise` (the D = noise 1 of sparse_gp.py:191-192) as b2gp_sparse_posterior; every block follows `flags`
+ * (B2GP_FLAG_DEVICE_PTRS; B2GP_FLAG_F32 gives B2GP_ERR_UNSUPPORTED).  Outputs, info and timing as b2gp_sparse_posterior. */
+int  b2gp_sparse_posterior_gram(b2gp_ctx* ctx, const double* Kuu, int64_t M, const double* Kuf, int64_t N, const double* yres,
+                                double noise, const double* Kus, const double* Kss, int64_t P, unsigned flags,
+                                double* mean, double* var, double* cov, int* info, b2gp_timing* timing);
+
 /* Fit side (SURVEY.md section 8f-1): value and gradient of the exact-GP log marginal likelihood
  *   log N(yres; 0, K_theta),  K_theta = kernel(X, X, theta, noise, jitter)
  * i.e. the numpyro.sample("y", MultivariateNormal(f_loc, covariance_matrix=k), obs=y) term of
@@ -337,6 +351,37 @@ int  b2gp_mll_multitask(b2gp_ctx* ctx, int kind, const double* X, const int* tas
 int  b2gp_sparse_elbo(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N,
                       const double* yres, int d, const double* theta, double jitter, unsigned flags,
                       double* value, double* grad_theta, double* grad_Xu, int* info);
+
+/* b2gp_sparse_elbo plus alpha_out[N] (HOST, optional) = (W^T W + noise I)^{-1} yres, the derivative of the bound w.r.t.
+ * the mean vector subtracted from y (sparse_gp.py:71-88's f_loc).  b2gp_sparse_elbo is this call with alpha_out = NULL;
+ * the other outputs are the same bits either way.  NaN alpha_out where info != 0.                                    */
+int  b2gp_sparse_elbo_ex(b2gp_ctx* ctx, int kind, const double* Xu, int64_t M, const double* X, int64_t N,
+                         const double* yres, int d, const double* theta, double jitter, unsigned flags,
+                         double* value, double* grad_theta, double* grad_Xu, double* alpha_out, int* info);
+
+/* The bound of b2gp_sparse_elbo from caller-supplied blocks (a user kernel callable's fit, sparse_gp.py:88-103):
+ *   Kuu [M, M]     kernel(Xu, Xu, params, jitter=jitter), factored as (Kuu + Kuu^T) / 2; the library adds no jitter
+ *   Kuf [M, N]     kernel(Xu, X, params)
+ *   kff_diag [N]   diag(kernel(X, X, params, jitter=0)); the trace term is sum kff_diag - |W|_F^2, clipped at 0
+ * and yres [N], noise.  Outputs (HOST):
+ *   value            the bound
+ *   grad[j]          sum Gs * dKuu[j] + sum Guf * dKuf[j] + g_d sum dkff[j],  j < p, where Gs (M x M, symmetric) and
+ *                    Guf (M x N) are the adjoints of the bound w.r.t. the symmetrised Kuu and Kuf, g_d = -coef / (2 noise)
+ *                    and coef = 1 when the trace term is positive, else 0
+ *   grad_log_noise   d value / d log noise (optional)
+ *   grad_rows[k, m]  sum_i Gs[m, i] rKuu[k][m, i] + sum_n Guf[m, n] rKuf[k][m, n],  k < q: with rKuu_k, rKuf_k the
+ *                    derivatives of Kuu and Kuf w.r.t. Xu[:, k] (row m moving with Xu[m, k]), d value / d Xu[m, k]
+ *   alpha_out[N]     (W^T W + noise I)^{-1} yres (optional)
+ * dKuu, dKuf, dkff (p each), rKuu, rKuf (q each) are HOST arrays of pointers; any of them, and any entry, may be NULL (a
+ * zero block).  No symmetry is assumed of the direction blocks.  Every block is a host array, or a device array under
+ * B2GP_FLAG_DEVICE_PTRS; host direction blocks are streamed through two device buffers.  The contraction runs in a fixed
+ * order, so identical calls give identical bits.  info as b2gp_sparse_elbo; NaN outputs where info != 0.  B2GP_FLAG_F32
+ * gives B2GP_ERR_UNSUPPORTED.                                                                                          */
+int  b2gp_sparse_elbo_gram(b2gp_ctx* ctx, const double* Kuu, int64_t M, const double* Kuf, int64_t N, const double* kff_diag,
+                           const double* yres, double noise, const double* const* dKuu, const double* const* dKuf,
+                           const double* const* dkff, int64_t p, const double* const* rKuu, const double* const* rKuf,
+                           int64_t q, unsigned flags, double* value, double* grad, double* grad_log_noise, double* grad_rows,
+                           double* alpha_out, int* info);
 
 /* ---- deep kernel learning (gpax/models/vidkl.py, gpax/models/dkl.py) ---------------------------------------------
  * The feature extractor is a dense MLP, H_{l+1} = act(H_l W_l + b_l) with no activation after the last layer.
