@@ -104,6 +104,8 @@ SIGNATURES = {
                                  _vp, _vp]),
     "b2gp_mll_draws": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_int, C.c_int64, _vp, C.c_double, C.c_uint, _vp,
                                  _vp, _vp, _vp]),
+    "b2gp_mll_draws_v": (C.c_int, [_vp, C.c_int, _vp, C.c_int64, _vp, C.c_int64, C.c_int, C.c_int64, _vp, _vp, C.c_int64, C.c_double,
+                                   C.c_uint, _vp, _vp, _vp, _vp, _vp]),
     "b2gp_mll_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int64, C.c_uint, _dp, _vp, _vp, _ip]),
     "b2gp_posterior_gram": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
                                       C.c_int64, C.c_uint, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.POINTER(Timing)]),
@@ -529,6 +531,26 @@ class Context:
                                             0 if yres.ndim == 1 else N, d, S, _ptr(theta), float(jitter), 0, _ptr(val),
                                             _ptr(grad), _ptr(alpha), _ptr(info)))
         return val, grad, alpha, info
+
+    def mll_draws_v(self, kind, X, yres, theta, noise_vec, jitter=1e-6, want_grad=True, want_alpha=False):
+        """mll_draws with per-point noise variances (b2gp_mll_draws_v): draw s is ctx.mll(kind, X, yres[s], theta[s],
+        noise_vec=noise_vec[s]) bit for bit.  noise_vec [N] (shared) or [S, N]; the rest as mll_draws.
+        Returns (value [S], grad [S, d+3] or None, alpha [S, N] or None, grad_noise_vec [S, N] or None, info [S])."""
+        X, yres, nv = _f64(X), _f64(yres), _f64(noise_vec)
+        N, d = X.shape
+        theta = _f64(theta).reshape(-1, d + 3)
+        S = theta.shape[0]
+        if yres.shape not in ((N,), (S, N)) or nv.shape not in ((N,), (S, N)):
+            raise ValueError(f"yres and noise_vec must be [{N}] or [{S}, {N}], got shapes {yres.shape} and {nv.shape}")
+        val = np.zeros(S)
+        grad = np.zeros((S, d + 3)) if want_grad else None
+        alpha = np.zeros((S, N)) if want_alpha else None
+        gnv = np.zeros((S, N)) if want_grad else None
+        info = np.zeros(S, dtype=np.int32)
+        self._check(self.lib.b2gp_mll_draws_v(self.h, KIND[kind] if isinstance(kind, str) else kind, _ptr(X), N, _ptr(yres),
+                                              0 if yres.ndim == 1 else N, d, S, _ptr(theta), _ptr(nv), 0 if nv.ndim == 1 else N,
+                                              float(jitter), 0, _ptr(val), _ptr(grad), _ptr(alpha), _ptr(gnv), _ptr(info)))
+        return val, grad, alpha, gnv, info
 
     def mll_gram(self, K, yres, dKs=(), want_grad=True, want_alpha=False):
         """log N(yres; 0, K) from a caller-supplied K [N, N] (factored as (K + K^T) / 2), the traces

@@ -592,8 +592,11 @@ struct StageEvents {
 };
 }
 
-// diag(A) += v   (per-point noise variances: mngp.py:96, hskgp.py:147)
-__global__ void add_diag_vec_kernel(double* A, int64_t ld, int64_t n, const double* __restrict__ v) {
+// diag(A) += v   (per-point noise variances: mngp.py:96, hskgp.py:147); the draw of a batch is blockIdx.z (A `bstride`
+// doubles apart, v `vstride` apart)
+__global__ void add_diag_vec_kernel(double* A, int64_t ld, int64_t n, const double* __restrict__ v, int64_t bstride, int64_t vstride) {
+    A += (int64_t)blockIdx.z * bstride;
+    v += (int64_t)blockIdx.z * vstride;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) A[i * ld + i] += v[i];
 }
@@ -897,7 +900,7 @@ static int posterior_impl(b2gp_ctx* ctx, int kind, const double* Xtr, int64_t xt
                 RET_IF(launch_gram_lcm(ctx, st, LCM_LOWER, kind, dXtr_s, dtr, N, dXtr_s, dtr, N, d, T, L, grp, th, Bs, ns, 1.0, jitter, A, ldA));
             else
                 RET_IF(launch_gram(ctx, st, kind, dXtr_s, N, dXtr_s, N, d, th, 1.0, jitter, 1, 1, A, ldA));
-            if (dnv) RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ldA, N, dnv + s * nv_stride));
+            if (dnv) RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ldA, N, dnv + s * nv_stride, (int64_t)0, (int64_t)0));
             if (fused_solve) RET_IF(rhs_rows());
             if (timing) CUDA_TRY(ctx, cudaEventRecord(sev[s].e[1], st));
             return B2GP_OK;
@@ -1627,9 +1630,13 @@ extern "C" int b2gp_copy2d(b2gp_ctx* ctx, double* dst, int64_t ldd, const double
 // value and gradient (w.r.t. log lengthscale[d], log k_scale, log noise, log period) of the exact-GP log marginal
 // likelihood -- see mll.cuh.  X[N,d], yres[N] host or device pointers (flags); theta is a HOST pointer (d+3);
 // value, grad[d+3] and the optional alpha[N] = K^{-1} yres are HOST outputs.
-// g[i] = 1/2 (alpha_i^2 - Kinv_ii): d log N(y; 0, K) / d K_ii, the gradient w.r.t. a per-point noise variance
+// g[i] = 1/2 (alpha_i^2 - Kinv_ii): d log N(y; 0, K) / d K_ii, the gradient w.r.t. a per-point noise variance; the draw
+// of a batch is blockIdx.z (every operand `bstride` doubles apart)
 __global__ void mll_diag_grad_kernel(const double* __restrict__ alpha, const double* __restrict__ Kinv, int64_t ldk, int64_t n,
-                                     double* __restrict__ g) {
+                                     double* __restrict__ g, int64_t bstride) {
+    alpha += (int64_t)blockIdx.z * bstride;
+    Kinv += (int64_t)blockIdx.z * bstride;
+    g += (int64_t)blockIdx.z * bstride;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) g[i] = 0.5 * (alpha[i] * alpha[i] - Kinv[i * ldk + i]);
 }
@@ -1755,7 +1762,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
     else
         RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, dth, 1.0, jitter, 1, 1, A, ld));
     if (dnv)   // k + diag(measured_noise) / k + diag(exp(log_var)): mngp.py:96, hskgp.py:147
-        RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ld, N, dnv));
+        RET_IF(launch(ctx, st, grid_for(N), 256, 0, add_diag_vec_kernel, A, ld, N, dnv, (int64_t)0, (int64_t)0));
     CUDA_TRY(ctx, cudaMemcpyAsync(w, dy, (size_t)N * 8, cudaMemcpyDeviceToDevice, st));
     // the scheme of the posterior (tall-panel int8 at N >= 2048); w = L^{-1} y falls out of the panel solves instead of
     // a separate chain of 2 N / 128 strip launches for one row
@@ -1811,7 +1818,7 @@ static int mll_impl(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
                                   (const double*)alpha, (const double*)Kinv, ld, grad_x_dev));
             }
             if (grad_noise_vec) {
-                RET_IF(launch(ctx, st, grid_for(N), 256, 0, mll_diag_grad_kernel, alpha, Kinv, ld, N, w));   // w is free again
+                RET_IF(launch(ctx, st, grid_for(N), 256, 0, mll_diag_grad_kernel, alpha, Kinv, ld, N, w, (int64_t)0));   // w is free again
                 CUDA_TRY(ctx, cudaMemcpyAsync(grad_noise_vec, w, (size_t)N * 8, cudaMemcpyDeviceToHost, st));
             }
         }
@@ -1919,22 +1926,37 @@ __global__ void zero_batch_kernel(double* p, int64_t n, int64_t bstride) {
 
 constexpr int MLLD_HS = 8 + MLL_MAX_D + 3;   // the scalars of sc read back per draw (mll_impl's hsc)
 
-extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
-                              int64_t S, const double* theta, double jitter, unsigned flags, double* value, double* grad,
-                              double* alpha_out, int* info) {
+// Stage S vectors of N doubles, `stride` apart (0: one vector for every draw), as [S, N] in `buf`; `rows` holds the
+// repeated host copy until the call's end
+static int stage_rows(b2gp_ctx* ctx, cudaStream_t st, DevBuf& buf, std::vector<double>& rows, const double* src, int64_t stride,
+                      int64_t S, int64_t N, const double** out) {
+    if (stride != N) {
+        rows.resize((size_t)S * N);
+        for (int64_t s = 0; s < S; ++s) memcpy(rows.data() + s * N, src + s * stride, (size_t)N * 8);
+        src = rows.data();
+    }
+    return stage_in(ctx, st, buf, src, (size_t)S * N * 8, false, out);
+}
+
+// b2gp_mll_draws and b2gp_mll_draws_v: noise_vec == nullptr is the plain likelihood, with no launch of the noise-vector form
+static int mll_draws_impl(b2gp_ctx* ctx, const char* who, int kind, const double* X, int64_t N, const double* yres,
+                          int64_t yres_stride, int d, int64_t S, const double* theta, const double* noise_vec, int64_t nv_stride,
+                          double jitter, unsigned flags, double* value, double* grad, double* alpha_out, double* grad_noise_vec,
+                          int* info) {
     if (!ctx) return B2GP_ERR_ARG;
-    if (f32_io(flags) || dev_ptrs(flags))
-        return set_err(ctx, B2GP_ERR_UNSUPPORTED, "b2gp_mll_draws", "host fp64 arrays only", __FILE__, __LINE__);
+    if (f32_io(flags) || dev_ptrs(flags)) return set_err(ctx, B2GP_ERR_UNSUPPORTED, who, "host fp64 arrays only", __FILE__, __LINE__);
     ARG_CHECK(ctx, kind >= 0 && kind <= B2GP_KERNEL_NNGP_RELU);
     const bool nngp = is_nngp(kind);
     ARG_CHECK(ctx, X && yres && theta && value && info);
     ARG_CHECK(ctx, N >= 1 && S >= 1 && d >= 1 && d <= (nngp ? GRAM_MAX_D : MLL_MAX_D));
     ARG_CHECK(ctx, yres_stride == 0 || yres_stride >= N);
+    ARG_CHECK(ctx, !noise_vec || nv_stride == 0 || nv_stride >= N);
+    ARG_CHECK(ctx, !grad_noise_vec || (noise_vec && grad));
     const int nth = d + 3;
     int depth = 0;   // NNGP: the deepest draw sizes the self-chains and the gradient kernel's shared memory
     if (nngp)
         for (int64_t s = 0; s < S; ++s) {
-            RET_IF(nngp_check_depth(ctx, "b2gp_mll_draws", theta[s * nth]));
+            RET_IF(nngp_check_depth(ctx, who, theta[s * nth]));
             depth = std::max(depth, (int)theta[s * nth]);
         }
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
@@ -1961,25 +1983,22 @@ extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t 
             B = ctx->draw_batch;
         B = std::min<int64_t>(std::min<int64_t>(B, S), 65535);
     }
-    // inputs: X, theta [S, nth] and yres as [S, N] (a shared yres repeated), staged once
-    std::vector<double> yrows;
-    const double* ysrc = yres;
-    if (yres_stride != N) {
-        yrows.resize((size_t)S * N);
-        for (int64_t s = 0; s < S; ++s) memcpy(yrows.data() + s * N, yres + s * yres_stride, (size_t)N * 8);
-        ysrc = yrows.data();
-    }
-    const double *dX, *dy, *dth;
+    // inputs: X, theta [S, nth], yres and the noise vectors as [S, N] (a shared vector repeated), staged once
+    std::vector<double> yrows, nvrows;
+    const double *dX, *dy, *dth, *dnv = nullptr;
     RET_IF(stage_in(ctx, st, ctx->d_in[0], X, (size_t)N * d * 8, false, &dX));
-    RET_IF(stage_in(ctx, st, ctx->d_in[1], ysrc, (size_t)S * N * 8, false, &dy));
+    RET_IF(stage_rows(ctx, st, ctx->d_in[1], yrows, yres, yres_stride, S, N, &dy));
     RET_IF(stage_in(ctx, st, ctx->d_in[3], theta, (size_t)S * nth * 8, false, &dth));
+    if (noise_vec) RET_IF(stage_rows(ctx, st, ctx->d_in[6], nvrows, noise_vec, nv_stride, S, N, &dnv));
     RET_IF(ensure(ctx, ctx->d_info, (size_t)S * sizeof(int)));
     RET_IF(ensure(ctx, ctx->d_out[0], (size_t)S * MLLD_HS * 8));
     if (alpha_out) RET_IF(ensure(ctx, ctx->d_out[1], (size_t)S * N * 8));
+    if (grad_noise_vec) RET_IF(ensure(ctx, ctx->d_out[2], (size_t)S * N * 8));
     RET_IF(ensure(ctx, ctx->post, (size_t)B * stride * 8));
     int* dinfo = (int*)ctx->d_info.p;
     double* dsc = (double*)ctx->d_out[0].p;
     double* dal = (double*)ctx->d_out[1].p;
+    double* dgnv = (double*)ctx->d_out[2].p;
     CUDA_TRY(ctx, cudaMemsetAsync(dinfo, 0, (size_t)S * sizeof(int), st));
     double* R = (double*)ctx->post.p;
     double *Linv = R, *A = R + oA, *w = A + N * ld, *Bt = R + oBt, *Kinv = R + oKi, *scr = R + oScr, *alpha = R + oAl, *sc = R + oSc,
@@ -2001,6 +2020,8 @@ extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t 
                       (int64_t)nth));
         RET_IF(launch(ctx, st, grid_for((int64_t)nb * N), 256, 0, copy2d_kernel, w, stride, dy + g0 * N, N, (int64_t)nb, N));
         RET_IF(launch_gram(ctx, st, kind, dX, N, dX, N, d, th, 1.0, jitter, 1, 1, A, ld, bt));
+        if (dnv)
+            RET_IF(launch(ctx, st, dim3(grid_for(N), 1, z), 256, 0, add_diag_vec_kernel, A, ld, N, dnv + g0 * N, stride, N));
         if (nb == 1) {   // mll_impl's factorisation on every route
             RET_IF(potrf_auto(ctx, st, A, ld, N, 1, Linv, dinfo + g0));
         } else if (tall64) {   // fp64 tall-panel route, y riding below K
@@ -2037,6 +2058,9 @@ extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t 
                               (const double*)th, (const double*)alpha, (const double*)Kinv, ld, partial, stride));
                 RET_IF(launch(ctx, st, dim3(1, 1, z), 32, 0, mll_finish_kernel, (const double*)partial, tiles * tiles, nth, sc + 8, stride));
             }
+            if (grad_noise_vec)   // the draw's w row is free once alpha is formed
+                RET_IF(launch(ctx, st, dim3(grid_for(N), 1, z), 256, 0, mll_diag_grad_kernel, (const double*)alpha, (const double*)Kinv, ld, N,
+                              w, stride));
         }
         // the group's results leave the regions before the next group reuses them
         RET_IF(launch(ctx, st, grid_for((int64_t)nb * MLLD_HS), 256, 0, copy2d_kernel, dsc + g0 * MLLD_HS, (int64_t)MLLD_HS,
@@ -2044,11 +2068,15 @@ extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t 
         if (alpha_out)
             RET_IF(launch(ctx, st, grid_for((int64_t)nb * N), 256, 0, copy2d_kernel, dal + g0 * N, N, (const double*)alpha, stride,
                           (int64_t)nb, N));
+        if (grad_noise_vec)
+            RET_IF(launch(ctx, st, grid_for((int64_t)nb * N), 256, 0, copy2d_kernel, dgnv + g0 * N, N, (const double*)w, stride,
+                          (int64_t)nb, N));
     }
     std::vector<double> hsc((size_t)S * MLLD_HS);
     CUDA_TRY(ctx, cudaMemcpyAsync(hsc.data(), dsc, hsc.size() * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(ctx, cudaMemcpyAsync(info, dinfo, (size_t)S * sizeof(int), cudaMemcpyDeviceToHost, st));
     if (alpha_out) CUDA_TRY(ctx, cudaMemcpyAsync(alpha_out, dal, (size_t)S * N * 8, cudaMemcpyDeviceToHost, st));
+    if (grad_noise_vec) CUDA_TRY(ctx, cudaMemcpyAsync(grad_noise_vec, dgnv, (size_t)S * N * 8, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
     for (int64_t s = 0; s < S; ++s) {   // mll_impl's host epilogue, per draw
         const double* h = hsc.data() + s * MLLD_HS;
@@ -2066,10 +2094,27 @@ extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t 
                 for (int k = 0; k < nth; ++k) g[k] = NAN;
             if (alpha_out)
                 for (int64_t i = 0; i < N; ++i) alpha_out[s * N + i] = NAN;
+            if (grad_noise_vec)
+                for (int64_t i = 0; i < N; ++i) grad_noise_vec[s * N + i] = NAN;
         }
     }
     ctx->last.flops = (double)S * N * N * N * (grad ? 1.0 / 3 + 1.0 + 1.0 : 1.0 / 3);
     return B2GP_OK;
+}
+
+extern "C" int b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
+                              int64_t S, const double* theta, double jitter, unsigned flags, double* value, double* grad,
+                              double* alpha_out, int* info) {
+    return mll_draws_impl(ctx, "b2gp_mll_draws", kind, X, N, yres, yres_stride, d, S, theta, nullptr, 0, jitter, flags, value, grad,
+                          alpha_out, nullptr, info);
+}
+
+extern "C" int b2gp_mll_draws_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
+                                int64_t S, const double* theta, const double* noise_vec, int64_t nv_stride, double jitter,
+                                unsigned flags, double* value, double* grad, double* alpha_out, double* grad_noise_vec, int* info) {
+    if (ctx && !noise_vec) return set_err(ctx, B2GP_ERR_ARG, "b2gp_mll_draws_v", "noise_vec is required", __FILE__, __LINE__);
+    return mll_draws_impl(ctx, "b2gp_mll_draws_v", kind, X, N, yres, yres_stride, d, S, theta, noise_vec, nv_stride, jitter, flags, value,
+                          grad, alpha_out, grad_noise_vec, info);
 }
 
 // ------------------------------------------------------------------------------------------ deep kernel learning (dkl.cuh)

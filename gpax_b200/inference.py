@@ -149,9 +149,23 @@ class NNGPLogJoint(LogJoint):
         return {"var_b": th[:, self.d + 2], "var_w": th[:, self.d], "noise": th[:, self.d + 1]}
 
 
-def gp_model_program(m, d, kind):
+def gp_model_program(m, d, kind, noise_site=True):
     """the host side of ExactGP.model (gp.py:137-154): every statement except the likelihood.  Runs under
-    priors.run_program; returns (kernel-parameter dict, noise, mean-function parameter dict or None)."""
+    priors.run_program; returns (kernel-parameter dict, noise, mean-function parameter dict or None).  noise_site=False
+    is MeasuredNoiseGP.model (mngp.py:75-97): no noise site, noise 0."""
+    kp = kernel_program(m, d, kind)
+    if not noise_site:
+        noise = 0.0
+    elif m.noise_prior is not None:
+        noise = m.noise_prior()
+    else:                                                              # gp.py:222-227
+        noise = P.sample("noise", m.noise_prior_dist or P.LogNormal(0.0, 1.0))
+    mp = m.mean_fn_prior() if (m.mean_fn is not None and m.mean_fn_prior is not None) else None
+    return kp, noise, mp
+
+
+def kernel_program(m, d, kind):
+    """the kernel-parameter statements of gp.py:141-144: kernel_prior() or the default sites of gp.py:229-247"""
     if m.kernel_prior is not None:
         kp = m.kernel_prior()
     elif _is_nngp(getattr(m, "_fused", None)):                         # ibnn.py:54-61, vi_ibnn.py:53-60
@@ -162,12 +176,7 @@ def gp_model_program(m, d, kind):
             length = P.sample("k_length", lp)
         kp = {"k_length": length, "k_scale": P.sample("k_scale", P.LogNormal(0.0, 1.0))}
         kp["period"] = P.sample("period", P.LogNormal(0.0, 1.0)) if kind == "Periodic" else None
-    if m.noise_prior is not None:
-        noise = m.noise_prior()
-    else:                                                              # gp.py:222-227
-        noise = P.sample("noise", m.noise_prior_dist or P.LogNormal(0.0, 1.0))
-    mp = m.mean_fn_prior() if (m.mean_fn is not None and m.mean_fn_prior is not None) else None
-    return kp, noise, mp
+    return kp
 
 
 def prior_draws(model, rng, num_samples, d):
@@ -195,11 +204,16 @@ class ProgramLogJoint:
 
     FD_STEP = 1e-5
     CALLABLE_KERNEL = False      # GramLogJoint: the kernel is the model's callable, not a fused GPU kernel
+    noise_vec = None
 
-    def __init__(self, model, jitter=1e-6, lik=None):
+    def __init__(self, model, jitter=1e-6, lik=None, noise_vec=None):
+        """noise_vec [N]: fixed per-point noise variances on the diagonal instead of a noise site (MeasuredNoiseGP,
+        mngp.py:75-97: likelihood log N(y - m; 0, K_theta + diag(noise_vec)), noise 0)"""
         if model._fused is None and not self.CALLABLE_KERNEL:
             raise NotImplementedError("fit() needs kernel 'RBF', 'Matern' or 'Periodic'")
         self.m, self.jitter = model, float(jitter)
+        if noise_vec is not None:
+            self.noise_vec = np.asarray(noise_vec, dtype=np.float64).reshape(-1)
         X, y = model._train_arrays()
         self.X, self.d, self.y0 = X, X.shape[1], y
         self.kind = model._fused
@@ -222,7 +236,7 @@ class ProgramLogJoint:
         self.hierarchical = any(vars(sites[k].prior) != vars(sites2[k].prior) for k in sites)
 
     def _model_program(self):
-        return gp_model_program(self.m, self.d, self.kind)
+        return gp_model_program(self.m, self.d, self.kind, noise_site=self.noise_vec is None)
 
     def _site_values(self, u):
         """u -> {site name: constrained value, shaped as the program sampled it}"""
@@ -285,12 +299,14 @@ class ProgramLogJoint:
         if self._lik_fn is not None:
             return self._lik_fn(th, yres)
         val, g, alpha, info = self.m.ctx.mll(self.kind, self.X, yres, th, self.jitter, want_grad=True,
-                                             want_alpha=self.has_mean_params)
+                                             want_alpha=self.has_mean_params, noise_vec=self.noise_vec)[:4]
         return val, g, alpha, info
 
     def _valid(self, th):
         if _is_nngp(self.kind):     # the depth slots may be 0; var_w, noise and var_b must be positive
             return np.all(np.isfinite(th)) and np.all(th[self.d:] > 0)
+        if self.noise_vec is not None:   # noise is 0: the fixed vector is the noise
+            return np.all(np.isfinite(th)) and np.all(th[:self.d + 1] > 0)
         return np.all(np.isfinite(th)) and np.all(th[:self.d + 2] > 0)
 
     def _dval_dth(self, th, g):
@@ -299,6 +315,8 @@ class ProgramLogJoint:
             out = np.zeros_like(th)
             out[self.d:] = g[self.d:] / th[self.d:]
             return out
+        if self.noise_vec is not None:   # noise is the constant 0
+            return np.where(np.arange(self.d + 3) == self.d + 1, 0.0, g / np.where(th == 0, 1.0, th))
         return g / th
 
     def __call__(self, u, jacobian):
@@ -329,9 +347,13 @@ class ProgramLogJoint:
         out = [(-np.inf, np.zeros(self.dim))] * len(rows)
         live = [r for r, row in enumerate(rows) if self._valid(row[1])]
         if live:
-            vals, G, A, info = self.m.ctx.mll_draws(self.kind, self.X, np.stack([rows[r][3] for r in live]),
-                                                    np.stack([rows[r][1] for r in live]), self.jitter, want_grad=True,
-                                                    want_alpha=self.has_mean_params)
+            Y, TH = np.stack([rows[r][3] for r in live]), np.stack([rows[r][1] for r in live])
+            if self.noise_vec is None:
+                vals, G, A, info = self.m.ctx.mll_draws(self.kind, self.X, Y, TH, self.jitter, want_grad=True,
+                                                        want_alpha=self.has_mean_params)
+            else:   # one shared noise vector (nv_stride 0)
+                vals, G, A, _, info = self.m.ctx.mll_draws_v(self.kind, self.X, Y, TH, self.noise_vec, self.jitter,
+                                                             want_grad=True, want_alpha=self.has_mean_params)
             for j, r in enumerate(live):
                 u, th, sites, _ = rows[r]
                 out[r] = self._joint(u, th, sites, float(vals[j]), G[j], None if A is None else A[j], int(info[j]), jacobian)
@@ -371,6 +393,8 @@ class ProgramLogJoint:
             for s in self.sites:
                 out[s.name][r] = np.asarray(s.prior.transform(u[o:o + s.size])).reshape(s.shape)
                 o += s.size
+        if self.noise_vec is not None:      # numpyro.deterministic("noise", 0.0), mngp.py:85
+            out["noise"] = np.zeros(U.shape[0])
         return out
 
 

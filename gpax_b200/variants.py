@@ -61,6 +61,19 @@ class _MeasuredNoiseLogJoint:
         th = self.theta_of(u)
         val, g, _, info, _ = self.base.m.ctx.mll(self.kind, self.base.X, self.base.y, th, self.base.jitter, True, False, self.nv)
         self.n_evals += 1
+        return self._joint(u, th, val, g, info, jacobian)
+
+    def batch(self, U, jacobian):
+        """the rows of U (one per chain of a vectorized NUTS round) in one b2gp_mll_draws_v call with the shared measured
+        noise; row r is self(U[r], jacobian) bit for bit"""
+        TH = np.stack([self.theta_of(u) for u in U])
+        vals, G, _, _, info = self.base.m.ctx.mll_draws_v(self.kind, self.base.X, self.base.y, TH, self.nv, self.base.jitter,
+                                                          want_grad=True)
+        self.n_evals += len(U)
+        out = [self._joint(u, th, float(v), g, int(i), jacobian) for u, th, v, g, i in zip(U, TH, vals, G, info)]
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, th, val, g, info, jacobian):
         if info != 0 or not np.isfinite(val):
             return -np.inf, np.zeros(self.dim)
         grad = np.zeros(self.dim)
@@ -94,12 +107,18 @@ class MeasuredNoiseGP(ExactGP):
     def fit(self, rng_key, X, y, measured_noise, num_warmup: int = 2000, num_samples: int = 2000, num_chains: int = 1,
             chain_method: str = "sequential", progress_bar: bool = True, print_summary: bool = True, device=None,
             **kwargs: float) -> None:
-        """mngp.py:100-158."""
-        from .inference import run_nuts
+        """mngp.py:100-158.  kernel_prior / mean_fn_prior programs go through ProgramLogJoint with the measured noise as
+        its fixed noise vector."""
+        from .inference import ProgramLogJoint, run_nuts
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
         self.measured_noise = np.asarray(measured_noise, dtype=np.float64)
-        lj = _MeasuredNoiseLogJoint(self, self.measured_noise, kwargs.get("jitter", 1e-6))
+        jitter = kwargs.get("jitter", 1e-6)
+        if self.kernel_prior is not None or (self.mean_fn is not None and self.mean_fn_prior is not None):
+            _need_fused(self)
+            lj = ProgramLogJoint(self, jitter, noise_vec=self.measured_noise)
+        else:
+            lj = _MeasuredNoiseLogJoint(self, self.measured_noise, jitter)
         self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             self._print_summary()
@@ -174,6 +193,17 @@ class VarNoiseGP(ExactGP):
              "noise": np.zeros_like(np.asarray(params["k_noise_scale"], dtype=np.float64)), "period": params.get("period")}
         return _theta_rows(n, d, batched)
 
+    def _log_noise_mean(self, X, params, batched, S):
+        """log noise_mean_fn at X (hskgp.py:117-121, 192-200): [N], or [S, N] when the function has a prior and params
+        carry a draw axis (evaluated once per draw, as _residuals does for mean_fn)"""
+        f = self.noise_mean_fn
+        if self.noise_mean_fn_prior is None:
+            return np.log(np.asarray(f(X), dtype=np.float64)).squeeze()
+        if not batched:
+            return np.log(np.asarray(f(X, params), dtype=np.float64)).squeeze()
+        return np.stack([np.log(np.asarray(f(X, {k: np.asarray(v)[s] for k, v in params.items()}), dtype=np.float64)).reshape(-1)
+                         for s in range(S)])
+
     def _both_posteriors(self, X_new, params, batched, want, **kwargs):
         """hskgp.py:165-204 for one or S draws: the main GP with ZERO noise in k_XX and k_pp, and the noise GP's
         posterior mean of the log-variances; returns (out dict of the main GP, predicted noise variance [S, P])."""
@@ -195,8 +225,7 @@ class VarNoiseGP(ExactGP):
         log_var = np.asarray(params["log_var"], dtype=np.float64).reshape(S, -1)
         shift_tr = shift_new = 0.0
         if self.noise_mean_fn is not None:                                                    # hskgp.py:192-200
-            a = (lambda x: self.noise_mean_fn(x, params)) if self.noise_mean_fn_prior else self.noise_mean_fn
-            shift_tr, shift_new = np.log(np.asarray(a(X))).squeeze(), np.log(np.asarray(a(Xn))).squeeze()
+            shift_tr, shift_new = self._log_noise_mean(X, params, batched, S), self._log_noise_mean(Xn, params, batched, S)
         nout = self.ctx.posterior(self._noise_fused, X, log_var - shift_tr, Xn, self._noise_theta(params, batched), True, jitter,
                                   ("mean",))
         bad = (out["info"] != 0) | (nout["info"] != 0)
@@ -248,11 +277,17 @@ class VarNoiseGP(ExactGP):
             chain_method: str = "sequential", progress_bar: bool = True, print_summary: bool = True, device=None,
             **kwargs: float) -> None:
         """NUTS over (main kernel, noise kernel, log_var[N]) for hskgp.py:105-149; both multivariate-normal terms and
-        their gradients (w.r.t. the kernel parameters AND the latent log-variances) come from b2gp_mll / b2gp_mll_v."""
+        their gradients (w.r.t. the kernel parameters AND the latent log-variances) come from b2gp_mll / b2gp_mll_v.
+        kernel_prior, noise_kernel_prior, mean_fn_prior and noise_mean_fn_prior programs go through
+        _VarNoiseProgramLogJoint."""
         from .inference import run_nuts
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y
-        lj = _VarNoiseLogJoint(self, kwargs.get("jitter", 1e-6))
+        jitter = kwargs.get("jitter", 1e-6)
+        programs = self.kernel_prior is not None or self.noise_kernel_prior is not None or \
+            (self.mean_fn is not None and self.mean_fn_prior is not None) or \
+            (self.noise_mean_fn is not None and self.noise_mean_fn_prior is not None)
+        lj = _VarNoiseProgramLogJoint(self, jitter) if programs else _VarNoiseLogJoint(self, jitter)
         self.mcmc = run_nuts(lj, rng_key, num_warmup, num_samples, num_chains, progress_bar, chain_method)
         if print_summary:
             s = self.get_samples(1)
@@ -263,17 +298,19 @@ class VarNoiseGP(ExactGP):
 
 class _VarNoiseLogJoint:
     """u = [log k_length (d), log k_scale, log k_noise_length (1), log k_noise_scale, log_var (N)] -- hskgp.py:105-163 with
-    the default LogNormal(0, 1) priors (or gpax_b200.priors objects for the two lengthscales)."""
+    the default LogNormal(0, 1) priors (or gpax_b200.priors objects for the two lengthscales), a fixed mean_fn and a
+    fixed noise_mean_fn (log_var ~ N(log noise_mean_fn(X), k_noise))."""
 
     def __init__(self, model, jitter):
         _need_fused(model)
-        if model.kernel_prior is not None or model.noise_kernel_prior is not None or model.mean_fn_prior is not None \
-                or model.noise_mean_fn is not None:
-            raise NotImplementedError("VarNoiseGP.fit: NumPyro-program priors / probabilistic mean functions are not interpreted")
         self.m, self.jitter = model, float(jitter)
         self.X, self.y = model._train_arrays()
         if model.mean_fn is not None:
             self.y = self.y - np.asarray(model.mean_fn(self.X), dtype=np.float64).squeeze()
+        self.mu_n = None
+        if model.noise_mean_fn is not None:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                self.mu_n = model._log_noise_mean(self.X, None, False, 1)
         self.N, self.d = self.X.shape
         d = self.d
         lp = model.lengthscale_prior_dist or P.LogNormal(0.0, 1.0)
@@ -298,13 +335,40 @@ class _VarNoiseLogJoint:
         thn[:d], thn[d], thn[d + 1] = t[d + 1], t[d + 2], 0.0
         return t, th, thn
 
+    def _lv_res(self, lv):
+        return lv if self.mu_n is None else lv - self.mu_n
+
     def __call__(self, u, jacobian):
-        d, ctx = self.d, self.m.ctx
+        ctx = self.m.ctx
         t, th, thn = self._thetas(u)
         lv = u[self.nk:]
         self.n_evals += 1
-        vA, gA, alphaA, infoA = ctx.mll(self.m._noise_fused, self.X, lv, thn, self.jitter, True, True)      # log N(log_var; 0, k_noise)
+        if self.mu_n is not None and not np.all(np.isfinite(self.mu_n)):
+            return -np.inf, np.zeros(self.dim)
+        vA, gA, alphaA, infoA = ctx.mll(self.m._noise_fused, self.X, self._lv_res(lv), thn, self.jitter, True, True)   # log N(log_var; mu_n, k_noise)
         vB, gB, _, infoB, gnv = ctx.mll(self.m._fused, self.X, self.y, th, self.jitter, True, False, np.exp(lv))
+        return self._joint(u, t, vA, gA, alphaA, infoA, vB, gB, infoB, gnv, jacobian)
+
+    def batch(self, U, jacobian):
+        """the rows of U (one per chain of a vectorized NUTS round): one b2gp_mll_draws call for the noise GP and one
+        b2gp_mll_draws_v call for the main GP; row r is self(U[r], jacobian) bit for bit"""
+        ctx, U = self.m.ctx, np.asarray(U, dtype=np.float64)
+        self.n_evals += len(U)
+        if self.mu_n is not None and not np.all(np.isfinite(self.mu_n)):
+            return np.full(len(U), -np.inf), np.zeros((len(U), self.dim))
+        parts = [self._thetas(u) for u in U]
+        LV = U[:, self.nk:]
+        vA, GA, AA, iA = ctx.mll_draws(self.m._noise_fused, self.X, self._lv_res(LV), np.stack([p[2] for p in parts]), self.jitter,
+                                       want_grad=True, want_alpha=True)
+        vB, GB, _, GNV, iB = ctx.mll_draws_v(self.m._fused, self.X, self.y, np.stack([p[1] for p in parts]),
+                                             np.stack([np.exp(lv) for lv in LV]), self.jitter, want_grad=True)
+        out = [self._joint(u, p[0], float(vA[r]), GA[r], AA[r], int(iA[r]), float(vB[r]), GB[r], int(iB[r]), GNV[r], jacobian)
+               for r, (u, p) in enumerate(zip(U, parts))]
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    def _joint(self, u, t, vA, gA, alphaA, infoA, vB, gB, infoB, gnv, jacobian):
+        d = self.d
+        lv = u[self.nk:]
         if infoA != 0 or infoB != 0 or not (np.isfinite(vA) and np.isfinite(vB)):
             return -np.inf, np.zeros(self.dim)
         val = vA + vB
@@ -326,6 +390,219 @@ class _VarNoiseLogJoint:
         T = np.stack([self._thetas(u)[0] for u in U])
         return {"k_length": T[:, :d], "k_scale": T[:, d], "k_noise_length": T[:, d + 1:d + 2], "k_noise_scale": T[:, d + 2],
                 "log_var": U[:, self.nk:], "noise": np.zeros(len(U))}
+
+
+class _VarNoiseProgramLogJoint:
+    """The log joint of VarNoiseGP.model (hskgp.py:105-149) when any of kernel_prior, noise_kernel_prior, mean_fn_prior,
+    noise_mean_fn_prior is a program (gpax_b200.priors' sample / plate).  u holds the sites in the reference's order:
+    noise-kernel sites, noise-mean sites, log_var [N], kernel sites (period for a Periodic kernel), mean sites.
+
+      value = log N(lv; mu_n, K_n) [b2gp_mll]  +  log N(y - m; 0, K + diag(e^lv)) [b2gp_mll_v]  +  sum log p(site) (+ Jac.)
+
+    d value / d lv = -alpha_n + g_nv e^lv in closed form.  The programs are differenced centrally over their own sites
+    only (never over the N log_var coordinates): theta, theta_n, mu_n (against +alpha_n) and m (against alpha_m)."""
+
+    FD_STEP = 1e-5
+    INIT_TRIES = 100
+
+    def __init__(self, model, jitter):
+        _need_fused(model)
+        if model._noise_fused is None:
+            raise NotImplementedError("noise_kernel must be 'RBF', 'Matern' or 'Periodic'")
+        self.m, self.jitter = model, float(jitter)
+        self.kind, self.nkind = model._fused, model._noise_fused
+        self.X, self.y0 = model._train_arrays()
+        self.N, self.d = self.X.shape
+        self.mean_params = model.mean_fn is not None and model.mean_fn_prior is not None
+        self.noise_mean_params = model.noise_mean_fn is not None and model.noise_mean_fn_prior is not None
+        self.fixed_mean = None if model.mean_fn is None or self.mean_params else \
+            np.asarray(model.mean_fn(self.X), dtype=np.float64).squeeze()
+        self.fixed_mu_n = None
+        if model.noise_mean_fn is not None and not self.noise_mean_params:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                self.fixed_mu_n = model._log_noise_mean(self.X, None, False, 1)
+        _, s1, _ = P.run_program(self._noise_program)
+        _, s2, _ = P.run_program(self._main_program)
+        self.pre, self.post = list(s1.values()), list(s2.values())
+        n1 = sum(s.size for s in self.pre)
+        self.lv = slice(n1, n1 + self.N)
+        self.dim = n1 + self.N + sum(s.size for s in self.post)
+        # (site, its slice of u) in u's order
+        self.blocks, o = [], 0
+        for s in self.pre + [None] + self.post:
+            if s is None:
+                o += self.N
+                continue
+            self.blocks.append((s, slice(o, o + s.size)))
+            o += s.size
+        self.prog_idx = np.concatenate([np.arange(self.dim)[sl] for _, sl in self.blocks]) if self.blocks else np.zeros(0, int)
+        # does any site's distribution depend on the value of another (two runs at different values)?
+        sites1 = self._run(np.full(self.dim, 0.37))[4]
+        self.hierarchical = any(vars(sites1[s.name].prior) != vars(s.prior) for s, _ in self.blocks)
+        self._u0 = None
+        self.n_evals = 0
+
+    # ---- the host programs
+    def _noise_program(self):
+        m = self.m
+        if m.noise_kernel_prior is not None:
+            nkp = m.noise_kernel_prior()
+        else:                                                                                # hskgp.py:151-163
+            nkp = {"k_noise_scale": P.sample("k_noise_scale", P.LogNormal(0.0, 1.0)),
+                   "k_noise_length": P.sample("k_noise_length", m.noise_lengthscale_prior_dist or P.LogNormal(0.0, 1.0))}
+        nmp = m.noise_mean_fn_prior() if self.noise_mean_params else None
+        return nkp, nmp
+
+    def _main_program(self):
+        from .inference import kernel_program
+        kp = kernel_program(self.m, self.d, self.kind)
+        mp = self.m.mean_fn_prior() if self.mean_params else None
+        return kp, mp
+
+    def _run(self, u):
+        """u -> (theta [d+3], theta_n [d+3], m [N] or None, mu_n [N] or None, sites with their priors)"""
+        vals = {s.name: np.asarray(s.prior.transform(u[sl])).reshape(s.shape) for s, sl in self.blocks}
+        (nkp, nmp), s1, _ = P.run_program(self._noise_program, vals)
+        (kp, mp), s2, _ = P.run_program(self._main_program, vals)
+        d = self.d
+        thn = np.ones(d + 3)
+        thn[:d] = np.asarray(nkp["k_noise_length"], dtype=np.float64).reshape(-1)[0]     # one noise lengthscale
+        thn[d], thn[d + 1] = float(np.asarray(nkp["k_noise_scale"]).reshape(-1)[0]), 0.0
+        th = np.ones(d + 3)
+        ell = np.asarray(kp["k_length"], dtype=np.float64).reshape(-1)
+        th[:d] = np.broadcast_to(ell, (d,)) if ell.size in (1, d) else np.nan
+        th[d], th[d + 1] = float(np.asarray(kp["k_scale"]).reshape(-1)[0]), 0.0
+        if self.kind == "Periodic":
+            if kp.get("period") is None:
+                raise ValueError("the Periodic kernel needs 'period' in the dict kernel_prior returns")
+            th[d + 2] = float(np.asarray(kp["period"]).reshape(-1)[0])
+        mean = np.asarray(self.m.mean_fn(self.X, mp), dtype=np.float64).squeeze() if self.mean_params else self.fixed_mean
+        mu_n = self.fixed_mu_n
+        if self.noise_mean_params:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                mu_n = np.log(np.asarray(self.m.noise_mean_fn(self.X, nmp), dtype=np.float64)).squeeze()
+        return th, thn, mean, mu_n, {**s1, **s2}
+
+    def _valid(self, th, thn, mean, mu_n):
+        ok = np.all(np.isfinite(th)) and np.all(th[:self.d + 1] > 0) and np.all(np.isfinite(thn)) and np.all(thn[:self.d + 1] > 0)
+        ok = ok and (self.kind != "Periodic" or th[self.d + 2] > 0)
+        return bool(ok and (mean is None or np.all(np.isfinite(mean))) and (mu_n is None or np.all(np.isfinite(mu_n))))
+
+    def _log_prior(self, u, sites, jacobian, want_grad=True):
+        val, grad = 0.0, np.zeros(self.dim)
+        for s0, sl in self.blocks:
+            pr, uu = sites[s0.name].prior, u[sl]
+            t = np.asarray(pr.transform(uu), dtype=np.float64)
+            val += float(np.sum(pr.log_prob(t)))
+            if want_grad:
+                grad[sl] = np.asarray(pr.dlog_prob(t)) * np.asarray(pr.dtheta_du(uu))
+            if jacobian:
+                val += float(np.sum(pr.log_abs_jac(uu)))
+                if want_grad:
+                    grad[sl] += np.asarray(pr.dlog_abs_jac(uu))
+        return val, grad
+
+    # ---- the log joint
+    def init_u(self):
+        """init_to_median on the program sites; log_var at the default route's start, log(0.1 var(y)).  When the programs
+        give an invalid point at the medians (a noise mean a + b x is 0 at a = b = 0), up to INIT_TRIES points uniform in
+        (-2, 2) on the unconstrained scale of the program sites (NumPyro's init_to_uniform fallback), from a fixed seed so
+        that every chain and chain method starts alike.  Host programs only: no likelihood is evaluated."""
+        if self._u0 is None:
+            u = np.zeros(self.dim)
+            for s, sl in self.blocks:
+                u[sl] = float(s.prior.inverse(s.prior.median()))
+            u[self.lv] = np.log(0.1 * np.var(self.y0) + 1e-8)
+            rng = np.random.default_rng(0)
+            for _ in range(self.INIT_TRIES):
+                if self._valid(*self._run(u)[:4]):
+                    break
+                u[self.prog_idx] = rng.uniform(-2.0, 2.0, len(self.prog_idx))
+            self._u0 = u
+        return self._u0.copy()
+
+    def __call__(self, u, jacobian):
+        u = np.asarray(u, dtype=np.float64)
+        run = self._run(u)
+        self.n_evals += 1
+        if not self._valid(*run[:4]):
+            return -np.inf, np.zeros(self.dim)
+        th, thn, mean, mu_n, _ = run
+        lv = u[self.lv]
+        ctx = self.m.ctx
+        vA, gA, alphaA, infoA = ctx.mll(self.nkind, self.X, lv if mu_n is None else lv - mu_n, thn, self.jitter, True, True)
+        vB, gB, alphaB, infoB, gnv = ctx.mll(self.kind, self.X, self.y0 if mean is None else self.y0 - mean, th, self.jitter, True,
+                                             self.mean_params, np.exp(lv))
+        return self._joint(u, run, vA, gA, alphaA, infoA, vB, gB, alphaB, infoB, gnv, jacobian)
+
+    def batch(self, U, jacobian):
+        """the rows of U (one per chain of a vectorized NUTS round): the host programs per row, then one b2gp_mll_draws
+        call (noise GP) and one b2gp_mll_draws_v call (main GP) over the valid rows; row r is self(U[r], jacobian) bit for
+        bit"""
+        U = np.asarray(U, dtype=np.float64)
+        runs = [self._run(u) for u in U]
+        self.n_evals += len(U)
+        out = [(-np.inf, np.zeros(self.dim))] * len(U)
+        live = [r for r, run in enumerate(runs) if self._valid(*run[:4])]
+        if live:
+            ctx = self.m.ctx
+            LV = [U[r][self.lv] for r in live]
+            RA = np.stack([lv if runs[r][3] is None else lv - runs[r][3] for r, lv in zip(live, LV)])
+            RB = np.stack([self.y0 if runs[r][2] is None else self.y0 - runs[r][2] for r in live])
+            vA, GA, AA, iA = ctx.mll_draws(self.nkind, self.X, RA, np.stack([runs[r][1] for r in live]), self.jitter,
+                                           want_grad=True, want_alpha=True)
+            vB, GB, AB, GNV, iB = ctx.mll_draws_v(self.kind, self.X, RB, np.stack([runs[r][0] for r in live]),
+                                                  np.stack([np.exp(lv) for lv in LV]), self.jitter, want_grad=True,
+                                                  want_alpha=self.mean_params)
+            for j, r in enumerate(live):
+                out[r] = self._joint(U[r], runs[r], float(vA[j]), GA[j], AA[j], int(iA[j]), float(vB[j]), GB[j],
+                                     None if AB is None else AB[j], int(iB[j]), GNV[j], jacobian)
+        return np.array([o[0] for o in out]), np.stack([o[1] for o in out])
+
+    @staticmethod
+    def _dval_dth(th, g):
+        """d value / d theta from d value / d log(theta); the noise slot (0) is a constant"""
+        out = np.zeros_like(th)
+        nz = th != 0
+        out[nz] = g[nz] / th[nz]
+        return out
+
+    def _joint(self, u, run, vA, gA, alphaA, infoA, vB, gB, alphaB, infoB, gnv, jacobian):
+        if infoA != 0 or infoB != 0 or not (np.isfinite(vA) and np.isfinite(vB)):
+            return -np.inf, np.zeros(self.dim)
+        th, thn, mean, mu_n, sites = run
+        # site densities: analytic gradient, unless the programs are hierarchical (then differenced below)
+        lp, grad = self._log_prior(u, sites, jacobian, want_grad=not self.hierarchical)
+        grad[self.lv] = -alphaA + gnv * np.exp(u[self.lv])
+        dB, dA = self._dval_dth(th, gB), self._dval_dth(thn, gA)
+        h = self.FD_STEP
+        for k in self.prog_idx:
+            e = np.zeros(self.dim)
+            e[k] = h
+            thp, thnp, mp_, mup, sp = self._run(u + e)
+            thm, thnm, mm_, mum, sm_ = self._run(u - e)
+            grad[k] += float(np.dot(dB, (thp - thm) / (2 * h))) + float(np.dot(dA, (thnp - thnm) / (2 * h)))
+            if self.mean_params:
+                grad[k] += float(np.dot(alphaB, (mp_ - mm_) / (2 * h)))
+            if self.noise_mean_params:
+                grad[k] += float(np.dot(alphaA, (mup - mum) / (2 * h)))
+            if self.hierarchical:
+                grad[k] += (self._log_prior(u + e, sp, jacobian, False)[0] - self._log_prior(u - e, sm_, jacobian, False)[0]) / (2 * h)
+        return vA + vB + lp, grad
+
+    def to_dict(self, U):
+        """program sites and log_var in u's order, shaped as sampled; noise 0 (the main kernel's noise, hskgp.py:147)"""
+        U = np.atleast_2d(U)
+        out = {}
+        for s in self.pre:
+            out[s.name] = None
+        out["log_var"] = U[:, self.lv]
+        for s in self.post:
+            out[s.name] = None
+        for s, sl in self.blocks:
+            out[s.name] = np.stack([np.asarray(s.prior.transform(u[sl])).reshape(s.shape) for u in U])
+        out["noise"] = np.zeros(len(U))
+        return out
 
 
 # ---------------------------------------------------------------------------------------------- vExactGP

@@ -457,10 +457,21 @@ int  b2gp_mll_batch(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const d
  *   int8 (ozaki != 0):         one draw at a time (those GEMMs take one draw), one host sync for the call.
  * Groups hold as many draws as an eighth of the device memory takes (option draw_batch: 1 = one draw per group, B >= 2 =
  * groups of B); each group counts once in the route counter mll_draws_batch.  Host fp64 arrays only: B2GP_FLAG_F32 and
- * B2GP_FLAG_DEVICE_PTRS give B2GP_ERR_UNSUPPORTED before any launch; there is no noise-vector or multi-task form.      */
+ * B2GP_FLAG_DEVICE_PTRS give B2GP_ERR_UNSUPPORTED before any launch; there is no multi-task form (the noise-vector
+ * form is b2gp_mll_draws_v).                                                                                           */
 int  b2gp_mll_draws(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
                     int64_t S, const double* theta, double jitter, unsigned flags, double* value, double* grad,
                     double* alpha_out, int* info);
+
+/* b2gp_mll_draws with a per-point noise vector per draw (the chains of MeasuredNoiseGP / VarNoiseGP): draw s is
+ * b2gp_mll_v(kind, X, yres + s * yres_stride, theta + s * (d+3), noise_vec + s * nv_stride) and returns that call's
+ * value, grad, alpha, grad_noise_vec and info bit for bit, whatever S and the grouping, on every route of
+ * b2gp_mll_draws.  noise_vec is required; nv_stride = 0 shares one [N] vector between the draws, else >= N doubles
+ * between draws.  grad_noise_vec[S,N] (optional, needs grad) is d value / d noise_vec.  A draw with info[s] != 0 has NaN
+ * in all of its outputs.  Routes, groups, the mll_draws_batch counter and the refusals are b2gp_mll_draws'.            */
+int  b2gp_mll_draws_v(b2gp_ctx* ctx, int kind, const double* X, int64_t N, const double* yres, int64_t yres_stride, int d,
+                      int64_t S, const double* theta, const double* noise_vec, int64_t nv_stride, double jitter,
+                      unsigned flags, double* value, double* grad, double* alpha_out, double* grad_noise_vec, int* info);
 
 /* The multi-task counterpart (the likelihood of viMTDKL.model, gpax/models/vi_mtdkl.py): log N(yres; 0, K) with K the
  * LCM covariance of b2gp_mll_multitask on the embedding z = MLP(X), expanded to the GP rows:
