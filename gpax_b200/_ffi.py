@@ -119,7 +119,9 @@ SIGNATURES = {
                                  _vp, _vp, _vp, _vp, C.c_double, C.c_uint, _dp, _vp, _vp, _vp, _vp, _vp, _ip]),
     "b2gp_bnn_loglik": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_double, C.c_uint,
                                   _dp, _dp, _vp]),
-    "b2gp_bnn_predict": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
+    "b2gp_bnn_loglik_draws": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int64, C.c_int, _vp, C.c_int, C.c_int64, _vp,
+                                        C.c_int64, _vp, C.c_uint, _vp, _vp, _vp]),
+    "b2gp_bnn_predict":(C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, C.c_int64, _vp,
                                    _vp, C.c_int64, _vp, _vp, C.c_uint]),
     "b2gp_bnn_predict_grad": (C.c_int, [_vp, _vp, C.c_int64, C.c_int64, C.c_int, _vp, C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp,
                                         C.c_uint]),
@@ -823,6 +825,33 @@ class Context:
         self._check(self.lib.b2gp_bnn_loglik(self.h, Xp, N, D, yp, int(w[-1]), int(w.size), _ptr(w), int(act), _ptr(p),
                                              float(sigma), flags, C.byref(val), C.byref(gs), _ptr(gp)))
         return val.value, gs.value, gp
+
+    def bnn_loglik_draws(self, X, y, widths, act, params, sigma, want_params=True):
+        """bnn_loglik for S weight sets on one X and y (b2gp_bnn_loglik_draws): draw s is bnn_loglik(X, y, widths, act,
+        params[s], sigma[s]) bit for bit.  X, y as in bnn_loglik; params [S, P] (rows may be a strided view's) and sigma
+        [S].  Returns (values [S], d/dsigma [S], grad_params [S, P] or None)."""
+        X, Xp, flags = self._arg(X)
+        y, yp, yflags = self._arg(y)
+        if flags != yflags:
+            raise ValueError("X and y must both be host arrays or both DeviceArrays")
+        N, D = X.shape
+        w = np.ascontiguousarray(widths, dtype=np.int64).reshape(-1)
+        p = np.asarray(params, dtype=np.float64)
+        if p.ndim != 2 or p.shape[1] != _mlp_nparams(D, w):
+            raise ValueError(f"params has shape {p.shape}, expected (S, {_mlp_nparams(D, w)}) for D={D}, widths={w.tolist()}")
+        if p.strides[1] != 8 or p.strides[0] % 8 or p.strides[0] < 8 * p.shape[1]:
+            p = np.ascontiguousarray(p)
+        S = p.shape[0]
+        sg = _f64(sigma).reshape(-1)
+        if sg.size != S:
+            raise ValueError(f"sigma has {sg.size} entries for {S} weight sets")
+        if tuple(y.shape) != (N, int(w[-1])):
+            raise ValueError(f"y has shape {tuple(y.shape)}, the network needs ({N}, {int(w[-1])})")
+        val, gs = np.empty(S), np.empty(S)
+        gp = np.empty((S, p.shape[1])) if want_params else None
+        self._check(self.lib.b2gp_bnn_loglik_draws(self.h, Xp, N, D, yp, int(w[-1]), int(w.size), _ptr(w), int(act), S, _ptr(p),
+                                                   p.strides[0] // 8, _ptr(sg), flags, _ptr(val), _ptr(gs), _ptr(gp)))
+        return val, gs, gp
 
     def bnn_predict(self, X, widths, act, params, sigma=None, eps=None):
         """loc [S, P, O] = MLP(X) for S weight sets and, given eps [S, n, P, O] and sigma [S], y_sampled [S, P, O] =

@@ -3,7 +3,8 @@ bnn.py -- the fully Bayesian MLP with the reference's surface: `BNN` (gpax/model
 A tanh MLP over `hidden_dim` (default [64, 32]) and a linear output layer map X [N, D] to the mean of y [N, O]; NUTS
 samples every weight (Normal(0, 1)) and bias (Cauchy(0, 1)) together with the observation noise (LogNormal(0, 1) or
 `noise_prior_dist`).  Every numerical step is on the GPU: b2gp_bnn_loglik evaluates sum log N(y; MLP(X), noise) and its
-gradient w.r.t. the noise and every weight for each leapfrog step, b2gp_bnn_predict runs the network for all draws at
+gradient w.r.t. the noise and every weight for each leapfrog step (b2gp_bnn_loglik_draws for every chain of a round under
+chain_method="vectorized"), b2gp_bnn_predict runs the network for all draws at
 once with the predictive sampling in the same epilogue.  The sampler is the host NUTS loop the other models use
 (inference.run_nuts).
 
@@ -58,13 +59,38 @@ class BNNLogJoint:
                        np.median(self.rng.standard_cauchy((INIT_MEDIAN_DRAWS, n)), axis=0))
         return np.concatenate([[u_noise], net])
 
+    def _sigma(self, u):
+        """the noise of u, or None where it is not a valid scale (the likelihood is not evaluated there)"""
+        sigma = float(self.noise.transform(u[0]))
+        return sigma if np.isfinite(sigma) and sigma > 0.0 else None
+
     def __call__(self, u, jacobian):
         self.n_evals += 1
-        pr, flat = self.noise, u[1:]
-        sigma = float(pr.transform(u[0]))
-        if not (np.isfinite(sigma) and sigma > 0.0):
+        sigma = self._sigma(u)
+        if sigma is None:
             return -np.inf, np.zeros(self.dim)
-        val, gs, gp = self._lik(flat, sigma)
+        val, gs, gp = self._lik(u[1:], sigma)
+        return self._joint(u, sigma, val, gs, gp, jacobian)
+
+    def batch(self, U, jacobian):
+        """`batch(U, jacobian) -> (values [k], grads [k, dim])` for run_nuts' vectorized chains: the rows with a valid noise
+        in one b2gp_bnn_loglik_draws call on the resident X and y, each finished as __call__ finishes it, so row r is
+        self(U[r], jacobian) bit for bit"""
+        U = np.asarray(U, dtype=np.float64)
+        self.n_evals += len(U)
+        vals, grads = np.full(len(U), -np.inf), np.zeros((len(U), self.dim))
+        sig = [self._sigma(u) for u in U]
+        ok = [r for r, s in enumerate(sig) if s is not None]
+        if ok:
+            m = self.m
+            v, gs, gp = m.ctx.bnn_loglik_draws(self.Xd, self.yd, m.widths, _ffi.ACT_TANH, U[ok, 1:], [sig[r] for r in ok])
+            for i, r in enumerate(ok):
+                vals[r], grads[r] = self._joint(U[r], sig[r], float(v[i]), float(gs[i]), gp[i], jacobian)
+        return vals, grads
+
+    def _joint(self, u, sigma, val, gs, gp, jacobian):
+        """the log joint and its gradient w.r.t. u from the likelihood's value and gradients at sigma = noise(u)"""
+        pr, flat = self.noise, u[1:]
         ds = float(pr.dtheta_du(u[0]))
         val += float(pr.log_prob(sigma))
         gu = (gs + float(pr.dlog_prob(sigma))) * ds
@@ -170,7 +196,9 @@ class BNN:
     # ---- fit
     def fit(self, rng_key, X, y, num_warmup: int = 2000, num_samples: int = 2000, num_chains: int = 1,
             chain_method: str = "sequential", progress_bar: bool = True, print_summary: bool = True, device=None) -> None:
-        """spm.py:88-130: NUTS over the weights and the noise (chains run one after another), then `mu` on X_train"""
+        """spm.py:88-130: NUTS over the weights and the noise, then `mu` on X_train.  chain_method "vectorized" runs the
+        chains in lock-step, each round's likelihoods in one b2gp_bnn_loglik_draws call; any other value runs them one
+        after another.  Both give the same samples bit for bit."""
         from .inference import MCMCResult, run_nuts
         X, y = self._set_data(X, y)
         self.X_train, self.y_train = X, y

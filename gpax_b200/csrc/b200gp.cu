@@ -2221,11 +2221,11 @@ static MlpBack mlp_back_layout(const MlpShape& s) {
     return b;
 }
 
-// The backward pass from gz = d value / dz (at base, the start of mlp[3]) to grad_params (HOST): per layer the bias
-// gradient (column sum), the weight gradient H_l^T G (gemm_nt on the transposes) and, below the first layer, G W_l^T
-// masked by the activation's derivative.
+// The backward pass from gz = d value / dz (at base, the start of mlp[3]) to grad_params (HOST, or a device array when
+// dev_out): per layer the bias gradient (column sum), the weight gradient H_l^T G (gemm_nt on the transposes) and, below
+// the first layer, G W_l^T masked by the activation's derivative.
 static int mlp_backward_dev(b2gp_ctx* ctx, cudaStream_t st, const MlpShape& s, const MlpBack& b, int act, const double* dP,
-                            const std::vector<double*>& H, double* base, double* grad_params) {
+                            const std::vector<double*>& H, double* base, double* grad_params, bool dev_out = false) {
     const int64_t N = s.N, ldN = b.ldN;
     double *gp = base + b.o_gp, *G0 = base + b.o_g0, *G1 = base + b.o_g1, *Ht = base + b.o_ht, *Gt = base + b.o_gt;
     double* G = base;   // d value / d (pre-activation output of layer l), [N, out_l]
@@ -2242,7 +2242,8 @@ static int mlp_backward_dev(b2gp_ctx* ctx, cudaStream_t st, const MlpShape& s, c
             G = Gn;
         }
     }
-    CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, gp, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, gp, (size_t)s.nparams * 8, dev_out ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                                  st));
     return B2GP_OK;
 }
 
@@ -2577,16 +2578,24 @@ static int bnn_optin(b2gp_ctx* ctx) {
     return B2GP_OK;
 }
 
-// BNN's likelihood sum_{i,o} log N(y_io; z_io, sigma): two launches on the fused route, the DKL forward / backward pass
-// around bnn_resid_kernel on the layered one.  Both leave sum r^2 in the slot after the parameter gradient.
-extern "C" int b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
-                               const int64_t* widths, int act, const double* params, double sigma, unsigned flags, double* value,
-                               double* grad_sigma, double* grad_params) {
-    if (!ctx) return B2GP_ERR_ARG;
+// the partial rows one fused launch of the BNN likelihood keeps, [draws, nblk, nparams + 1] (doubles, 256 MiB): draws
+// are taken in chunks that stay under it and under grid.y's 65535
+constexpr int64_t BNN_PARTIAL_KEEP = (int64_t)1 << 25;
+
+// BNN's likelihood sum_{i,o} log N(y_io; z_io, sigma_s) for S weight sets (params + s * stride, stride < 0: one packed
+// set) on one X, y.  Fused route: two launches per chunk of draws, the tile kernel on a (nblk, draws) grid and the
+// fixed-order reduction per draw.  Layered route: the DKL forward / backward pass around bnn_resid_kernel per draw.  Both
+// leave [grad params | sum r^2] per draw in one [S, nparams + 1] device array, copied back once; the scalars are
+// finished on the host.  Every argument is checked before any launch.
+static int bnn_loglik_impl(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                           const int64_t* widths, int act, int64_t S, const double* params, int64_t params_stride, const double* sigma,
+                           unsigned flags, double* value, double* grad_sigma, double* grad_params) {
     MlpShape s;
     RET_IF(mlp_shape(ctx, N, D, n_layers, widths, act, s));
-    ARG_CHECK(ctx, X && y && params && value && grad_sigma && n_layers >= 1 && s.d == O && !f32_io(flags));
-    ARG_CHECK(ctx, sigma > 0.0 && std::isfinite(sigma));
+    ARG_CHECK(ctx, X && y && params && sigma && value && grad_sigma && n_layers >= 1 && s.d == O && !f32_io(flags));
+    const int64_t stride = params_stride < 0 ? s.nparams : params_stride;
+    ARG_CHECK(ctx, S >= 1 && stride >= s.nparams);
+    for (int64_t m = 0; m < S; ++m) ARG_CHECK(ctx, sigma[m] > 0.0 && std::isfinite(sigma[m]));
     CUDA_TRY(ctx, cudaSetDevice(ctx->device));
     ctx->fcache.valid = false;
     cudaStream_t st = ctx->slots[0].stream;
@@ -2596,42 +2605,75 @@ extern "C" int b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_
     const double *dX, *dy, *dP;
     RET_IF(stage_in(ctx, st, ctx->mlp[0], X, (size_t)N * D * 8, dev, &dX));
     RET_IF(stage_in(ctx, st, ctx->d_in[1], y, (size_t)N * O * 8, dev, &dy));
-    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)s.nparams * 8, false, &dP));
-    const double inv_s2 = 1.0 / (sigma * sigma);
+    RET_IF(stage_in(ctx, st, ctx->mlp[1], params, (size_t)((S - 1) * stride + s.nparams) * 8, false, &dP));
+    std::vector<double> inv_s2(S);
+    for (int64_t m = 0; m < S; ++m) inv_s2[m] = 1.0 / (sigma[m] * sigma[m]);
+    const int64_t np = s.nparams, ld = np + 1;
+    std::vector<double> sums((size_t)(S * ld));   // [grad params | sum r^2] per draw
+    const double* dsums;
     const size_t smem = ctx->bnn_fused ? bnn_fused_smem(D, n_layers, widths, true, ctx->smem_optin) : 0;
-    const double* sums;   // [grad params | sum r^2] on the device
     if (smem) {
         RET_IF(bnn_optin(ctx));
         int per_sm = 0;
         CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bnn_loglik_tile_kernel, BNN_THREADS, smem));
+        // each draw's grid width is the one-draw width, so its partial rows and their sum do not depend on S
         const int64_t nblk = std::min<int64_t>(ceil_div(N, BNN_ROWS), (int64_t)ctx->sm_count * std::max(per_sm, 1));
-        const int64_t ld = s.nparams + 1;
-        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(nblk + 1) * ld * 8));
+        const int64_t chunk = std::min<int64_t>({S, 65535, std::max<int64_t>(1, BNN_PARTIAL_KEEP / (nblk * ld))});
+        const double* dis;
+        RET_IF(stage_in(ctx, st, ctx->d_in[2], inv_s2.data(), (size_t)S * 8, false, &dis));
+        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(chunk * nblk + S) * ld * 8));
         double* partial = (double*)ctx->mlp[3].p;
-        double* out = partial + nblk * ld;
-        RET_IF(launch(ctx, st, (unsigned)nblk, BNN_THREADS, smem, bnn_loglik_tile_kernel, bnn_net(D, n_layers, widths), act, dX, dy,
-                      N, dP, inv_s2, partial));
-        RET_IF(launch(ctx, st, (unsigned)ceil_div(ld, 256), 256, 0, bnn_reduce_kernel, (const double*)partial, (int)nblk, (int)ld, out));
-        if (grad_params) CUDA_TRY(ctx, cudaMemcpyAsync(grad_params, out, (size_t)s.nparams * 8, cudaMemcpyDeviceToHost, st));
-        sums = out;
+        double* out = partial + chunk * nblk * ld;
+        const BnnNet net = bnn_net(D, n_layers, widths);
+        for (int64_t s0 = 0; s0 < S; s0 += chunk) {
+            const unsigned nc = (unsigned)std::min(chunk, S - s0);
+            RET_IF(launch(ctx, st, dim3((unsigned)nblk, nc), BNN_THREADS, smem, bnn_loglik_tile_kernel, net, act, dX, dy, N, dP, stride,
+                          dis, s0, partial));
+            RET_IF(launch(ctx, st, dim3((unsigned)ceil_div(ld, 256), nc), 256, 0, bnn_reduce_kernel, (const double*)partial, (int)nblk,
+                          (int)ld, out + s0 * ld));
+        }
+        dsums = out;
     } else {
-        std::vector<double*> H;
-        RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dP, H));
         const MlpBack b = mlp_back_layout(s);
-        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(b.tot + 1) * 8));
+        RET_IF(ensure(ctx, ctx->mlp[3], (size_t)(b.tot + S * ld) * 8));
         double* base = (double*)ctx->mlp[3].p;
-        double* r2 = base + b.tot;
-        RET_IF(launch(ctx, st, 1, BNN_THREADS, 0, bnn_resid_kernel, (const double*)H[s.L], dy, N * O, inv_s2, base, r2));
-        if (grad_params) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dP, H, base, grad_params));
-        sums = r2;
+        double* out = base + b.tot;
+        std::vector<double*> H;
+        for (int64_t m = 0; m < S; ++m) {
+            const double* dPm = dP + m * stride;
+            RET_IF(mlp_forward_dev(ctx, st, s, act, dX, dPm, H));
+            RET_IF(launch(ctx, st, 1, BNN_THREADS, 0, bnn_resid_kernel, (const double*)H[s.L], dy, N * O, inv_s2[m], base,
+                          out + m * ld + np));
+            if (grad_params) RET_IF(mlp_backward_dev(ctx, st, s, b, act, dPm, H, base, out + m * ld, true));
+        }
+        dsums = out;
     }
-    double r2sum = 0.0;
-    CUDA_TRY(ctx, cudaMemcpyAsync(&r2sum, sums + (smem ? s.nparams : 0), 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(ctx, cudaMemcpyAsync(sums.data(), dsums, (size_t)(S * ld) * 8, cudaMemcpyDeviceToHost, st));
     RET_IF(tm.end(st, nullptr));
     const double no = (double)N * (double)O;
-    *value = -0.5 * r2sum * inv_s2 - no * (log(sigma) + 0.5 * log(2.0 * 3.141592653589793));
-    *grad_sigma = r2sum * inv_s2 / sigma - no / sigma;
+    for (int64_t m = 0; m < S; ++m) {
+        const double r2sum = sums[m * ld + np], sg = sigma[m];
+        value[m] = -0.5 * r2sum * inv_s2[m] - no * (log(sg) + 0.5 * log(2.0 * 3.141592653589793));
+        grad_sigma[m] = r2sum * inv_s2[m] / sg - no / sg;
+        if (grad_params) memcpy(grad_params + m * np, sums.data() + m * ld, (size_t)np * 8);
+    }
     return B2GP_OK;
+}
+
+extern "C" int b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                               const int64_t* widths, int act, const double* params, double sigma, unsigned flags, double* value,
+                               double* grad_sigma, double* grad_params) {
+    if (!ctx) return B2GP_ERR_ARG;
+    return bnn_loglik_impl(ctx, X, N, D, y, O, n_layers, widths, act, 1, params, -1, &sigma, flags, value, grad_sigma, grad_params);
+}
+
+extern "C" int b2gp_bnn_loglik_draws(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                                     const int64_t* widths, int act, int64_t S, const double* params, int64_t params_stride,
+                                     const double* sigma, unsigned flags, double* value, double* grad_sigma, double* grad_params) {
+    if (!ctx) return B2GP_ERR_ARG;
+    ARG_CHECK(ctx, params_stride >= 0);
+    return bnn_loglik_impl(ctx, X, N, D, y, O, n_layers, widths, act, S, params, params_stride, sigma, flags, value, grad_sigma,
+                           grad_params);
 }
 
 // loc[s] = MLP(X; weight set s) and y_sampled[s] = loc[s] + sigma[s] * mean_k eps[s, k] for S weight sets: one launch on

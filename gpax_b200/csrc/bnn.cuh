@@ -12,7 +12,9 @@
 // gradient = column sum of G, dW_l = H_l^T G, and G <- (G W_l^T) * act'(H_l) written over H_l (each element is read and
 // written by one thread, so in place is safe).  Each gradient element is owned by one thread and accumulated in tile
 // order; sum r^2 per thread, then a fixed tree.  The CTA writes one partial row [grad params | sum r^2].
-// bnn_reduce_kernel sums the rows in CTA order: no atomics, identical calls give identical bits.
+// bnn_reduce_kernel sums the rows in CTA order: no atomics, identical calls give identical bits.  Both kernels have a draw
+// axis (grid.y, b2gp_bnn_loglik_draws): CTA (c, j) runs weight set s0 + j with its own 1 / sigma^2 over the same tiles a
+// one-draw launch gives CTA c, so every draw gets the bits of its own b2gp_bnn_loglik call.
 //
 // bnn_predict_kernel: grid (row tiles, draws s0 .. s0 + gridDim.y - 1; more than 65535 draws take several launches).
 // CTA (t, s) stages weight set s, runs the forward pass on its tile and writes
@@ -142,15 +144,22 @@ static __device__ void bnn_stage_x(const BnnNet& net, const double* __restrict__
     }
 }
 
+// grid (row-tile CTAs, draws s0 .. s0 + gridDim.y - 1): CTA (c, j) stages weight set s = s0 + j (P + s * stride) with
+// 1 / sigma_s^2 = inv_s2[s] and writes partial row j * gridDim.x + c.  Every draw sees the grid width and tile order of a
+// one-draw launch, so its partial rows do not depend on how many draws share the launch.
 __global__ void __launch_bounds__(BNN_THREADS)
 bnn_loglik_tile_kernel(const BnnNet net, int act, const double* __restrict__ X, const double* __restrict__ y, int64_t N,
-                       const double* __restrict__ P, double inv_s2, double* __restrict__ partial) {
+                       const double* __restrict__ P, int64_t stride, const double* __restrict__ inv_s2v, int64_t s0,
+                       double* __restrict__ partial) {
     extern __shared__ double sm[];
     __shared__ double red[BNN_THREADS];
     double* Ws = sm;
     double* gs = sm + net.nparams;
     double* H = gs + net.nparams;
     const int np = net.nparams, O = net.dims[net.L];
+    const int64_t s = s0 + blockIdx.y;
+    const double inv_s2 = inv_s2v[s];
+    P += s * stride;
     for (int i = threadIdx.x; i < np; i += BNN_THREADS) {
         Ws[i] = P[i];
         gs[i] = 0.0;
@@ -204,18 +213,19 @@ bnn_loglik_tile_kernel(const BnnNet net, int act, const double* __restrict__ X, 
         if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
         __syncthreads();
     }
-    double* row = partial + (int64_t)blockIdx.x * (np + 1);
+    double* row = partial + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * (np + 1);
     for (int i = threadIdx.x; i < np; i += BNN_THREADS) row[i] = gs[i];
     if (threadIdx.x == 0) row[np] = red[0];
 }
 
-// out[p] = sum_c partial[c, p] over the rows in order
+// out[j, p] = sum_c partial[j, c, p] over the nrows rows of draw j (blockIdx.y) in order
 __global__ void bnn_reduce_kernel(const double* __restrict__ partial, int nrows, int ld, double* __restrict__ out) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= ld) return;
+    partial += (int64_t)blockIdx.y * nrows * ld;
     double s = 0.0;
     for (int c = 0; c < nrows; ++c) s += partial[(int64_t)c * ld + p];
-    out[p] = s;
+    out[(int64_t)blockIdx.y * ld + p] = s;
 }
 
 // loc and y_sampled of one (row, output) element of draw s: the epilogue both predict routes share

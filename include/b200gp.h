@@ -510,6 +510,17 @@ int  b2gp_mtdkl_mll(b2gp_ctx* ctx, int kind, const double* X, const int* task, i
 int  b2gp_bnn_loglik(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
                      const int64_t* widths, int act, const double* params, double sigma, unsigned flags, double* value,
                      double* grad_sigma, double* grad_params);
+
+/* b2gp_bnn_loglik_draws: b2gp_bnn_loglik for S >= 1 weight sets on one X and y -- the likelihoods of S NUTS chains in one
+ *   call.  Draw s takes params + s * params_stride (params_stride >= nparams) and sigma[s] (> 0, finite) and writes
+ *   value[s], grad_sigma[s] and, when grad_params is given, grad_params[s * nparams ..] ([S, nparams]): bit for bit what
+ *   b2gp_bnn_loglik returns for that weight set on the same route and options, whatever S is.  X, y follow `flags` as in
+ *   b2gp_bnn_loglik; params, sigma, widths and the outputs are HOST pointers.  Every argument is checked before any launch.
+ *   Fused route: two launches per chunk of draws (at most 65535 draws, and a 256 MiB cap on the per-CTA partial rows);
+ *   layered route: b2gp_bnn_loglik's sequence per draw.  One copy back and one synchronise per call.               */
+int  b2gp_bnn_loglik_draws(b2gp_ctx* ctx, const double* X, int64_t N, int64_t D, const double* y, int64_t O, int n_layers,
+                           const int64_t* widths, int act, int64_t S, const double* params, int64_t params_stride,
+                           const double* sigma, unsigned flags, double* value, double* grad_sigma, double* grad_params);
 int  b2gp_bnn_predict(b2gp_ctx* ctx, const double* X, int64_t P, int64_t D, int n_layers, const int64_t* widths, int act,
                       const double* params, int64_t S, int64_t params_stride, int64_t O, const double* sigma,
                       const double* eps, int64_t n, double* loc, double* y_sampled, unsigned flags);
